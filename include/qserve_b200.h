@@ -202,6 +202,32 @@ QS_API int qs_single_query_attention_quant(const void* q, const void* k, const v
 QS_API int qs_argmax_rows(int64_t* out, const void* logits, int rows, int vocab, void* stream);
 QS_API int qs_silu_and_mul_quant(int8_t* out, const void* input, void* input_sum, void* scale, int tokens, int d, void* stream);
 
+/* Prompt chunks over a cached prefix (chunked prefill, prefix reuse, continuing a conversation).
+ *
+ * qs_apply_bias_rope_update_kv_cache_at: qs_apply_bias_rope_update_kv_cache for a batch of chunks that continue sequences whose first
+ *   start_pos[b] tokens (int32 [batch], device) are already in the pages; seq_lens are the CHUNK lengths.  Token pos of chunk b is rotated at
+ *   position start_pos[b] + pos and stored in that position's page and slot; the cyclic window uses the total length start_pos[b] + seq_lens[b].
+ *   Appending a prompt in several chunks leaves the same bytes in the pages and in the rotated q / k as appending it in one call.      */
+QS_API int qs_apply_bias_rope_update_kv_cache_at(void* qkv, const int32_t* seq_lens, const int32_t* padding_offset, const int32_t* start_pos,
+                                                 const int64_t* kv_pointers, int batch, int num_tokens, int max_blocks_per_seq, int head_num,
+                                                 int kv_head_num, int head_dim, int seq_len, int tokens_per_block, int size_per_token,
+                                                 int rotary_embedding_dim, float rotary_embedding_base, int rotary_embedding_max_positions,
+                                                 int neox_rotary_style, int int4_kv_cache, int kv_cache_with_zeros, void* stream);
+/* qs_prefix_prefill_attention: causal attention of a batch of chunks.  q [T,Hq,128], k / v [T,Hkv,128] fp16: the chunk rows, strided views of
+ *   the qkv buffer qs_apply_bias_rope_update_kv_cache_at has rotated (row strides in halfs, multiples of 8); cu_seqlens int32 [batch+1] chunk
+ *   offsets; prefix_lens int32 [batch] cached tokens per sequence; kv_pointers int64 [batch,2,max_blocks_per_seq] as for
+ *   qs_single_query_attention; out fp16 [T,Hq,128].  Query i of sequence b (position prefix_lens[b] + i) attends to the prefix keys
+ *   0 .. prefix_lens[b]-1, dequantised from the ZINT4 / ZINT8 pages exactly as the reference dequantises them, and to the chunk keys 0 .. i as
+ *   the un-quantised fp16 k / v.  GQA by Hq / Hkv, head_dim 128, tokens_per_block 64, fp32 softmax, P rounded to fp16 before the PV product;
+ *   wgmma, sm_90a only; deterministic.  max_prefix_len is a host bound (like flash-attn's max_seqlen_k): the call checks
+ *   max_prefix_len + max_seqlen <= max_blocks_per_seq * 64, and the kernel TRUSTS prefix_lens[b] <= max_prefix_len.  prefix_lens and the page
+ *   table are read before the PDL dependency wait (see qs_set_pdl), the page contents after it.                                          */
+QS_API int qs_prefix_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
+                                       int64_t out_stride, const int32_t* cu_seqlens, const int32_t* prefix_lens, const int64_t* kv_pointers,
+                                       int batch, int num_tokens, int max_seqlen, int max_prefix_len, int max_blocks_per_seq, int num_heads,
+                                       int num_kv_heads, int head_dim, int tokens_per_block, int size_per_token, int int4_kv_cache,
+                                       float softmax_scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

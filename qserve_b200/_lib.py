@@ -32,6 +32,8 @@ SIGNATURES = {
     "qs_apply_bias_rope_update_kv_cache": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _I, _I, _I, _I, _P]),
     "qs_compute_padding_offsets": (c_int, [_P, _P, _I, _I, _P]),
     "qs_prefill_attention": (c_int, [_P, _P, _P, _L, _L, _L, _P, _L, _P, _I, _I, _I, _I, _I, _I, _F, _P]),
+    "qs_apply_bias_rope_update_kv_cache_at": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _I, _I, _I, _I, _P]),
+    "qs_prefix_prefill_attention": (c_int, [_P, _P, _P, _L, _L, _L, _P, _L, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
     "qs_rms_norm": (c_int, [_P, _P, _P, _F, _I, _I, _I, _P]),
     "qs_rms_norm_general": (c_int, [_P, _P, _P, _P, _F, _I, _I, _I, _P]),
     "qs_rms_norm_general_fuse_sum": (c_int, [_P, _P, _P, _P, _P, _F, _I, _I, _I, _P]),

@@ -444,6 +444,68 @@ def single_query_attention_quant(q, k, v, kv_pointers, length_per_sample, memory
                                               ws.data_ptr(), ws.numel())
 
 
+def apply_bias_rope_update_kv_cache_at(qkv, seq_lens, padding_offset, start_pos, kv_pointers: Optional[torch.Tensor], head_num: int,
+                                       kv_head_num: int, seq_len: int, tokens_per_block: int, size_per_token: int, rotary_embedding_dim: int,
+                                       rotary_embedding_base: float, rotary_embedding_max_positions: int, neox_rotary_style: bool,
+                                       int4_kv_cache: bool, kv_cache_with_zeros: bool) -> None:
+    """apply_bias_rope_update_kv_cache for prompt CHUNKS that continue sequences whose first start_pos[b] tokens (int32 [B], device) are
+    already cached: seq_lens are the chunk lengths, token pos of chunk b is rotated at position start_pos[b] + pos and appended there.
+    Appending a prompt in chunks leaves the same bytes as one apply_bias_rope_update_kv_cache call over the whole prompt."""
+    for t, n in ((qkv, "qkv"), (seq_lens, "seq_lens"), (padding_offset, "padding_offset"), (start_pos, "start_pos")):
+        _cuda(t, n)
+    _require(qkv.dtype == _HALF and qkv.is_contiguous(), "qkv must be contiguous float16")
+    _require(seq_lens.dtype == torch.int32 and padding_offset.dtype == torch.int32, "seq_lens and padding_offset must be int32")
+    _require(start_pos.dtype == torch.int32 and start_pos.is_contiguous() and tuple(start_pos.shape) == (seq_lens.size(0),),
+             "start_pos must be contiguous int32 [batch]")
+    head_dim = int(rotary_embedding_dim)
+    _require(head_dim == 128, "apply_bias_rope_update_kv_cache_at: head_dim must be 128")
+    _require(qkv.size(-1) == (head_num + 2 * kv_head_num) * head_dim, "qkv width does not match (head_num + 2*kv_head_num) * head_dim")
+    kvp, max_blocks = None, 0
+    if kv_pointers is not None:
+        _cuda(kv_pointers, "kv_pointers")
+        _require(kv_pointers.is_contiguous() and kv_pointers.dtype == torch.int64, "kv_pointers must be contiguous int64")
+        kvp, max_blocks = kv_pointers.data_ptr(), kv_pointers.size(-1)
+    _call(qkv, lib.qs_apply_bias_rope_update_kv_cache_at, qkv.data_ptr(), seq_lens.data_ptr(), padding_offset.data_ptr(), start_pos.data_ptr(), kvp,
+          seq_lens.size(0), qkv.size(0), max_blocks, int(head_num), int(kv_head_num), head_dim, int(seq_len), int(tokens_per_block),
+          int(size_per_token), int(rotary_embedding_dim), float(rotary_embedding_base), int(rotary_embedding_max_positions),
+          int(bool(neox_rotary_style)), int(bool(int4_kv_cache)), int(bool(kv_cache_with_zeros)))
+
+
+def prefix_prefill_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, max_prefix_len: int, kv_pointers, tokens_per_block: int,
+                             size_per_token: int, int4_kv_cache: bool, softmax_scale: Optional[float] = None) -> torch.Tensor:
+    """Causal attention of a batch of prompt chunks over their cached prefix.  q [T,Hq,128], k / v [T,Hkv,128] fp16 (strided views of the qkv
+    buffer apply_bias_rope_update_kv_cache_at has rotated), cu_seqlens int32 [B+1] chunk offsets, prefix_lens int32 [B] cached tokens,
+    kv_pointers int64 [B,2,max_blocks] page addresses (the block table covers the prefix and the chunk).  Query i of sequence b attends to the
+    prefix keys dequantised from the ZINT4 / ZINT8 pages and to chunk keys 0..i in fp16.  max_prefix_len bounds prefix_lens (it is not checked
+    on the device).  Returns fp16 [T,Hq,128]."""
+    for t, n in ((q, "q"), (k, "k"), (v, "v"), (cu_seqlens, "cu_seqlens"), (prefix_lens, "prefix_lens"), (kv_pointers, "kv_pointers")):
+        _cuda(t, n)
+    _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
+    _require(q.dim() == 3 and k.dim() == 3 and v.dim() == 3 and q.size(2) == 128 and k.size(2) == 128 and v.size(2) == 128, "q, k, v must be [T, H, 128]")
+    _require(k.shape == v.shape and q.size(0) == k.size(0), "q, k, v must cover the same tokens; k and v the same heads")
+    for t, name in ((q, "q"), (k, "k"), (v, "v")):
+        _require(t.stride(2) == 1 and t.stride(1) == 128, f"{name}: heads must be contiguous rows of 128 halfs")
+    _require(cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous() and cu_seqlens.dim() == 1, "cu_seqlens must be contiguous int32")
+    batch = cu_seqlens.size(0) - 1
+    _require(prefix_lens.dtype == torch.int32 and prefix_lens.is_contiguous() and tuple(prefix_lens.shape) == (batch,), "prefix_lens must be contiguous int32 [batch]")
+    _require(kv_pointers.dtype == torch.int64 and kv_pointers.is_contiguous() and kv_pointers.dim() == 3 and kv_pointers.size(0) == batch
+             and kv_pointers.size(1) == 2, "kv_pointers must be contiguous int64 [batch, 2, max_blocks]")
+    _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
+    T, hq, hkv = q.size(0), q.size(1), k.size(1)
+    _require(hq % hkv == 0, "num_heads must be a multiple of num_kv_heads")
+    _require(int(size_per_token) == hkv * 128 * (4 if int4_kv_cache else 8) // 8, "size_per_token does not match the kv heads and the cache type")
+    _require(int(max_prefix_len) >= 0 and int(max_seqlen) >= 0, "negative max_prefix_len / max_seqlen")
+    _require(int(max_prefix_len) + int(max_seqlen) <= kv_pointers.size(-1) * 64, "the page table is too short for max_prefix_len + max_seqlen")
+    out = torch.empty((T, hq, 128), dtype=_HALF, device=q.device)
+    if T == 0 or batch == 0:
+        return out
+    scale = float(softmax_scale) if softmax_scale is not None else 128 ** -0.5
+    _call(q, lib.qs_prefix_prefill_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), out.data_ptr(), out.stride(0),
+          cu_seqlens.data_ptr(), prefix_lens.data_ptr(), kv_pointers.data_ptr(), batch, T, int(max_seqlen), int(max_prefix_len), kv_pointers.size(-1),
+          hq, hkv, 128, int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), scale)
+    return out
+
+
 class PeerContext:
     """Peer-mapped buffers of a tensor-parallel group for the fused all-reduce (qs_add_rms_norm_general_peer): built once from
     torch.distributed._symmetric_memory (device memory + NVLink peer mappings are torch's plumbing; the kernel is ours).

@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libqserve_b200.so")
-SOURCES = ["capi.cu", "gemm.cu", "attention.cu", "prefill_attention.cu", "elementwise.cu"]
+SOURCES = ["capi.cu", "gemm.cu", "attention.cu", "prefill_attention.cu", "prefix_attention.cu", "elementwise.cu"]
 HEADERS = ["common.cuh", "launch.h", os.path.join("..", "..", "include", "qserve_b200.h")]
 
 NVCC_FLAGS = [

@@ -753,10 +753,10 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
 //     powf / sincosf per token: 365 us per layer for the 8 x 1024-token prompt batch), then quantises and appends K and V.
 //     applyBiasRopeUpdateKVCache.h:94-455 (STORE_QKV = true, no bias, NeoX)
 // ------------------------------------------------------------------------------------------------
-template <int BITS>
+template <int BITS, bool AT>  // AT: start_pos is given (qs_apply_bias_rope_update_kv_cache_at); otherwise it is ignored
 __global__ void __launch_bounds__(128) prefill_append_kernel(__half* __restrict__ qkv, const int* __restrict__ seq_lens,
                                                              const int* __restrict__ padding_offset, const long long* __restrict__ kv_pointers,
-                                                             int num_tokens, int max_blocks, int num_heads, int num_kv_heads, int seq_len,
+                                                             const int* __restrict__ start_pos, int num_tokens, int max_blocks, int num_heads, int num_kv_heads, int seq_len,
                                                              PageGeom pg, float rotary_base, int rotary_dim, int max_positions) {
   if (threadIdx.x == 0) pdl_launch_dependents();
   pdl_wait();
@@ -770,9 +770,13 @@ __global__ void __launch_bounds__(128) prefill_append_kernel(__half* __restrict_
        wi += static_cast<long long>(gridDim.x) * warps_per_cta) {
     const int token = static_cast<int>(wi / num_kv_heads), kvh = static_cast<int>(wi - static_cast<long long>(token) * num_kv_heads);
     const int gtok = token + (padding_offset ? padding_offset[token] : 0);
-    const int bidx = gtok / seq_len, pos = gtok - bidx * seq_len;
-    const int len = seq_lens[bidx];
-    if (pos >= len) continue;  // padded slot (cannot happen with un-padded inputs)
+    const int bidx = gtok / seq_len, cpos = gtok - bidx * seq_len;
+    const int clen = seq_lens[bidx];
+    if (cpos >= clen) continue;  // padded slot (cannot happen with un-padded inputs)
+    // with start_pos (a chunk appended behind start_pos[b] cached tokens) the position and the total length are shifted; the RoPE angle, the
+    // page / slot and the cyclic window all use the shifted values, so appending a prompt in chunks gives the bytes of a one-shot append
+    const int start = AT ? __ldg(start_pos + bidx) : 0;
+    const int pos = start + cpos, len = start + clen;
     __half* trow = qkv + static_cast<size_t>(token) * n;
     // lane handles rotary pairs i = 2*lane, 2*lane+1  (i in [0, 64)) -> dims i and i + half_rot: one half2 at each end
     float cs[2], sn[2];
@@ -979,10 +983,11 @@ int prefill_rope_append(const PrefillAppendArgs& a) {
   if (blocks > static_cast<long long>(num_sms()) * 16) blocks = static_cast<long long>(num_sms()) * 16;
   auto run = [&](auto kern) {
     return launch_pdl(kern, dim3(static_cast<unsigned>(blocks)), dim3(128), 0, a.stream, "apply_bias_rope_update_kv_cache", static_cast<__half*>(a.qkv),
-                      a.seq_lens, a.padding_offset, a.kv_pointers, a.num_tokens, a.max_blocks, a.num_heads, a.num_kv_heads, a.seq_len, pg,
+                      a.seq_lens, a.padding_offset, a.kv_pointers, a.start_pos, a.num_tokens, a.max_blocks, a.num_heads, a.num_kv_heads, a.seq_len, pg,
                       a.rotary_base, a.rotary_dim, a.max_positions);
   };
-  return a.int4_kv ? run(prefill_append_kernel<4>) : run(prefill_append_kernel<8>);
+  if (a.start_pos) return a.int4_kv ? run(prefill_append_kernel<4, true>) : run(prefill_append_kernel<8, true>);
+  return a.int4_kv ? run(prefill_append_kernel<4, false>) : run(prefill_append_kernel<8, false>);
 }
 
 int padding_offsets(int* out, const int* cu_seqlens, int batch, int max_seqlen, void* stream) {

@@ -169,6 +169,36 @@ int qs_apply_bias_rope_update_kv_cache(void* qkv, const int32_t* seq_lens, const
   return prefill_rope_append(a);
 }
 
+int qs_apply_bias_rope_update_kv_cache_at(void* qkv, const int32_t* seq_lens, const int32_t* padding_offset, const int32_t* start_pos,
+                                          const int64_t* kv_pointers, int batch, int num_tokens, int max_blocks_per_seq, int head_num, int kv_head_num,
+                                          int head_dim, int seq_len, int tokens_per_block, int size_per_token, int rotary_embedding_dim,
+                                          float rotary_embedding_base, int rotary_embedding_max_positions, int neox_rotary_style, int int4_kv_cache,
+                                          int kv_cache_with_zeros, void* stream) {
+  (void)neox_rotary_style;
+  QS_REQUIRE(qkv && seq_lens && start_pos, "apply_bias_rope_update_kv_cache_at: null tensor");
+  PrefillAppendArgs a;
+  a.qkv = qkv; a.seq_lens = seq_lens; a.padding_offset = padding_offset; a.start_pos = start_pos;
+  a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
+  a.batch = batch; a.num_tokens = num_tokens; a.max_blocks = max_blocks_per_seq; a.num_heads = head_num; a.num_kv_heads = kv_head_num;
+  a.head_dim = head_dim; a.seq_len = seq_len; a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token;
+  a.rotary_dim = rotary_embedding_dim; a.rotary_base = rotary_embedding_base; a.max_positions = rotary_embedding_max_positions;
+  a.int4_kv = int4_kv_cache; a.kv_zeros = kv_cache_with_zeros; a.stream = stream;
+  return prefill_rope_append(a);
+}
+
+int qs_prefix_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
+                                int64_t out_stride, const int32_t* cu_seqlens, const int32_t* prefix_lens, const int64_t* kv_pointers, int batch,
+                                int num_tokens, int max_seqlen, int max_prefix_len, int max_blocks_per_seq, int num_heads, int num_kv_heads, int head_dim,
+                                int tokens_per_block, int size_per_token, int int4_kv_cache, float softmax_scale, void* stream) {
+  PrefixAttnArgs a;
+  a.q = q; a.k = k; a.v = v; a.out = out; a.q_stride = q_stride; a.k_stride = k_stride; a.v_stride = v_stride; a.out_stride = out_stride;
+  a.cu_seqlens = cu_seqlens; a.prefix_lens = prefix_lens; a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
+  a.batch = batch; a.num_tokens = num_tokens; a.max_seqlen = max_seqlen; a.max_prefix_len = max_prefix_len; a.max_blocks = max_blocks_per_seq;
+  a.num_heads = num_heads; a.num_kv_heads = num_kv_heads; a.head_dim = head_dim; a.tokens_per_block = tokens_per_block;
+  a.size_per_token = size_per_token; a.int4_kv = int4_kv_cache; a.softmax_scale = softmax_scale; a.stream = stream;
+  return prefix_attention(a);
+}
+
 int qs_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
                          int64_t out_stride, const int32_t* cu_seqlens, int batch, int num_tokens, int max_seqlen, int num_heads, int num_kv_heads,
                          int head_dim, float softmax_scale, void* stream) {

@@ -28,6 +28,10 @@ int check_cuda(cudaError_t e, const char* what);
     if (!(cond)) return ::qs::set_error(::qs::QS_ERR_INVALID, __VA_ARGS__); \
   } while (0)
 
+// TMA descriptor of an fp16 [rows, cols] matrix with a row pitch of `stride` elements, box = 64 columns (128 B, 128-byte swizzle) x 128 rows
+// (prefill_attention.cu; shared by the prompt-attention kernels)
+int make_tmap_f16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t stride);
+
 // ---------------------------------------------------------------------------------------------
 // small utilities
 // ---------------------------------------------------------------------------------------------

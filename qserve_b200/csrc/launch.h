@@ -93,6 +93,7 @@ struct PrefillAppendArgs {
   const int* seq_lens = nullptr;
   const int* padding_offset = nullptr;
   const long long* kv_pointers = nullptr;  // may be null: rotate only
+  const int* start_pos = nullptr;          // optional [batch]: tokens of each sequence already cached; token pos sits at start_pos[b] + pos
   int batch = 0, num_tokens = 0, max_blocks = 0, num_heads = 0, num_kv_heads = 0, head_dim = 0;
   int seq_len = 0, tokens_per_block = 64, size_per_token = 0, rotary_dim = 0, max_positions = 0;
   float rotary_base = 10000.f;
@@ -115,5 +116,24 @@ struct PrefillAttnArgs {
   void* stream = nullptr;
 };
 int prefill_attention(const PrefillAttnArgs& a);
+
+// prefix_attention.cu: causal attention of a batch of prompt chunks over their cached prefix (dequantised from the INT4 / INT8 pages) and
+// over the chunk itself (fp16 q / k / v)
+struct PrefixAttnArgs {
+  const void* q = nullptr;    // fp16 [T, Hq, 128] chunk rows, rows of q_stride halfs
+  const void* k = nullptr;    // fp16 [T, Hkv, 128]
+  const void* v = nullptr;
+  void* out = nullptr;        // fp16 [T, Hq, 128], rows of out_stride halfs
+  long long q_stride = 0, k_stride = 0, v_stride = 0, out_stride = 0;
+  const int* cu_seqlens = nullptr;         // [batch + 1] chunk token offsets
+  const int* prefix_lens = nullptr;        // [batch] tokens already in the cache (<= max_prefix_len)
+  const long long* kv_pointers = nullptr;  // [batch, 2, max_blocks] absolute page addresses
+  int batch = 0, num_tokens = 0, max_seqlen = 0, max_prefix_len = 0, max_blocks = 0;
+  int num_heads = 0, num_kv_heads = 0, head_dim = 0, tokens_per_block = 64, size_per_token = 0;
+  int int4_kv = 1;
+  float softmax_scale = 0.f;
+  void* stream = nullptr;
+};
+int prefix_attention(const PrefixAttnArgs& a);
 
 }  // namespace qs

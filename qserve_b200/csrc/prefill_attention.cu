@@ -228,9 +228,12 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
   }
 }
 
+}  // namespace
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
+namespace {
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
@@ -244,6 +247,7 @@ PFN_encodeTiled get_encode() {
   });
   return fn;
 }
+}  // namespace
 
 // fp16 [rows, cols] with a row pitch of `stride` elements; box = 64 columns (128 B, swizzled) x 128 rows
 int make_tmap_f16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t stride) {
@@ -260,8 +264,6 @@ int make_tmap_f16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols,
                      (unsigned long long)cols, (unsigned long long)stride);
   return QS_OK;
 }
-
-}  // namespace
 
 int prefill_attention(const PrefillAttnArgs& a) {
   QS_REQUIRE(a.head_dim == kD, "prefill_attention: head_dim=%d (only 128 is built, as in the reference)", a.head_dim);
