@@ -228,6 +228,28 @@ QS_API int qs_prefix_prefill_attention(const void* q, const void* k, const void*
                                        int num_kv_heads, int head_dim, int tokens_per_block, int size_per_token, int int4_kv_cache,
                                        float softmax_scale, void* stream);
 
+/* Multi-token decode attention (speculative-decoding verification): n_b = cu_seqlens[b+1] - cu_seqlens[b] <= 16 draft tokens per sequence,
+ * rotated and appended at positions prefix_lens[b] .. prefix_lens[b] + n_b - 1 by qs_apply_bias_rope_update_kv_cache_at (start_pos =
+ * prefix_lens).  Arguments as for qs_prefix_prefill_attention.  Query token i of sequence b is computed as the decode step
+ * qs_single_query_attention would compute it at that position: it attends to the cache positions 0 .. prefix_lens[b] + i - 1 dequantised from
+ * the ZINT4 / ZINT8 pages (the earlier draft tokens of the step included, read back quantised) and to its own key and value as the un-quantised
+ * fp16 rows of k / v; its own cache slot is not read.  A greedy verify therefore reproduces the numbers of sequential decoding up to the fp32
+ * summation order.  (qs_prefix_prefill_attention instead uses every chunk key un-quantised.)  softmax_scale <= 0 selects 1/sqrt(128) as the
+ * decode kernel computes it.  Restrictions: fp16, head_dim 128, tokens_per_block 64, 1 <= max_seqlen <= 16, max_prefix_len + max_seqlen <=
+ * max_blocks_per_seq * 64; n_b = 0 and prefix_lens[b] = 0 are allowed; the kernel TRUSTS prefix_lens[b] <= max_prefix_len.  The page slots
+ * from prefix_lens[b] + n_b - 1 on are never read.  workspace: at least qs_multi_token_attention_workspace_bytes(batch, num_tokens,
+ * max_seqlen, max_prefix_len, num_heads, num_kv_heads, int4_kv_cache) bytes, zero-filled once and then owned by the library (its split counters clean
+ * themselves up, so the call is CUDA-graph capturable and bitwise deterministic).  cu_seqlens, prefix_lens and the page table are read
+ * before the PDL dependency wait, q / k / v and the page contents after it.                                                               */
+QS_API int qs_multi_token_decode_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride,
+                                           void* out, int64_t out_stride, const int32_t* cu_seqlens, const int32_t* prefix_lens,
+                                           const int64_t* kv_pointers, int batch, int num_tokens, int max_seqlen, int max_prefix_len,
+                                           int max_blocks_per_seq, int num_heads, int num_kv_heads, int head_dim, int tokens_per_block,
+                                           int size_per_token, int int4_kv_cache, float softmax_scale, void* workspace, size_t workspace_bytes,
+                                           void* stream);
+QS_API size_t qs_multi_token_attention_workspace_bytes(int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads,
+                                                       int num_kv_heads, int int4_kv_cache);
+
 #ifdef __cplusplus
 }
 #endif

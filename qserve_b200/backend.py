@@ -477,7 +477,8 @@ def prefix_prefill_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, 
     buffer apply_bias_rope_update_kv_cache_at has rotated), cu_seqlens int32 [B+1] chunk offsets, prefix_lens int32 [B] cached tokens,
     kv_pointers int64 [B,2,max_blocks] page addresses (the block table covers the prefix and the chunk).  Query i of sequence b attends to the
     prefix keys dequantised from the ZINT4 / ZINT8 pages and to chunk keys 0..i in fp16.  max_prefix_len bounds prefix_lens (it is not checked
-    on the device).  Returns fp16 [T,Hq,128]."""
+    on the device).  Returns fp16 [T,Hq,128].  Every chunk key is used un-quantised: this is prompt attention, not n decode steps (for those,
+    e.g. speculative-decoding verification, use multi_token_decode_attention, which reads the earlier chunk tokens back from the pages)."""
     for t, n in ((q, "q"), (k, "k"), (v, "v"), (cu_seqlens, "cu_seqlens"), (prefix_lens, "prefix_lens"), (kv_pointers, "kv_pointers")):
         _cuda(t, n)
     _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
@@ -503,6 +504,63 @@ def prefix_prefill_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, 
     _call(q, lib.qs_prefix_prefill_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), out.data_ptr(), out.stride(0),
           cu_seqlens.data_ptr(), prefix_lens.data_ptr(), kv_pointers.data_ptr(), batch, T, int(max_seqlen), int(max_prefix_len), kv_pointers.size(-1),
           hq, hkv, 128, int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), scale)
+    return out
+
+
+def multi_token_workspace(device: torch.device, batch: int, num_tokens: int, max_seqlen: int, max_prefix_len: int, num_heads: int,
+                          num_kv_heads: int, int4_kv_cache: bool) -> torch.Tensor:
+    """Zero-initialised workspace of multi_token_decode_attention, grown on demand and never freed once handed out (as attention_workspace)."""
+    key = ("mtok", device.index)
+    need = max(1, lib.qs_multi_token_attention_workspace_bytes(batch, num_tokens, max_seqlen, max_prefix_len, num_heads, num_kv_heads,
+                                                                           int(bool(int4_kv_cache))))
+    ws = _workspaces.get(key)
+    if ws is None or ws.numel() < need:
+        if ws is not None:
+            _retired.append(ws)
+        with torch.cuda.device(device):
+            ws = torch.zeros(need, dtype=torch.uint8, device=device)
+        _workspaces[key] = ws
+    return ws
+
+
+def multi_token_decode_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, max_prefix_len: int, kv_pointers, tokens_per_block: int,
+                                 size_per_token: int, int4_kv_cache: bool, softmax_scale: Optional[float] = None) -> torch.Tensor:
+    """Decode attention of n_b <= 16 draft tokens per sequence in one launch (speculative-decoding verification).  Arguments as for
+    prefix_prefill_attention: q [T,Hq,128], k / v [T,Hkv,128] fp16, the draft rows apply_bias_rope_update_kv_cache_at has rotated and appended
+    at positions prefix_lens[b] .. prefix_lens[b] + n_b - 1; cu_seqlens int32 [B+1]; prefix_lens int32 [B]; kv_pointers int64 [B,2,max_blocks].
+
+    Query token i of sequence b is computed as single_query_attention computes that decode step: it attends to the cache positions
+    0 .. prefix_lens[b] + i - 1 dequantised from the ZINT4 / ZINT8 pages (the earlier draft tokens included, read back quantised) and to its own
+    key and value un-quantised.  So a greedy verify gives the numbers of n sequential decode steps up to the fp32 summation order.  This differs
+    from prefix_prefill_attention, which uses every chunk key un-quantised.  1 <= max_seqlen <= 16; max_prefix_len bounds prefix_lens (it is
+    not checked on the device).  The default softmax scale is the decode kernel's 1/sqrt(128).  Returns fp16 [T,Hq,128]."""
+    for t, n in ((q, "q"), (k, "k"), (v, "v"), (cu_seqlens, "cu_seqlens"), (prefix_lens, "prefix_lens"), (kv_pointers, "kv_pointers")):
+        _cuda(t, n)
+    _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
+    _require(q.dim() == 3 and k.dim() == 3 and v.dim() == 3 and q.size(2) == 128 and k.size(2) == 128 and v.size(2) == 128, "q, k, v must be [T, H, 128]")
+    _require(k.shape == v.shape and q.size(0) == k.size(0), "q, k, v must cover the same tokens; k and v the same heads")
+    for t, name in ((q, "q"), (k, "k"), (v, "v")):
+        _require(t.stride(2) == 1 and t.stride(1) == 128, f"{name}: heads must be contiguous rows of 128 halfs")
+    _require(cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous() and cu_seqlens.dim() == 1, "cu_seqlens must be contiguous int32")
+    batch = cu_seqlens.size(0) - 1
+    _require(prefix_lens.dtype == torch.int32 and prefix_lens.is_contiguous() and tuple(prefix_lens.shape) == (batch,), "prefix_lens must be contiguous int32 [batch]")
+    _require(kv_pointers.dtype == torch.int64 and kv_pointers.is_contiguous() and kv_pointers.dim() == 3 and kv_pointers.size(0) == batch
+             and kv_pointers.size(1) == 2, "kv_pointers must be contiguous int64 [batch, 2, max_blocks]")
+    _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
+    T, hq, hkv = q.size(0), q.size(1), k.size(1)
+    _require(hq % hkv == 0, "num_heads must be a multiple of num_kv_heads")
+    _require(int(size_per_token) == hkv * 128 * (4 if int4_kv_cache else 8) // 8, "size_per_token does not match the kv heads and the cache type")
+    _require(1 <= int(max_seqlen) <= 16, "max_seqlen must be 1 .. 16 draft tokens")
+    _require(int(max_prefix_len) >= 0, "negative max_prefix_len")
+    _require(int(max_prefix_len) + int(max_seqlen) <= kv_pointers.size(-1) * 64, "the page table is too short for max_prefix_len + max_seqlen")
+    out = torch.empty((T, hq, 128), dtype=_HALF, device=q.device)
+    if T == 0 or batch == 0:
+        return out
+    ws = multi_token_workspace(q.device, batch, T, int(max_seqlen), int(max_prefix_len), hq, hkv, int4_kv_cache)
+    scale = float(softmax_scale) if softmax_scale is not None else 0.0
+    _call(q, lib.qs_multi_token_decode_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), out.data_ptr(),
+          out.stride(0), cu_seqlens.data_ptr(), prefix_lens.data_ptr(), kv_pointers.data_ptr(), batch, T, int(max_seqlen), int(max_prefix_len),
+          kv_pointers.size(-1), hq, hkv, 128, int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), scale, ws.data_ptr(), ws.numel())
     return out
 
 

@@ -199,6 +199,25 @@ int qs_prefix_prefill_attention(const void* q, const void* k, const void* v, int
   return prefix_attention(a);
 }
 
+int qs_multi_token_decode_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
+                                    int64_t out_stride, const int32_t* cu_seqlens, const int32_t* prefix_lens, const int64_t* kv_pointers, int batch,
+                                    int num_tokens, int max_seqlen, int max_prefix_len, int max_blocks_per_seq, int num_heads, int num_kv_heads,
+                                    int head_dim, int tokens_per_block, int size_per_token, int int4_kv_cache, float softmax_scale, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  MultiTokenAttnArgs a;
+  a.q = q; a.k = k; a.v = v; a.out = out; a.q_stride = q_stride; a.k_stride = k_stride; a.v_stride = v_stride; a.out_stride = out_stride;
+  a.cu_seqlens = cu_seqlens; a.prefix_lens = prefix_lens; a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
+  a.batch = batch; a.num_tokens = num_tokens; a.max_seqlen = max_seqlen; a.max_prefix_len = max_prefix_len; a.max_blocks = max_blocks_per_seq;
+  a.num_heads = num_heads; a.num_kv_heads = num_kv_heads; a.head_dim = head_dim; a.tokens_per_block = tokens_per_block;
+  a.size_per_token = size_per_token; a.int4_kv = int4_kv_cache; a.softmax_scale = softmax_scale;
+  a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = stream;
+  return multi_token_attention(a);
+}
+size_t qs_multi_token_attention_workspace_bytes(int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads,
+                                                int int4_kv_cache) {
+  return multi_token_attention_workspace_bytes(batch, num_tokens, max_seqlen, max_prefix_len, num_heads, num_kv_heads, int4_kv_cache);
+}
+
 int qs_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
                          int64_t out_stride, const int32_t* cu_seqlens, int batch, int num_tokens, int max_seqlen, int num_heads, int num_kv_heads,
                          int head_dim, float softmax_scale, void* stream) {

@@ -136,4 +136,27 @@ struct PrefixAttnArgs {
 };
 int prefix_attention(const PrefixAttnArgs& a);
 
+// multi_token_attention.cu: n <= 16 draft tokens per sequence over the paged INT4 / INT8 cache, each with the semantics of one decode step
+// (speculative-decoding verification)
+struct MultiTokenAttnArgs {
+  const void* q = nullptr;    // fp16 [T, Hq, 128] draft rows (rotated), rows of q_stride halfs
+  const void* k = nullptr;    // fp16 [T, Hkv, 128] (rotated)
+  const void* v = nullptr;
+  void* out = nullptr;        // fp16 [T, Hq, 128], rows of out_stride halfs
+  long long q_stride = 0, k_stride = 0, v_stride = 0, out_stride = 0;
+  const int* cu_seqlens = nullptr;         // [batch + 1] draft token offsets
+  const int* prefix_lens = nullptr;        // [batch] tokens cached before the draft tokens (<= max_prefix_len)
+  const long long* kv_pointers = nullptr;  // [batch, 2, max_blocks] absolute page addresses
+  int batch = 0, num_tokens = 0, max_seqlen = 0, max_prefix_len = 0, max_blocks = 0;
+  int num_heads = 0, num_kv_heads = 0, head_dim = 0, tokens_per_block = 64, size_per_token = 0;
+  int int4_kv = 1;
+  float softmax_scale = 0.f;  // <= 0: 1 / sqrt(128) exactly as the decode kernel computes it
+  void* workspace = nullptr;  // zero-initialised once, then owned by the library (self-cleaning counters)
+  size_t workspace_bytes = 0;
+  void* stream = nullptr;
+};
+int multi_token_attention(const MultiTokenAttnArgs& a);
+size_t multi_token_attention_workspace_bytes(int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads,
+                                             int int4_kv);
+
 }  // namespace qs

@@ -94,8 +94,15 @@ class _Linear:
 class DecodeRunner:
     def __init__(self, model: str = "llama-3-8b", precision: str = "w4a8kv4", batch: int = 64, ctx: int = 1024,
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
-                 process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False):
+                 process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
+                 verify_len: int = 0):
+        """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
+        ctx + verify_len tokens and verify buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers and its
+        random draws exactly as they are without it."""
         assert precision in PRECISIONS, precision
+        assert 0 <= verify_len <= 16, "verify_len: at most 16 draft tokens per sequence"
+        assert verify_len == 0 or (tp_size == 1 and fused), "the verify step is single-GPU and uses the fused path"
+        self.verify_len = verify_len
         self.ops = ops = ops or DEFAULT_OPS
         self.tp_exact = tp_exact
         self.fuse_attn_quant = True  # attention with the per-token quant fused in: one launch per layer fewer
@@ -141,7 +148,7 @@ class DecodeRunner:
         self.lm_head = (torch.randn((cfg.vocab, H), device=dev, generator=gen) * (1.0 / H ** 0.5)).half()  # fp16, cuBLAS (:432)
 
         # ---- paged KV cache: ctx tokens present, the step decodes token ctx (length ctx+1) ---------------------
-        self.blocks_per_seq = (ctx + 1 + 63) // 64
+        self.blocks_per_seq = (ctx + max(1, verify_len) + 63) // 64
         self.size_per_token = self.Hkv * D * self.kv_bits // 8
         code_bytes = 64 * self.size_per_token
         self.page_bytes = code_bytes + self.Hkv * 64 * 4  # cache_engine.py:62-66
@@ -185,6 +192,8 @@ class DecodeRunner:
         self.tokens_out = torch.zeros(M, dtype=torch.int64, device=dev)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.launches_per_step = 0
+        if verify_len:
+            self._alloc_verify_buffers()
 
     # ---------------------------------------------------------------------------------------------------------
     def _norm_quant(self, x, gamma):
@@ -319,6 +328,102 @@ class DecodeRunner:
         self.launches_per_step = n + 2
         self.last_logits = logits
         return logits if return_logits else _ext.argmax_rows(logits)  # one launch instead of torch's two-pass reduction
+
+    # ---------------------------------------------------------------------------------------------------------
+    # speculative-decoding verify: n draft tokens per sequence at positions ctx .. ctx + n - 1 in one step
+    # ---------------------------------------------------------------------------------------------------------
+    def _alloc_verify_buffers(self) -> None:
+        """Activation buffers for batch * verify_len rows, separate from the decode step's (torch.empty: no random draws)."""
+        dev, H, M = self.dev, self.cfg.hidden, self.batch * self.verify_len
+        self.v_qkv = torch.empty((M, self.q_size + 2 * self.kv_size), dtype=torch.half, device=dev)
+        self.v_out = torch.empty((M, H), dtype=torch.half, device=dev)
+        self.v_gate_up = torch.empty((M, 2 * self.Iloc), dtype=torch.half, device=dev)
+        self.v_q_hidden = torch.empty((M, H), dtype=torch.int8, device=dev)
+        self.v_q_attn = torch.empty((M, self.q_size), dtype=torch.int8, device=dev)
+        self.v_q_mlp = torch.empty((M, self.Iloc), dtype=torch.int8, device=dev)
+        self.v_q_scale = torch.empty(M, dtype=torch.half, device=dev)
+        self.v_q_sum = torch.empty(M, dtype=torch.half, device=dev)
+        self.v_start = torch.full((self.batch,), self.ctx, dtype=torch.int32, device=dev)  # tokens cached before the drafts
+        self.v_meta = {}  # n -> (draft lengths [B], cu_seqlens [B + 1], padding offsets [B n]), built on first use (before any capture)
+        self.v_tokens_in = torch.zeros((self.batch, self.verify_len), dtype=torch.int64, device=dev)
+        self.v_tokens_out = torch.zeros((self.batch, self.verify_len), dtype=torch.int64, device=dev)
+        self.v_graphs = {}
+
+    def _verify_meta(self, n: int):
+        if n not in self.v_meta:
+            B, dev = self.batch, self.dev
+            cu = torch.arange(0, B * n + 1, n, dtype=torch.int32, device=dev)
+            self.v_meta[n] = (torch.full((B,), n, dtype=torch.int32, device=dev), cu, _ext.compute_padding_offsets(cu, n, B * n))
+        return self.v_meta[n]
+
+    def verify_forward(self, tokens: torch.Tensor, return_logits: bool = False) -> torch.Tensor:
+        """Score n = tokens.size(1) <= verify_len draft tokens per sequence at positions ctx .. ctx + n - 1 in one step: tokens [B, n] ->
+        greedy tokens [B, n] (or fp16 logits [B, n, vocab]).  Per layer: qkv GEMM at M = B n, apply_bias_rope_update_kv_cache_at at ctx,
+        multi_token_decode_attention (each draft token gets the numbers of its own decode step), invoke_quant[_fuse_sum], then o, gate_up,
+        silu+quant and down as the fused decode step.  The drafts' K / V stay in the pages; a later step at the same positions overwrites
+        them, so rejected drafts need no cleanup."""
+        assert self.verify_len, "construct the runner with verify_len > 0"
+        B, n = tokens.shape
+        assert B == self.batch and 1 <= n <= self.verify_len
+        cfg, D, M = self.cfg, self.cfg.head_dim, B * n
+        lens, cu, pad = self._verify_meta(n)
+        qkv, out_buf, gate_up = self.v_qkv[:M], self.v_out[:M], self.v_gate_up[:M]
+        q_hidden, q_attn, q_mlp = self.v_q_hidden[:M], self.v_q_attn[:M], self.v_q_mlp[:M]
+        q_scale, q_sum = self.v_q_scale[:M], self.v_q_sum[:M]
+        qsum = q_sum if self.act_sum else None
+        hidden = self.embed[tokens.reshape(-1)]
+        nxt = torch.empty_like(hidden)
+        if self.act_sum:
+            layernorm_ops.rms_norm_general_fuse_sum(q_hidden, hidden, self.layers[0]["ln1"], q_sum, q_scale, cfg.eps, True)
+        else:
+            layernorm_ops.rms_norm_general(q_hidden, hidden, self.layers[0]["ln1"], q_scale, cfg.eps, True)
+        for li, ly in enumerate(self.layers):
+            ly["qkv"](q_hidden, q_scale, q_sum, qkv)
+            table = self.block_tables[li]
+            _ext.apply_bias_rope_update_kv_cache_at(qkv, lens, pad, self.v_start, table, self.Hq, self.Hkv, n, 64, self.size_per_token, D,
+                                                   cfg.rope_theta, min(8192, cfg.max_pos), True, self.kv_bits == 4, True)
+            q, k, v = qkv.split([self.q_size, self.kv_size, self.kv_size], dim=-1)
+            attn = _ext.multi_token_decode_attention(q.reshape(M, self.Hq, D), k.reshape(M, self.Hkv, D), v.reshape(M, self.Hkv, D), cu, n, self.v_start,
+                                                     self.ctx, table, 64, self.size_per_token, self.kv_bits == 4)
+            if self.act_sum:
+                fused_kernels.invoke_quant_fuse_sum(q_attn, attn.view(M, -1), q_sum, q_scale)
+            else:
+                fused_kernels.invoke_quant(q_attn, attn.view(M, -1), q_scale)
+            ly["o"](q_attn, q_scale, q_sum, out_buf)
+            _ext.add_rms_norm_general(q_hidden, nxt, hidden, out_buf, ly["ln2"], qsum, q_scale, cfg.eps)
+            hidden, nxt = nxt, hidden
+            ly["gate_up"](q_hidden, q_scale, q_sum, gate_up)
+            _ext.silu_and_mul_quant(q_mlp, gate_up, qsum, q_scale)
+            ly["down"](q_mlp, q_scale, q_sum, out_buf)
+            if li + 1 < len(self.layers):
+                _ext.add_rms_norm_general(q_hidden, nxt, hidden, out_buf, self.layers[li + 1]["ln1"], qsum, q_scale, cfg.eps)
+                hidden, nxt = nxt, hidden
+            else:
+                hidden = hidden + out_buf
+        out = torch.empty_like(hidden)
+        layernorm_ops.rms_norm(out, hidden, self.norm_w, cfg.eps, False)
+        logits = torch.nn.functional.linear(out, self.lm_head)
+        self.last_verify_logits = logits.view(B, n, -1)
+        return self.last_verify_logits if return_logits else _ext.argmax_rows(logits).view(B, n)
+
+    def capture_verify(self, n: int, warmup: int = 2) -> None:
+        """Capture the verify step for n draft tokens in a CUDA graph: v_tokens_in[:, :n] -> v_tokens_out[:, :n]."""
+        tin, tout = self.v_tokens_in[:, :n], self.v_tokens_out[:, :n]
+        s = torch.cuda.Stream(device=self.dev)
+        s.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(s), torch.no_grad():
+            for _ in range(warmup):
+                tout.copy_(self.verify_forward(tin.contiguous()))
+        torch.cuda.current_stream(self.dev).wait_stream(s)
+        torch.cuda.synchronize(self.dev)
+        g = torch.cuda.CUDAGraph()
+        with torch.no_grad(), torch.cuda.graph(g):
+            tout.copy_(self.verify_forward(tin.contiguous()))
+        self.v_graphs[n] = g
+
+    def verify_step(self, n: int) -> None:
+        """Replay the captured verify step for n draft tokens."""
+        self.v_graphs[n].replay()
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
