@@ -250,6 +250,49 @@ QS_API int qs_multi_token_decode_attention(const void* q, const void* k, const v
 QS_API size_t qs_multi_token_attention_workspace_bytes(int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads,
                                                        int num_kv_heads, int int4_kv_cache);
 
+/* Tree-structured drafts (speculative decoding with token trees: Medusa, EAGLE, SpecInfer-style candidate trees).
+ *
+ * Sequence b has prefix_lens[b] = P_b cached tokens and n_b <= 16 draft NODES 0 .. n_b - 1 in topological order (every ancestor has a smaller
+ * index than its descendants).  tree_mask int32 [num_tokens], one word per draft row (aligned with the q rows / cu_seqlens): bit j of node i's
+ * word means "node j is an ancestor of node i"; bits >= i are ignored.  A chain is mask_i = (1 << i) - 1.  The depth of node i is
+ * d_i = popcount(mask_i & ((1 << i) - 1)).  The mask contents are not validated; whatever they hold, no kernel reads a slot >= P_b + i for
+ * node i.  tree_mask is read after the PDL dependency wait (a drafter kernel on the same stream may have just produced it).
+ *
+ * qs_apply_bias_rope_update_kv_cache_tree: qs_apply_bias_rope_update_kv_cache_at (start_pos = P_b, seq_lens = n_b <= 16) for draft nodes:
+ *   node i is rotated (q and k) at position P_b + d_i and quantised into cache slot P_b + i.  The cyclic window uses the slot position and
+ *   the total length P_b + n_b.
+ * qs_tree_decode_attention: qs_multi_token_decode_attention (same arguments, same workspace) with the tree mask: node i attends to the cache
+ *   positions 0 .. P_b - 1, to the slots P_b + j of its ancestors j (read back quantised) and to its own key / value un-quantised; so it gets
+ *   what qs_single_query_attention computes at position P_b + d_i after sequential decoding along its root path, up to the fp32 summation
+ *   order.  With a chain mask the result is bitwise that of qs_multi_token_decode_attention.
+ * qs_tree_accept_greedy: draft_tokens int64 [batch, num_nodes] (padding nodes: -1, which never matches), tree_mask int32 [batch, num_nodes],
+ *   target_tokens int64 [batch, num_nodes] (the target model's greedy token after each node).  From the root (node 0) the walk moves to the
+ *   lowest-index child c of the current node with draft[c] == target[current] (the parent of c is the highest set bit of mask_c below c) until
+ *   no child matches.  Outputs accept_len int32 [batch] (>= 1, root included), path int32 [batch, num_nodes] (path[0] = 0, -1 past
+ *   accept_len) and bonus int64 [batch] = target[path[accept_len - 1]].  One warp per sequence; inputs read after the dependency wait.
+ * qs_kv_cache_compact: for every layer, sequence, K / V and KV head, copies the slot bytes (codes, scale, zero) of P_b + path[k] to slot P_b + k
+ *   for k < accept_len[b].  Node path[k] has depth k, so afterwards slots P_b .. P_b + accept_len - 1 are byte-identical to sequential
+ *   decoding of the accepted tokens; the engine then advances the context by accept_len and feeds bonus as the next root.  kv_pointers is
+ *   [num_layers, batch, 2, max_blocks_per_seq] (num_layers = 1: one layer's table); start_pos int32 [batch].  The page table and start_pos are
+ *   read before the dependency wait, path and accept_len after it.  Slots outside the page table are not touched.  num_nodes <= 16.    */
+QS_API int qs_apply_bias_rope_update_kv_cache_tree(void* qkv, const int32_t* seq_lens, const int32_t* padding_offset, const int32_t* start_pos,
+                                                   const int32_t* tree_mask, const int64_t* kv_pointers, int batch, int num_tokens,
+                                                   int max_blocks_per_seq, int head_num, int kv_head_num, int head_dim, int seq_len,
+                                                   int tokens_per_block, int size_per_token, int rotary_embedding_dim, float rotary_embedding_base,
+                                                   int rotary_embedding_max_positions, int neox_rotary_style, int int4_kv_cache,
+                                                   int kv_cache_with_zeros, void* stream);
+QS_API int qs_tree_decode_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
+                                    int64_t out_stride, const int32_t* cu_seqlens, const int32_t* prefix_lens, const int32_t* tree_mask,
+                                    const int64_t* kv_pointers, int batch, int num_tokens, int max_seqlen, int max_prefix_len,
+                                    int max_blocks_per_seq, int num_heads, int num_kv_heads, int head_dim, int tokens_per_block,
+                                    int size_per_token, int int4_kv_cache, float softmax_scale, void* workspace, size_t workspace_bytes,
+                                    void* stream);
+QS_API int qs_tree_accept_greedy(const int64_t* draft_tokens, const int32_t* tree_mask, const int64_t* target_tokens, int32_t* accept_len,
+                                 int32_t* path, int64_t* bonus, int batch, int num_nodes, void* stream);
+QS_API int qs_kv_cache_compact(const int64_t* kv_pointers, const int32_t* start_pos, const int32_t* path, const int32_t* accept_len, int num_layers,
+                               int batch, int num_nodes, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token,
+                               int int4_kv_cache, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

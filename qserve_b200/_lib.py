@@ -36,6 +36,10 @@ SIGNATURES = {
     "qs_prefix_prefill_attention": (c_int, [_P, _P, _P, _L, _L, _L, _P, _L, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
     "qs_multi_token_decode_attention": (c_int, [_P, _P, _P, _L, _L, _L, _P, _L, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P, _Z, _P]),
     "qs_multi_token_attention_workspace_bytes": (c_size_t, [_I, _I, _I, _I, _I, _I, _I]),
+    "qs_apply_bias_rope_update_kv_cache_tree": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _I, _I, _I, _I, _P]),
+    "qs_tree_decode_attention": (c_int, [_P, _P, _P, _L, _L, _L, _P, _L, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P, _Z, _P]),
+    "qs_tree_accept_greedy": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _P]),
+    "qs_kv_cache_compact": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "qs_rms_norm": (c_int, [_P, _P, _P, _F, _I, _I, _I, _P]),
     "qs_rms_norm_general": (c_int, [_P, _P, _P, _P, _F, _I, _I, _I, _P]),
     "qs_rms_norm_general_fuse_sum": (c_int, [_P, _P, _P, _P, _P, _F, _I, _I, _I, _P]),

@@ -447,10 +447,13 @@ def single_query_attention_quant(q, k, v, kv_pointers, length_per_sample, memory
 def apply_bias_rope_update_kv_cache_at(qkv, seq_lens, padding_offset, start_pos, kv_pointers: Optional[torch.Tensor], head_num: int,
                                        kv_head_num: int, seq_len: int, tokens_per_block: int, size_per_token: int, rotary_embedding_dim: int,
                                        rotary_embedding_base: float, rotary_embedding_max_positions: int, neox_rotary_style: bool,
-                                       int4_kv_cache: bool, kv_cache_with_zeros: bool) -> None:
+                                       int4_kv_cache: bool, kv_cache_with_zeros: bool, tree_mask: Optional[torch.Tensor] = None) -> None:
     """apply_bias_rope_update_kv_cache for prompt CHUNKS that continue sequences whose first start_pos[b] tokens (int32 [B], device) are
     already cached: seq_lens are the chunk lengths, token pos of chunk b is rotated at position start_pos[b] + pos and appended there.
-    Appending a prompt in chunks leaves the same bytes as one apply_bias_rope_update_kv_cache call over the whole prompt."""
+    Appending a prompt in chunks leaves the same bytes as one apply_bias_rope_update_kv_cache call over the whole prompt.
+
+    tree_mask (int32 [T], one ancestor word per row, see tree_decode_attention in multi_token_decode_attention): the rows are draft-tree
+    nodes (seq_len <= 16); node i is rotated at position start_pos[b] + depth(i) and stored in slot start_pos[b] + i.  None: the call above."""
     for t, n in ((qkv, "qkv"), (seq_lens, "seq_lens"), (padding_offset, "padding_offset"), (start_pos, "start_pos")):
         _cuda(t, n)
     _require(qkv.dtype == _HALF and qkv.is_contiguous(), "qkv must be contiguous float16")
@@ -465,6 +468,14 @@ def apply_bias_rope_update_kv_cache_at(qkv, seq_lens, padding_offset, start_pos,
         _cuda(kv_pointers, "kv_pointers")
         _require(kv_pointers.is_contiguous() and kv_pointers.dtype == torch.int64, "kv_pointers must be contiguous int64")
         kvp, max_blocks = kv_pointers.data_ptr(), kv_pointers.size(-1)
+    if tree_mask is not None:
+        _tree_mask_check(tree_mask, qkv.size(0), qkv.device)
+        _require(1 <= int(seq_len) <= 16, "apply_bias_rope_update_kv_cache_at: a draft tree has at most 16 nodes per sequence (seq_len)")
+        _call(qkv, lib.qs_apply_bias_rope_update_kv_cache_tree, qkv.data_ptr(), seq_lens.data_ptr(), padding_offset.data_ptr(), start_pos.data_ptr(),
+              tree_mask.data_ptr(), kvp, seq_lens.size(0), qkv.size(0), max_blocks, int(head_num), int(kv_head_num), head_dim, int(seq_len),
+              int(tokens_per_block), int(size_per_token), int(rotary_embedding_dim), float(rotary_embedding_base), int(rotary_embedding_max_positions),
+              int(bool(neox_rotary_style)), int(bool(int4_kv_cache)), int(bool(kv_cache_with_zeros)))
+        return
     _call(qkv, lib.qs_apply_bias_rope_update_kv_cache_at, qkv.data_ptr(), seq_lens.data_ptr(), padding_offset.data_ptr(), start_pos.data_ptr(), kvp,
           seq_lens.size(0), qkv.size(0), max_blocks, int(head_num), int(kv_head_num), head_dim, int(seq_len), int(tokens_per_block),
           int(size_per_token), int(rotary_embedding_dim), float(rotary_embedding_base), int(rotary_embedding_max_positions),
@@ -523,8 +534,16 @@ def multi_token_workspace(device: torch.device, batch: int, num_tokens: int, max
     return ws
 
 
+def _tree_mask_check(tree_mask: torch.Tensor, rows: int, device: torch.device) -> None:
+    _cuda(tree_mask, "tree_mask")
+    _require(tree_mask.device == device, "tree_mask must be on the device of the other tensors")
+    _require(tree_mask.dtype == torch.int32 and tree_mask.is_contiguous() and tree_mask.numel() == rows,
+             "tree_mask must be contiguous int32 with one word per draft row")
+
+
 def multi_token_decode_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, max_prefix_len: int, kv_pointers, tokens_per_block: int,
-                                 size_per_token: int, int4_kv_cache: bool, softmax_scale: Optional[float] = None) -> torch.Tensor:
+                                 size_per_token: int, int4_kv_cache: bool, softmax_scale: Optional[float] = None,
+                                 tree_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Decode attention of n_b <= 16 draft tokens per sequence in one launch (speculative-decoding verification).  Arguments as for
     prefix_prefill_attention: q [T,Hq,128], k / v [T,Hkv,128] fp16, the draft rows apply_bias_rope_update_kv_cache_at has rotated and appended
     at positions prefix_lens[b] .. prefix_lens[b] + n_b - 1; cu_seqlens int32 [B+1]; prefix_lens int32 [B]; kv_pointers int64 [B,2,max_blocks].
@@ -533,7 +552,14 @@ def multi_token_decode_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_le
     0 .. prefix_lens[b] + i - 1 dequantised from the ZINT4 / ZINT8 pages (the earlier draft tokens included, read back quantised) and to its own
     key and value un-quantised.  So a greedy verify gives the numbers of n sequential decode steps up to the fp32 summation order.  This differs
     from prefix_prefill_attention, which uses every chunk key un-quantised.  1 <= max_seqlen <= 16; max_prefix_len bounds prefix_lens (it is
-    not checked on the device).  The default softmax scale is the decode kernel's 1/sqrt(128).  Returns fp16 [T,Hq,128]."""
+    not checked on the device).  The default softmax scale is the decode kernel's 1/sqrt(128).  Returns fp16 [T,Hq,128].
+
+    tree_mask (int32 [T], one word per draft row): the draft tokens of a sequence are the nodes 0 .. n_b - 1 of a token tree in topological
+    order, appended by apply_bias_rope_update_kv_cache_at(..., tree_mask=tree_mask); bit j of node i's word means "node j is an ancestor of
+    node i" (bits >= i are ignored; a chain is (1 << i) - 1).  Node i attends to the cache positions 0 .. prefix_lens[b] - 1, to the slots of
+    its ancestors and to its own key / value, i.e. it gets the decode step at position prefix_lens[b] + depth(i) after sequential decoding
+    along its root path.  The mask contents are not validated (that would need a host synchronisation); whatever they hold, the kernels never
+    read a slot >= prefix_lens[b] + i for node i.  A chain mask gives this function's result without a mask bit for bit.  None: no mask."""
     for t, n in ((q, "q"), (k, "k"), (v, "v"), (cu_seqlens, "cu_seqlens"), (prefix_lens, "prefix_lens"), (kv_pointers, "kv_pointers")):
         _cuda(t, n)
     _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
@@ -558,10 +584,75 @@ def multi_token_decode_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_le
         return out
     ws = multi_token_workspace(q.device, batch, T, int(max_seqlen), int(max_prefix_len), hq, hkv, int4_kv_cache)
     scale = float(softmax_scale) if softmax_scale is not None else 0.0
+    if tree_mask is not None:
+        _tree_mask_check(tree_mask, T, q.device)
+        _call(q, lib.qs_tree_decode_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), out.data_ptr(),
+              out.stride(0), cu_seqlens.data_ptr(), prefix_lens.data_ptr(), tree_mask.data_ptr(), kv_pointers.data_ptr(), batch, T, int(max_seqlen),
+              int(max_prefix_len), kv_pointers.size(-1), hq, hkv, 128, int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), scale,
+              ws.data_ptr(), ws.numel())
+        return out
     _call(q, lib.qs_multi_token_decode_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), out.data_ptr(),
           out.stride(0), cu_seqlens.data_ptr(), prefix_lens.data_ptr(), kv_pointers.data_ptr(), batch, T, int(max_seqlen), int(max_prefix_len),
           kv_pointers.size(-1), hq, hkv, 128, int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), scale, ws.data_ptr(), ws.numel())
     return out
+
+
+def tree_accept_greedy(draft_tokens, tree_mask, target_tokens, accept_len: Optional[torch.Tensor] = None, path: Optional[torch.Tensor] = None,
+                       bonus: Optional[torch.Tensor] = None):
+    """Greedy acceptance of a draft tree, one warp per sequence and no host synchronisation.  draft_tokens int64 [B, n] (node 0 is the root:
+    the token emitted by the previous step; padding nodes carry -1, which never matches), tree_mask int32 [B, n] (ancestor words as for
+    multi_token_decode_attention), target_tokens int64 [B, n] (the target model's greedy token after each node), n <= 16.  From the root the
+    walk moves to the lowest-index child c of the current node with draft[c] == target[current] until no child matches.  Returns
+    (accept_len int32 [B] >= 1, path int32 [B, n] with path[:, 0] = 0 and -1 past accept_len, bonus int64 [B] = target[last accepted node]);
+    the optional out tensors are written in place (CUDA-graph capture)."""
+    for t, n in ((draft_tokens, "draft_tokens"), (tree_mask, "tree_mask"), (target_tokens, "target_tokens")):
+        _cuda(t, n)
+        _require(t.dim() == 2 and t.is_contiguous() and t.device == draft_tokens.device, f"{n} must be a contiguous [B, n] tensor on one device")
+    _require(draft_tokens.dtype == torch.int64 and target_tokens.dtype == torch.int64 and tree_mask.dtype == torch.int32,
+             "draft_tokens / target_tokens must be int64, tree_mask int32")
+    B, n = draft_tokens.shape
+    _require(tuple(tree_mask.shape) == (B, n) and tuple(target_tokens.shape) == (B, n), "draft_tokens, tree_mask and target_tokens must have one shape")
+    _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
+    dev = draft_tokens.device
+    accept_len = torch.empty(B, dtype=torch.int32, device=dev) if accept_len is None else accept_len
+    path = torch.empty((B, n), dtype=torch.int32, device=dev) if path is None else path
+    bonus = torch.empty(B, dtype=torch.int64, device=dev) if bonus is None else bonus
+    for t, n_, dt, shape in ((accept_len, "accept_len", torch.int32, (B,)), (path, "path", torch.int32, (B, n)), (bonus, "bonus", torch.int64, (B,))):
+        _require(t.device == dev and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, f"{n_} must be contiguous {dt} {shape}")
+    if B:
+        _call(draft_tokens, lib.qs_tree_accept_greedy, draft_tokens.data_ptr(), tree_mask.data_ptr(), target_tokens.data_ptr(), accept_len.data_ptr(),
+              path.data_ptr(), bonus.data_ptr(), B, n)
+    return accept_len, path, bonus
+
+
+def kv_cache_compact(kv_pointers, start_pos, path, accept_len, num_kv_heads: int, tokens_per_block: int, size_per_token: int,
+                     int4_kv_cache: bool) -> None:
+    """Move the accepted path of a draft tree into consecutive cache slots, for every layer in one launch: for k < accept_len[b] the slot
+    bytes (codes, scale, zero; K and V; every KV head) of start_pos[b] + path[b, k] are copied to slot start_pos[b] + k.  Node path[b, k] has
+    depth k and was rotated at that position, so afterwards slots start_pos[b] .. start_pos[b] + accept_len[b] - 1 hold exactly what sequential
+    decoding of the accepted tokens writes; the engine then advances the context by accept_len.  kv_pointers int64 [L, B, 2, max_blocks] or
+    [B, 2, max_blocks]; start_pos int32 [B]; path int32 [B, n] and accept_len int32 [B] as tree_accept_greedy returns them (n <= 16).
+    The page table must cover start_pos[b] + n slots (not checked on the device: slots outside the table are left alone)."""
+    for t, n in ((kv_pointers, "kv_pointers"), (start_pos, "start_pos"), (path, "path"), (accept_len, "accept_len")):
+        _cuda(t, n)
+        _require(t.is_contiguous() and t.device == kv_pointers.device, f"{n} must be contiguous and on the device of kv_pointers")
+    _require(kv_pointers.dtype == torch.int64 and kv_pointers.dim() in (3, 4) and kv_pointers.size(-2) == 2,
+             "kv_pointers must be int64 [L, B, 2, max_blocks] or [B, 2, max_blocks]")
+    L = kv_pointers.size(0) if kv_pointers.dim() == 4 else 1
+    B = kv_pointers.size(-3)
+    _require(start_pos.dtype == torch.int32 and tuple(start_pos.shape) == (B,), "start_pos must be int32 [B]")
+    _require(path.dtype == torch.int32 and path.dim() == 2 and path.size(0) == B, "path must be int32 [B, n]")
+    _require(accept_len.dtype == torch.int32 and tuple(accept_len.shape) == (B,), "accept_len must be int32 [B]")
+    n = path.size(1)
+    _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
+    _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
+    _require(int(num_kv_heads) >= 1 and int(size_per_token) == int(num_kv_heads) * 128 * (4 if int4_kv_cache else 8) // 8,
+             "size_per_token does not match the kv heads and the cache type")
+    _require(n <= kv_pointers.size(-1) * 64, "the page table is too short for the draft nodes")
+    if B == 0 or L == 0:
+        return
+    _call(kv_pointers, lib.qs_kv_cache_compact, kv_pointers.data_ptr(), start_pos.data_ptr(), path.data_ptr(), accept_len.data_ptr(), L, B, n,
+          kv_pointers.size(-1), int(num_kv_heads), int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)))
 
 
 class PeerContext:

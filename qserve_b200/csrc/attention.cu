@@ -643,11 +643,14 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
 //     powf / sincosf per token: 365 us per layer for the 8 x 1024-token prompt batch), then quantises and appends K and V.
 //     applyBiasRopeUpdateKVCache.h:94-455 (STORE_QKV = true, no bias, NeoX)
 // ------------------------------------------------------------------------------------------------
-template <int BITS, bool AT>  // AT: start_pos is given (qs_apply_bias_rope_update_kv_cache_at); otherwise it is ignored
+// AT: start_pos is given (qs_apply_bias_rope_update_kv_cache_at); otherwise it is ignored.  TREE (with AT): the tokens are draft-tree nodes,
+// node cpos is rotated at start + depth(cpos) (the popcount of its ancestor word tree_mask[token]) and stored in slot start + cpos.
+template <int BITS, bool AT, bool TREE = false>
 __global__ void __launch_bounds__(128) prefill_append_kernel(__half* __restrict__ qkv, const int* __restrict__ seq_lens,
                                                              const int* __restrict__ padding_offset, const long long* __restrict__ kv_pointers,
                                                              const int* __restrict__ start_pos, int num_tokens, int max_blocks, int num_heads, int num_kv_heads, int seq_len,
-                                                             PageGeom pg, float rotary_base, int rotary_dim, int max_positions) {
+                                                             PageGeom pg, float rotary_base, int rotary_dim, int max_positions,
+                                                             const int* __restrict__ tree_mask) {
   if (threadIdx.x == 0) pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31;
@@ -667,13 +670,14 @@ __global__ void __launch_bounds__(128) prefill_append_kernel(__half* __restrict_
     // page / slot and the cyclic window all use the shifted values, so appending a prompt in chunks gives the bytes of a one-shot append
     const int start = AT ? __ldg(start_pos + bidx) : 0;
     const int pos = start + cpos, len = start + clen;
+    const int rpos = TREE ? start + __popc(static_cast<uint32_t>(tree_mask[token]) & ((1u << cpos) - 1u)) : pos;  // RoPE position
     __half* trow = qkv + static_cast<size_t>(token) * n;
     // lane handles rotary pairs i = 2*lane, 2*lane+1  (i in [0, 64)) -> dims i and i + half_rot: one half2 at each end
     float cs[2], sn[2];
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
       const int i = 2 * lane + e;
-      const float inv_freq = __fdiv_rn(static_cast<float>(pos), powf(rotary_base, __fdiv_rn(static_cast<float>(2 * i), static_cast<float>(rotary_dim))));
+      const float inv_freq = __fdiv_rn(static_cast<float>(rpos), powf(rotary_base, __fdiv_rn(static_cast<float>(2 * i), static_cast<float>(rotary_dim))));
       sincosf(inv_freq, &sn[e], &cs[e]);
     }
     auto rotate = [&](__half* row, float (&lo)[2], float (&hi)[2]) {  // in place; returns the rotated values (rounded to fp16) as floats
@@ -874,8 +878,13 @@ int prefill_rope_append(const PrefillAppendArgs& a) {
   auto run = [&](auto kern) {
     return launch_pdl(kern, dim3(static_cast<unsigned>(blocks)), dim3(128), 0, a.stream, "apply_bias_rope_update_kv_cache", static_cast<__half*>(a.qkv),
                       a.seq_lens, a.padding_offset, a.kv_pointers, a.start_pos, a.num_tokens, a.max_blocks, a.num_heads, a.num_kv_heads, a.seq_len, pg,
-                      a.rotary_base, a.rotary_dim, a.max_positions);
+                      a.rotary_base, a.rotary_dim, a.max_positions, a.tree_mask);
   };
+  if (a.tree_mask) {
+    QS_REQUIRE(a.start_pos && a.seq_len <= 16, "apply_bias_rope_update_kv_cache_tree: needs start_pos and at most 16 draft nodes per sequence (seq_len=%d)",
+               a.seq_len);
+    return a.int4_kv ? run(prefill_append_kernel<4, true, true>) : run(prefill_append_kernel<8, true, true>);
+  }
   if (a.start_pos) return a.int4_kv ? run(prefill_append_kernel<4, true>) : run(prefill_append_kernel<8, true>);
   return a.int4_kv ? run(prefill_append_kernel<4, false>) : run(prefill_append_kernel<8, false>);
 }

@@ -186,6 +186,23 @@ int qs_apply_bias_rope_update_kv_cache_at(void* qkv, const int32_t* seq_lens, co
   return prefill_rope_append(a);
 }
 
+int qs_apply_bias_rope_update_kv_cache_tree(void* qkv, const int32_t* seq_lens, const int32_t* padding_offset, const int32_t* start_pos,
+                                            const int32_t* tree_mask, const int64_t* kv_pointers, int batch, int num_tokens, int max_blocks_per_seq,
+                                            int head_num, int kv_head_num, int head_dim, int seq_len, int tokens_per_block, int size_per_token,
+                                            int rotary_embedding_dim, float rotary_embedding_base, int rotary_embedding_max_positions,
+                                            int neox_rotary_style, int int4_kv_cache, int kv_cache_with_zeros, void* stream) {
+  (void)neox_rotary_style;
+  QS_REQUIRE(qkv && seq_lens && start_pos && tree_mask, "apply_bias_rope_update_kv_cache_tree: null tensor");
+  PrefillAppendArgs a;
+  a.qkv = qkv; a.seq_lens = seq_lens; a.padding_offset = padding_offset; a.start_pos = start_pos; a.tree_mask = tree_mask;
+  a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
+  a.batch = batch; a.num_tokens = num_tokens; a.max_blocks = max_blocks_per_seq; a.num_heads = head_num; a.num_kv_heads = kv_head_num;
+  a.head_dim = head_dim; a.seq_len = seq_len; a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token;
+  a.rotary_dim = rotary_embedding_dim; a.rotary_base = rotary_embedding_base; a.max_positions = rotary_embedding_max_positions;
+  a.int4_kv = int4_kv_cache; a.kv_zeros = kv_cache_with_zeros; a.stream = stream;
+  return prefill_rope_append(a);
+}
+
 int qs_prefix_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
                                 int64_t out_stride, const int32_t* cu_seqlens, const int32_t* prefix_lens, const int64_t* kv_pointers, int batch,
                                 int num_tokens, int max_seqlen, int max_prefix_len, int max_blocks_per_seq, int num_heads, int num_kv_heads, int head_dim,
@@ -216,6 +233,38 @@ int qs_multi_token_decode_attention(const void* q, const void* k, const void* v,
 size_t qs_multi_token_attention_workspace_bytes(int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads,
                                                 int int4_kv_cache) {
   return multi_token_attention_workspace_bytes(batch, num_tokens, max_seqlen, max_prefix_len, num_heads, num_kv_heads, int4_kv_cache);
+}
+
+int qs_tree_decode_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
+                             int64_t out_stride, const int32_t* cu_seqlens, const int32_t* prefix_lens, const int32_t* tree_mask,
+                             const int64_t* kv_pointers, int batch, int num_tokens, int max_seqlen, int max_prefix_len, int max_blocks_per_seq,
+                             int num_heads, int num_kv_heads, int head_dim, int tokens_per_block, int size_per_token, int int4_kv_cache,
+                             float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
+  QS_REQUIRE(tree_mask, "tree_decode_attention: null tree_mask");
+  MultiTokenAttnArgs a;
+  a.q = q; a.k = k; a.v = v; a.out = out; a.q_stride = q_stride; a.k_stride = k_stride; a.v_stride = v_stride; a.out_stride = out_stride;
+  a.cu_seqlens = cu_seqlens; a.prefix_lens = prefix_lens; a.tree_mask = tree_mask; a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
+  a.batch = batch; a.num_tokens = num_tokens; a.max_seqlen = max_seqlen; a.max_prefix_len = max_prefix_len; a.max_blocks = max_blocks_per_seq;
+  a.num_heads = num_heads; a.num_kv_heads = num_kv_heads; a.head_dim = head_dim; a.tokens_per_block = tokens_per_block;
+  a.size_per_token = size_per_token; a.int4_kv = int4_kv_cache; a.softmax_scale = softmax_scale;
+  a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = stream;
+  return multi_token_attention(a);
+}
+
+int qs_tree_accept_greedy(const int64_t* draft_tokens, const int32_t* tree_mask, const int64_t* target_tokens, int32_t* accept_len, int32_t* path,
+                          int64_t* bonus, int batch, int num_nodes, void* stream) {
+  return tree_accept_greedy(reinterpret_cast<const long long*>(draft_tokens), tree_mask, reinterpret_cast<const long long*>(target_tokens), accept_len,
+                            path, reinterpret_cast<long long*>(bonus), batch, num_nodes, stream);
+}
+
+int qs_kv_cache_compact(const int64_t* kv_pointers, const int32_t* start_pos, const int32_t* path, const int32_t* accept_len, int num_layers, int batch,
+                        int num_nodes, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token, int int4_kv_cache,
+                        void* stream) {
+  KvCompactArgs a;
+  a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers); a.start_pos = start_pos; a.path = path; a.accept_len = accept_len;
+  a.layers = num_layers; a.batch = batch; a.num_nodes = num_nodes; a.max_blocks = max_blocks_per_seq; a.num_kv_heads = num_kv_heads;
+  a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token; a.int4_kv = int4_kv_cache; a.stream = stream;
+  return kv_cache_compact(a);
 }
 
 int qs_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,

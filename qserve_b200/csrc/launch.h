@@ -94,6 +94,8 @@ struct PrefillAppendArgs {
   const int* padding_offset = nullptr;
   const long long* kv_pointers = nullptr;  // may be null: rotate only
   const int* start_pos = nullptr;          // optional [batch]: tokens of each sequence already cached; token pos sits at start_pos[b] + pos
+  const int* tree_mask = nullptr;          // optional [num_tokens] draft-tree ancestor words (needs start_pos): node i is rotated at
+                                           // start_pos[b] + depth(i) and stored in slot start_pos[b] + i
   int batch = 0, num_tokens = 0, max_blocks = 0, num_heads = 0, num_kv_heads = 0, head_dim = 0;
   int seq_len = 0, tokens_per_block = 64, size_per_token = 0, rotary_dim = 0, max_positions = 0;
   float rotary_base = 10000.f;
@@ -151,6 +153,7 @@ struct MultiTokenAttnArgs {
   int num_heads = 0, num_kv_heads = 0, head_dim = 0, tokens_per_block = 64, size_per_token = 0;
   int int4_kv = 1;
   float softmax_scale = 0.f;  // <= 0: 1 / sqrt(128) exactly as the decode kernel computes it
+  const int* tree_mask = nullptr;  // optional [num_tokens] ancestor words of tree-structured drafts (qs_tree_decode_attention)
   void* workspace = nullptr;  // zero-initialised once, then owned by the library (self-cleaning counters)
   size_t workspace_bytes = 0;
   void* stream = nullptr;
@@ -158,5 +161,18 @@ struct MultiTokenAttnArgs {
 int multi_token_attention(const MultiTokenAttnArgs& a);
 size_t multi_token_attention_workspace_bytes(int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads,
                                              int int4_kv);
+
+// tree_verify.cu: greedy acceptance of a draft tree and compaction of the accepted path's K / V slots (speculative decoding with token trees)
+int tree_accept_greedy(const long long* draft, const int* tree_mask, const long long* target, int* accept_len, int* path, long long* bonus,
+                       int batch, int num_nodes, void* stream);
+struct KvCompactArgs {
+  const long long* kv_pointers = nullptr;  // [layers, batch, 2, max_blocks] absolute page addresses
+  const int* start_pos = nullptr;          // [batch] tokens cached before the draft nodes
+  const int* path = nullptr;               // [batch, num_nodes] accepted node indices
+  const int* accept_len = nullptr;         // [batch]
+  int layers = 1, batch = 0, num_nodes = 0, max_blocks = 0, num_kv_heads = 0, tokens_per_block = 64, size_per_token = 0, int4_kv = 1;
+  void* stream = nullptr;
+};
+int kv_cache_compact(const KvCompactArgs& a);
 
 }  // namespace qs

@@ -12,6 +12,11 @@
 // biased-code operands, scale folding, the online softmax in log2 units and the self-cleaning split merge are the decode kernel's
 // (paged_attention.cuh); the per-column causal limit P_b + i is applied only to the slices that hold draft tokens.  There is no RoPE and no
 // page append here.
+//
+// Tree-structured drafts (TREE = true, qs_tree_decode_attention): tree_mask[tok0 + i] bit j says that node j is an ancestor of node i (bits
+// >= i are ignored).  Node i attends to the prefix 0 .. P_b - 1, to the slots P_b + j of its ancestors j and to its own un-quantised key /
+// value; the per-column limit becomes the column's ancestor word, tested in the same causal-tail branch.  A chain mask ((1 << i) - 1) masks
+// exactly the positions >= P_b + i, so it gives the chain kernel's result bit for bit.
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -37,6 +42,7 @@ struct MultiTokenParams {
   float scale_log2;               // softmax scale * log2(e); 0: the decode kernel's rsqrt(128) * log2(e)
   float* ws_part;                 // [T, Hq, nsplit, 130] split partials (O, max, sum)
   uint32_t* ws_cnt;               // [B, gridDim.x] arrival counters (zero between launches), in the fixed counter region
+  const int* tree_mask;           // TREE: [T] ancestor words of the draft nodes (read after the dependency wait)
 };
 
 // Resident CTAs per SM the register budget is sized for: ptxas needs 134 / 146 (KV4 / KV8) registers for one n8 tile and 211 / 241 for two
@@ -45,7 +51,7 @@ struct MultiTokenParams {
 template <int NT>
 constexpr int kMinBlocks = NT == 1 ? 3 : 2;
 
-template <int BITS, int NT>
+template <int BITS, int NT, bool TREE>
 __global__ void __launch_bounds__(kAttnConsumers, kMinBlocks<NT>) multi_token_attention_kernel(const MultiTokenParams p) {
   using SL = StageLayout<BITS>;
   constexpr int R = SL::kStages;
@@ -128,12 +134,20 @@ __global__ void __launch_bounds__(kAttnConsumers, kMinBlocks<NT>) multi_token_at
   }
   __syncthreads();
 
-  // causal limit of this thread's S^T columns 8t + 2q4, 8t + 2q4 + 1: cache positions >= P + i are masked (columns without data: the last token's)
+  // causal limit of this thread's S^T columns 8t + 2q4, 8t + 2q4 + 1: cache positions >= P + i are masked (columns without data: the last token's).
+  // TREE: the column's ancestor word instead (bits < i of tree_mask[tok0 + i]; the same registers)
   int lim[NT][2];
 #pragma unroll
   for (int t = 0; t < NT; ++t)
 #pragma unroll
-    for (int u = 0; u < 2; ++u) lim[t][u] = P + min((col0 + 8 * t + 2 * q4 + u) / G, n_b - 1);
+    for (int u = 0; u < 2; ++u) {
+      const int i = min((col0 + 8 * t + 2 * q4 + u) / G, n_b - 1);
+      if constexpr (TREE) {
+        lim[t][u] = p.tree_mask[tok0 + i] & static_cast<int>((1u << i) - 1u);
+      } else {
+        lim[t][u] = P + i;
+      }
+    }
 
   // ---- Q as the MMA "B" operand per n8 tile (q_operand).  The B fragments live in shared memory (s_qb[t][w][lane] = the two k-steps of
   //      word w), not in registers: with NT = 2 the O^T accumulators alone take 64 registers, and 32 more for Q would spill ----
@@ -196,10 +210,19 @@ __global__ void __launch_bounds__(kAttnConsumers, kMinBlocks<NT>) multi_token_at
           const int tA = t0 + c * kChunk + tokA, tB = tA + 8;
 #pragma unroll
           for (int t = 0; t < NT; ++t) {
-            if (tA >= lim[t][0]) tl[c][t][0] = -CUDART_INF_F;
-            if (tA >= lim[t][1]) tl[c][t][1] = -CUDART_INF_F;
-            if (tB >= lim[t][0]) tl[c][t][2] = -CUDART_INF_F;
-            if (tB >= lim[t][1]) tl[c][t][3] = -CUDART_INF_F;
+            if constexpr (TREE) {
+              // position P + r with r >= 0 is allowed iff bit r of the ancestor word is set (the word has no bits >= 16)
+              auto blocked = [&](int r, int word) { return r >= 0 && !((static_cast<uint32_t>(word) >> min(r, 31)) & 1u); };
+              if (blocked(tA - P, lim[t][0])) tl[c][t][0] = -CUDART_INF_F;
+              if (blocked(tA - P, lim[t][1])) tl[c][t][1] = -CUDART_INF_F;
+              if (blocked(tB - P, lim[t][0])) tl[c][t][2] = -CUDART_INF_F;
+              if (blocked(tB - P, lim[t][1])) tl[c][t][3] = -CUDART_INF_F;
+            } else {
+              if (tA >= lim[t][0]) tl[c][t][0] = -CUDART_INF_F;
+              if (tA >= lim[t][1]) tl[c][t][1] = -CUDART_INF_F;
+              if (tB >= lim[t][0]) tl[c][t][2] = -CUDART_INF_F;
+              if (tB >= lim[t][1]) tl[c][t][3] = -CUDART_INF_F;
+            }
           }
         }
       }
@@ -305,14 +328,28 @@ int resident_ctas() {
   if (r == 0) {
     const int smem = kWarps * StageLayout<BITS>::kWarpBytes;
     int n = 0;
-    if (cudaFuncSetAttribute(multi_token_attention_kernel<BITS, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, multi_token_attention_kernel<BITS, NT>, kAttnConsumers, smem) != cudaSuccess || n < 1) {
+    if (cudaFuncSetAttribute(multi_token_attention_kernel<BITS, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, multi_token_attention_kernel<BITS, NT, false>, kAttnConsumers, smem) != cudaSuccess || n < 1) {
       cudaGetLastError();
       n = 1;
     }
     r = n;
   }
   return r;
+}
+
+// The tree instantiations run with the chain kernel's launch plan; they only need the dynamic shared memory attribute (once per device).
+template <int BITS, int NT>
+int tree_smem_attribute() {
+  static bool done[kMaxDevices] = {};
+  bool& d = done[device_ordinal()];
+  if (!d) {
+    const int rc = check_cuda(cudaFuncSetAttribute(multi_token_attention_kernel<BITS, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   kWarps * StageLayout<BITS>::kWarpBytes), "tree_decode_attention smem attribute");
+    if (rc) return rc;
+    d = true;
+  }
+  return QS_OK;
 }
 
 MultiTokenPlan plan_multi_token(int bits, int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads) {
@@ -392,6 +429,7 @@ int multi_token_attention(const MultiTokenAttnArgs& a) {
   p.scale_log2 = a.softmax_scale > 0.f ? a.softmax_scale * 1.4426950408889634f : 0.f;
   p.ws_cnt = static_cast<uint32_t*>(a.workspace);
   p.ws_part = pl.nsplit > 1 ? reinterpret_cast<float*>(static_cast<uint8_t*>(a.workspace) + pl.cnt_bytes) : nullptr;
+  p.tree_mask = a.tree_mask;
   const dim3 grid(static_cast<unsigned>(gx), a.batch, pl.nsplit);
   auto run = [&](auto kern, size_t smem) {
     cudaLaunchConfig_t cfg{};
@@ -407,8 +445,17 @@ int multi_token_attention(const MultiTokenAttnArgs& a) {
     return check_cuda(cudaLaunchKernelEx(&cfg, kern, p), "multi_token_decode_attention");
   };
   const size_t smem4 = static_cast<size_t>(kWarps) * StageLayout<4>::kWarpBytes, smem8 = static_cast<size_t>(kWarps) * StageLayout<8>::kWarpBytes;
-  if (a.int4_kv) return pl.ntile == 1 ? run(multi_token_attention_kernel<4, 1>, smem4) : run(multi_token_attention_kernel<4, 2>, smem4);
-  return pl.ntile == 1 ? run(multi_token_attention_kernel<8, 1>, smem8) : run(multi_token_attention_kernel<8, 2>, smem8);
+  if (a.tree_mask) {
+    int rc;
+    if (a.int4_kv) {
+      if (pl.ntile == 1) return (rc = tree_smem_attribute<4, 1>()) ? rc : run(multi_token_attention_kernel<4, 1, true>, smem4);
+      return (rc = tree_smem_attribute<4, 2>()) ? rc : run(multi_token_attention_kernel<4, 2, true>, smem4);
+    }
+    if (pl.ntile == 1) return (rc = tree_smem_attribute<8, 1>()) ? rc : run(multi_token_attention_kernel<8, 1, true>, smem8);
+    return (rc = tree_smem_attribute<8, 2>()) ? rc : run(multi_token_attention_kernel<8, 2, true>, smem8);
+  }
+  if (a.int4_kv) return pl.ntile == 1 ? run(multi_token_attention_kernel<4, 1, false>, smem4) : run(multi_token_attention_kernel<4, 2, false>, smem4);
+  return pl.ntile == 1 ? run(multi_token_attention_kernel<8, 1, false>, smem8) : run(multi_token_attention_kernel<8, 2, false>, smem8);
 }
 
 }  // namespace qs

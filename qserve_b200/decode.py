@@ -347,7 +347,12 @@ class DecodeRunner:
         self.v_meta = {}  # n -> (draft lengths [B], cu_seqlens [B + 1], padding offsets [B n]), built on first use (before any capture)
         self.v_tokens_in = torch.zeros((self.batch, self.verify_len), dtype=torch.int64, device=dev)
         self.v_tokens_out = torch.zeros((self.batch, self.verify_len), dtype=torch.int64, device=dev)
-        self.v_graphs = {}
+        # draft-tree verify (capture_verify(n, tree=True)): ancestor words in, acceptance out
+        self.v_tree_mask = torch.zeros((self.batch, self.verify_len), dtype=torch.int32, device=dev)
+        self.v_accept_len = torch.zeros(self.batch, dtype=torch.int32, device=dev)
+        self.v_path = torch.zeros(self.batch * self.verify_len, dtype=torch.int32, device=dev)  # [:B n] viewed as [B, n] for n nodes
+        self.v_bonus = torch.zeros(self.batch, dtype=torch.int64, device=dev)
+        self.v_graphs = {}  # (n, tree) -> CUDA graph
 
     def _verify_meta(self, n: int):
         if n not in self.v_meta:
@@ -356,17 +361,24 @@ class DecodeRunner:
             self.v_meta[n] = (torch.full((B,), n, dtype=torch.int32, device=dev), cu, _ext.compute_padding_offsets(cu, n, B * n))
         return self.v_meta[n]
 
-    def verify_forward(self, tokens: torch.Tensor, return_logits: bool = False) -> torch.Tensor:
+    def verify_forward(self, tokens: torch.Tensor, return_logits: bool = False, tree_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Score n = tokens.size(1) <= verify_len draft tokens per sequence at positions ctx .. ctx + n - 1 in one step: tokens [B, n] ->
         greedy tokens [B, n] (or fp16 logits [B, n, vocab]).  Per layer: qkv GEMM at M = B n, apply_bias_rope_update_kv_cache_at at ctx,
         multi_token_decode_attention (each draft token gets the numbers of its own decode step), invoke_quant[_fuse_sum], then o, gate_up,
         silu+quant and down as the fused decode step.  The drafts' K / V stay in the pages; a later step at the same positions overwrites
-        them, so rejected drafts need no cleanup."""
+        them, so rejected drafts need no cleanup.
+
+        tree_mask (int32 [B, n], ancestor words, see backend.multi_token_decode_attention): the tokens are the nodes of a draft tree, node i
+        is rotated at ctx + depth(i), stored in slot ctx + i and attends to the prefix and its ancestors; follow with accept_and_compact."""
         assert self.verify_len, "construct the runner with verify_len > 0"
         B, n = tokens.shape
         assert B == self.batch and 1 <= n <= self.verify_len
         cfg, D, M = self.cfg, self.cfg.head_dim, B * n
         lens, cu, pad = self._verify_meta(n)
+        tm = None
+        if tree_mask is not None:
+            assert tuple(tree_mask.shape) == (B, n) and tree_mask.dtype == torch.int32
+            tm = tree_mask.contiguous().view(-1)
         qkv, out_buf, gate_up = self.v_qkv[:M], self.v_out[:M], self.v_gate_up[:M]
         q_hidden, q_attn, q_mlp = self.v_q_hidden[:M], self.v_q_attn[:M], self.v_q_mlp[:M]
         q_scale, q_sum = self.v_q_scale[:M], self.v_q_sum[:M]
@@ -381,10 +393,10 @@ class DecodeRunner:
             ly["qkv"](q_hidden, q_scale, q_sum, qkv)
             table = self.block_tables[li]
             _ext.apply_bias_rope_update_kv_cache_at(qkv, lens, pad, self.v_start, table, self.Hq, self.Hkv, n, 64, self.size_per_token, D,
-                                                   cfg.rope_theta, min(8192, cfg.max_pos), True, self.kv_bits == 4, True)
+                                                   cfg.rope_theta, min(8192, cfg.max_pos), True, self.kv_bits == 4, True, tree_mask=tm)
             q, k, v = qkv.split([self.q_size, self.kv_size, self.kv_size], dim=-1)
             attn = _ext.multi_token_decode_attention(q.reshape(M, self.Hq, D), k.reshape(M, self.Hkv, D), v.reshape(M, self.Hkv, D), cu, n, self.v_start,
-                                                     self.ctx, table, 64, self.size_per_token, self.kv_bits == 4)
+                                                     self.ctx, table, 64, self.size_per_token, self.kv_bits == 4, tree_mask=tm)
             if self.act_sum:
                 fused_kernels.invoke_quant_fuse_sum(q_attn, attn.view(M, -1), q_sum, q_scale)
             else:
@@ -406,24 +418,46 @@ class DecodeRunner:
         self.last_verify_logits = logits.view(B, n, -1)
         return self.last_verify_logits if return_logits else _ext.argmax_rows(logits).view(B, n)
 
-    def capture_verify(self, n: int, warmup: int = 2) -> None:
-        """Capture the verify step for n draft tokens in a CUDA graph: v_tokens_in[:, :n] -> v_tokens_out[:, :n]."""
-        tin, tout = self.v_tokens_in[:, :n], self.v_tokens_out[:, :n]
+    def accept_and_compact(self, tokens: torch.Tensor, tree_mask: torch.Tensor, target: torch.Tensor):
+        """After verify_forward(tokens, tree_mask=tree_mask) returned the greedy targets [B, n]: greedy acceptance of the tree and compaction
+        of the accepted path's K / V into slots ctx .. ctx + accept_len - 1 of every layer (one launch each).  Returns (accept_len int32 [B],
+        path int32 [B, n], bonus int64 [B]), written into v_accept_len, v_path and v_bonus.  The runner's positions stay at ctx: the engine
+        advances each context by accept_len and feeds bonus as the next root."""
+        n = tokens.size(1)
+        path = self.v_path[: self.batch * n].view(self.batch, n)
+        acc, path, bonus = _ext.tree_accept_greedy(tokens.contiguous(), tree_mask.contiguous(), target.contiguous(), self.v_accept_len, path,
+                                                   self.v_bonus)
+        _ext.kv_cache_compact(self.block_tables, self.v_start, path, acc, self.Hkv, 64, self.size_per_token, self.kv_bits == 4)
+        return acc, path, bonus
+
+    def _verify_graph_body(self, n: int, tree: bool) -> None:
+        tin, tout = self.v_tokens_in[:, :n].contiguous(), self.v_tokens_out[:, :n]
+        if not tree:
+            tout.copy_(self.verify_forward(tin))
+            return
+        mask = self.v_tree_mask[:, :n].contiguous()
+        tout.copy_(self.verify_forward(tin, tree_mask=mask))
+        self.accept_and_compact(tin, mask, tout)
+
+    def capture_verify(self, n: int, warmup: int = 2, tree: bool = False) -> None:
+        """Capture the verify step for n draft tokens in a CUDA graph: v_tokens_in[:, :n] -> v_tokens_out[:, :n].  tree=True: the graph
+        also reads v_tree_mask[:, :n] and runs accept_and_compact (v_accept_len, v_path, v_bonus).  The warm-up runs the step eagerly, so it
+        writes the draft slots (and, with tree=True, compacts them) like a replay does."""
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(s), torch.no_grad():
             for _ in range(warmup):
-                tout.copy_(self.verify_forward(tin.contiguous()))
+                self._verify_graph_body(n, tree)
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         g = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(g):
-            tout.copy_(self.verify_forward(tin.contiguous()))
-        self.v_graphs[n] = g
+            self._verify_graph_body(n, tree)
+        self.v_graphs[(n, tree)] = g
 
-    def verify_step(self, n: int) -> None:
+    def verify_step(self, n: int, tree: bool = False) -> None:
         """Replay the captured verify step for n draft tokens."""
-        self.v_graphs[n].replay()
+        self.v_graphs[(n, tree)].replay()
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
