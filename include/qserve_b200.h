@@ -293,6 +293,33 @@ QS_API int qs_kv_cache_compact(const int64_t* kv_pointers, const int32_t* start_
                                int batch, int num_nodes, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token,
                                int int4_kv_cache, void* stream);
 
+/* Sampling on the GPU (the sampler's warpers and draw, and sampled acceptance of draft trees).
+ *
+ * Per row: temperature T (fp32), top_k (int32, -1 disables) and top_p (fp32), device arrays.  A row is GREEDY if T < 1e-5 or top_p < 1e-8,
+ * or if it has no logit other than NaN / -inf: its token is what qs_argmax_rows returns.  Otherwise z = x / T (IEEE fp32), w = exp(z - max z),
+ * NaN and -inf logits weigh 0, and the kept set is {z >= max(tau_p, tau_k)}: tau_k is the k-th largest z (top_k > 0, clamped to the count
+ * of such logits), tau_p the smallest z whose strictly larger weight is < top_p * sum w (top_p < 1).  This is Hugging Face's TopP then TopK
+ * warper (min_tokens_to_keep = 1) independent of tie order.  Draws: Philox4x32-10 with counter (lo(off), hi(off), row, j) and key (lo(seed),
+ * hi(seed)), u = (x0 >> 8) * 2^-24, off = offsets[row]; every call advances offsets[row] by one (also for greedy rows).  The token is the
+ * smallest index t with sum_{j <= t, kept} w_j > u * sum_kept w.  Weight sums are exact 64-bit fixed-point sums, so a call is bitwise
+ * deterministic.  vocab % 8 == 0, vocab <= 196608; logits rows 16-byte aligned.  Parameter arrays are trusted (not read on the host);
+ * everything is read after the PDL dependency wait; CUDA-graph capturable.
+ *
+ * qs_sample_rows: out int64 [rows] (draw j = 0).
+ * qs_tree_accept_sampling: the sampled counterpart of qs_tree_accept_greedy (same draft_tokens, tree_mask and outputs), per-sequence
+ *   parameters and offsets [batch].  logits fp16 [batch, num_nodes, vocab] are the verify logits; draft_probs fp32 [batch, num_nodes, vocab]
+ *   or NULL: row c is the distribution q_c node c's token was drawn from (NULL: one-hot at draft[c]).  From the root with p = the warped
+ *   logits of node 0, the children of the current node are tried in index order: child c with token d is accepted iff u_c q_c(d) < p(d)
+ *   (u_c: draw j = c); accepting moves to c with p = the warped logits of c, rejecting sets p <- max(p - q_c, 0) renormalised (kept if its
+ *   mass is 0).  Padding and out-of-range drafts are never accepted and leave p unchanged.  With no child accepted, bonus is drawn from p
+ *   (draw j = 0).  This keeps the target distribution exactly (SpecInfer multi-step speculative sampling).  Greedy rows give exactly
+ *   qs_tree_accept_greedy(draft, mask, argmax of every node's logits).  num_nodes <= 16.                                                     */
+QS_API int qs_sample_rows(int64_t* out, const void* logits, const float* temperature, const int32_t* top_k, const float* top_p, uint64_t seed,
+                          int64_t* offsets, int rows, int vocab, void* stream);
+QS_API int qs_tree_accept_sampling(const int64_t* draft_tokens, const int32_t* tree_mask, const void* logits, const float* draft_probs,
+                                   const float* temperature, const int32_t* top_k, const float* top_p, uint64_t seed, int64_t* offsets,
+                                   int32_t* accept_len, int32_t* path, int64_t* bonus, int batch, int num_nodes, int vocab, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

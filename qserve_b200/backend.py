@@ -655,6 +655,96 @@ def kv_cache_compact(kv_pointers, start_pos, path, accept_len, num_kv_heads: int
           kv_pointers.size(-1), int(num_kv_heads), int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)))
 
 
+def _row_params(n: int, dev, temperature, top_k, top_p, offsets):
+    """Per-row sampling parameters as device tensors: scalars broadcast (and are checked on the host); tensors are used as given (their
+    values are trusted: checking them would synchronise with the device)."""
+    def vec(v, dt, name, ok, what):
+        if isinstance(v, torch.Tensor):
+            _cuda(v, name)
+            _require(v.dtype == dt and v.is_contiguous() and tuple(v.shape) == (n,) and v.device == dev, f"{name} must be contiguous {dt} [{n}]")
+            return v
+        _require(ok(v), f"{name}={v}: {what}")
+        return torch.full((n,), v, dtype=dt, device=dev)
+    T = vec(temperature, torch.float32, "temperature", lambda v: float(v) >= 0, "must be >= 0")
+    K = vec(top_k, torch.int32, "top_k", lambda v: int(v) == -1 or int(v) >= 1, "must be -1 (off) or >= 1")
+    P = vec(top_p, torch.float32, "top_p", lambda v: 0 < float(v) <= 1, "must lie in (0, 1]")
+    _cuda(offsets, "offsets")
+    _require(offsets.dtype == torch.int64 and offsets.is_contiguous() and tuple(offsets.shape) == (n,) and offsets.device == dev,
+             f"offsets must be a contiguous int64 [{n}] tensor")
+    return T, K, P
+
+
+def _seed(seed) -> int:
+    _require(0 <= int(seed) < (1 << 64), "seed must be an unsigned 64-bit integer")
+    return int(seed)
+
+
+def sample_rows(logits, temperature, top_k, top_p, seed: int, offsets, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Temperature / top-p / top-k sampling, one token per row of fp16 logits [rows, V] in one launch: the GPU work of the reference's
+    `Sampler.forward` (qserve/modeling/layers/sampler.py:24-93).  temperature (fp32), top_k (int32, -1 disables) and top_p (fp32) are
+    per-row tensors or scalars; seed is a uint64; offsets int64 [rows] (device) is read and advanced by one per call, so CUDA-graph
+    replays draw fresh numbers.  Greedy rows (T < 1e-5 or top_p < 1e-8) return exactly argmax_rows.  Otherwise the kept set is
+    {z >= max(tau_p, tau_k)} of z = x / T: what TopPLogitsWarper then TopKLogitsWarper keep, stated independently of tie order, and the
+    token is the inverse CDF of the kept softmax at the Philox draw u (see include/qserve_b200.h).  Differences from the reference: the
+    reference divides by T and runs softmax().cumsum() over the row in fp16 and draws with torch's RNG, so the distribution agrees up to its
+    fp16 rounding but the same seed does not give the same tokens.  V % 8 == 0, V <= 196608.  Returns out int64 [rows]."""
+    _cuda(logits, "logits")
+    _require(logits.dtype == _HALF and logits.dim() == 2 and logits.is_contiguous(), "logits must be contiguous float16 [rows, vocab]")
+    rows, V = logits.shape
+    dev = logits.device
+    _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
+    T, K, P = _row_params(rows, dev, temperature, top_k, top_p, offsets)
+    if out is None:
+        out = torch.empty(rows, dtype=torch.int64, device=dev)
+    _require(out.dtype == torch.int64 and out.is_contiguous() and tuple(out.shape) == (rows,) and out.device == dev, "out must be contiguous int64 [rows]")
+    if rows:
+        _call(logits, lib.qs_sample_rows, out.data_ptr(), logits.data_ptr(), T.data_ptr(), K.data_ptr(), P.data_ptr(), _seed(seed), offsets.data_ptr(),
+              rows, V)
+    return out
+
+
+def tree_accept_sampling(draft_tokens, tree_mask, logits, temperature, top_k, top_p, seed: int, offsets, draft_probs: Optional[torch.Tensor] = None,
+                         accept_len: Optional[torch.Tensor] = None, path: Optional[torch.Tensor] = None, bonus: Optional[torch.Tensor] = None):
+    """Sampled acceptance of a draft tree that keeps the target distribution exactly (SpecInfer multi-step speculative sampling; for a chain,
+    Leviathan / Chen rejection sampling): the counterpart of tree_accept_greedy with the same draft_tokens int64 [B, n], tree_mask int32
+    [B, n] and outputs.  logits fp16 [B, n, V] are the verify logits; temperature / top_k / top_p per sequence as for sample_rows; offsets
+    int64 [B] advanced by one; draft_probs fp32 [B, n, V] or None: row c is the distribution q_c node c's token was drawn from (None: one-hot
+    at the draft, for deterministic drafters such as Medusa / EAGLE top-k candidates or greedy draft models; i.i.d. siblings pass the same q,
+    siblings drawn without replacement the renormalised q each came from).  From the root with p = the warped logits of node 0, child c with
+    token d is accepted iff u_c q_c(d) < p(d) (u_c: Philox draw j = c); rejection sets p <- max(p - q_c, 0) renormalised (kept if the mass is
+    0); with no child accepted the bonus is drawn from p with draw j = 0.  Greedy rows (T < 1e-5 or top_p < 1e-8) give exactly
+    tree_accept_greedy(draft, mask, argmax_rows(logits)).  Returns (accept_len int32 [B], path int32 [B, n], bonus int64 [B]), ready for
+    kv_cache_compact; the optional out tensors are written in place (CUDA-graph capture)."""
+    for t, nm in ((draft_tokens, "draft_tokens"), (tree_mask, "tree_mask")):
+        _cuda(t, nm)
+        _require(t.dim() == 2 and t.is_contiguous() and t.device == draft_tokens.device, f"{nm} must be a contiguous [B, n] tensor on one device")
+    _require(draft_tokens.dtype == torch.int64 and tree_mask.dtype == torch.int32, "draft_tokens must be int64, tree_mask int32")
+    B, n = draft_tokens.shape
+    dev = draft_tokens.device
+    _require(tuple(tree_mask.shape) == (B, n), "draft_tokens and tree_mask must have one shape")
+    _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
+    _cuda(logits, "logits")
+    _require(logits.dtype == _HALF and logits.dim() == 3 and logits.is_contiguous() and tuple(logits.shape[:2]) == (B, n) and logits.device == dev,
+             "logits must be contiguous float16 [B, n, vocab] on the device of the drafts")
+    V = logits.size(2)
+    _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
+    if draft_probs is not None:
+        _cuda(draft_probs, "draft_probs")
+        _require(draft_probs.dtype == torch.float32 and draft_probs.is_contiguous() and tuple(draft_probs.shape) == (B, n, V) and draft_probs.device == dev,
+                 "draft_probs must be contiguous float32 [B, n, vocab]")
+    T, K, P = _row_params(B, dev, temperature, top_k, top_p, offsets)
+    accept_len = torch.empty(B, dtype=torch.int32, device=dev) if accept_len is None else accept_len
+    path = torch.empty((B, n), dtype=torch.int32, device=dev) if path is None else path
+    bonus = torch.empty(B, dtype=torch.int64, device=dev) if bonus is None else bonus
+    for t, n_, dt, shape in ((accept_len, "accept_len", torch.int32, (B,)), (path, "path", torch.int32, (B, n)), (bonus, "bonus", torch.int64, (B,))):
+        _require(t.device == dev and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, f"{n_} must be contiguous {dt} {shape}")
+    if B:
+        _call(draft_tokens, lib.qs_tree_accept_sampling, draft_tokens.data_ptr(), tree_mask.data_ptr(), logits.data_ptr(),
+              draft_probs.data_ptr() if draft_probs is not None else None, T.data_ptr(), K.data_ptr(), P.data_ptr(), _seed(seed), offsets.data_ptr(),
+              accept_len.data_ptr(), path.data_ptr(), bonus.data_ptr(), B, n, V)
+    return accept_len, path, bonus
+
+
 class PeerContext:
     """Peer-mapped buffers of a tensor-parallel group for the fused all-reduce (qs_add_rms_norm_general_peer): built once from
     torch.distributed._symmetric_memory (device memory + NVLink peer mappings are torch's plumbing; the kernel is ours).

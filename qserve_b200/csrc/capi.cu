@@ -267,6 +267,27 @@ int qs_kv_cache_compact(const int64_t* kv_pointers, const int32_t* start_pos, co
   return kv_cache_compact(a);
 }
 
+int qs_sample_rows(int64_t* out, const void* logits, const float* temperature, const int32_t* top_k, const float* top_p, uint64_t seed,
+                   int64_t* offsets, int rows, int vocab, void* stream) {
+  QS_REQUIRE(logits == nullptr || aligned16(logits), "sample_rows: logits must be 16-byte aligned");
+  SampleArgs a;
+  a.out = reinterpret_cast<long long*>(out); a.logits = logits; a.temperature = temperature; a.top_k = top_k; a.top_p = top_p;
+  a.offsets = reinterpret_cast<long long*>(offsets); a.seed = seed; a.rows = rows; a.vocab = vocab; a.stream = stream;
+  return sample_rows(a);
+}
+
+int qs_tree_accept_sampling(const int64_t* draft_tokens, const int32_t* tree_mask, const void* logits, const float* draft_probs,
+                            const float* temperature, const int32_t* top_k, const float* top_p, uint64_t seed, int64_t* offsets, int32_t* accept_len,
+                            int32_t* path, int64_t* bonus, int batch, int num_nodes, int vocab, void* stream) {
+  QS_REQUIRE(logits == nullptr || aligned16(logits), "tree_accept_sampling: logits must be 16-byte aligned");
+  TreeAcceptSamplingArgs a;
+  a.draft = reinterpret_cast<const long long*>(draft_tokens); a.tree_mask = tree_mask; a.logits = logits; a.draft_probs = draft_probs;
+  a.temperature = temperature; a.top_k = top_k; a.top_p = top_p; a.offsets = reinterpret_cast<long long*>(offsets); a.seed = seed;
+  a.accept_len = accept_len; a.path = path; a.bonus = reinterpret_cast<long long*>(bonus);
+  a.batch = batch; a.num_nodes = num_nodes; a.vocab = vocab; a.stream = stream;
+  return tree_accept_sampling(a);
+}
+
 int qs_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
                          int64_t out_stride, const int32_t* cu_seqlens, int batch, int num_tokens, int max_seqlen, int num_heads, int num_kv_heads,
                          int head_dim, float softmax_scale, void* stream) {

@@ -50,6 +50,15 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// argmax order of (value, index) pairs: torch.argmax semantics, NaN counts as the maximum and the first maximal index wins
+// (argmax_rows, and the greedy rows of sample_rows / tree_accept_sampling)
+__device__ __forceinline__ bool argmax_better(float v, int i, float bv, int bi) {
+  const bool vn = (v != v), bn = (bv != bv);
+  if (vn != bn) return vn;
+  if (vn) return i < bi;
+  return v > bv || (v == bv && i < bi);
+}
+
 // Programmatic dependent launch (PDL)
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

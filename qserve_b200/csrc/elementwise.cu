@@ -905,12 +905,6 @@ __global__ void __launch_bounds__(kThreads) dequant_silu_and_mul_quant_kernel(in
 // distributed shared memory.  First maximal index wins, NaN counts as the maximum (torch semantics).
 // ---------------------------------------------------------------------------------------------
 constexpr int kArgmaxCluster = 8;
-__device__ __forceinline__ bool argmax_better(float v, int i, float bv, int bi) {
-  const bool vn = (v != v), bn = (bv != bv);
-  if (vn != bn) return vn;
-  if (vn) return i < bi;
-  return v > bv || (v == bv && i < bi);
-}
 __global__ void __launch_bounds__(kThreads) argmax_rows_kernel(long long* __restrict__ out, const __half* __restrict__ logits, int V) {
   __shared__ float s_v[kThreads / 32];
   __shared__ int s_i[kThreads / 32];

@@ -175,4 +175,36 @@ struct KvCompactArgs {
 };
 int kv_cache_compact(const KvCompactArgs& a);
 
+// sampling.cu: temperature / top-p / top-k sampling of fp16 logits and sampled (lossless) acceptance of draft trees; Philox4x32-10 draws
+// keyed by `seed` and counted by the per-row `offsets`, which every call advances by one
+struct SampleArgs {
+  long long* out = nullptr;            // int64 [rows]
+  const void* logits = nullptr;        // fp16 [rows, vocab]
+  const float* temperature = nullptr;  // [rows]
+  const int* top_k = nullptr;          // [rows], -1 disables
+  const float* top_p = nullptr;        // [rows]
+  long long* offsets = nullptr;        // [rows], read and advanced by one
+  unsigned long long seed = 0;
+  int rows = 0, vocab = 0;
+  void* stream = nullptr;
+};
+int sample_rows(const SampleArgs& a);
+struct TreeAcceptSamplingArgs {
+  const long long* draft = nullptr;    // [batch, num_nodes]
+  const int* tree_mask = nullptr;      // [batch, num_nodes] ancestor words
+  const void* logits = nullptr;        // fp16 [batch, num_nodes, vocab]
+  const float* draft_probs = nullptr;  // optional fp32 [batch, num_nodes, vocab]; null: one-hot at the draft token
+  const float* temperature = nullptr;  // [batch]
+  const int* top_k = nullptr;
+  const float* top_p = nullptr;
+  long long* offsets = nullptr;        // [batch], read and advanced by one
+  unsigned long long seed = 0;
+  int* accept_len = nullptr;           // [batch]
+  int* path = nullptr;                 // [batch, num_nodes]
+  long long* bonus = nullptr;          // [batch]
+  int batch = 0, num_nodes = 0, vocab = 0;
+  void* stream = nullptr;
+};
+int tree_accept_sampling(const TreeAcceptSamplingArgs& a);
+
 }  // namespace qs

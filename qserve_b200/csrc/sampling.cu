@@ -1,0 +1,566 @@
+// qserve_b200 -- temperature / top-p / top-k sampling of fp16 logits and lossless sampled acceptance of draft trees, sm_90a.
+//
+// sample_rows_kernel: one token per row of fp16 logits [rows, V].  One cluster of 8 CTAs per row (the argmax_rows pattern); each CTA copies
+// its V / 8 slice into shared memory once and every later pass reads it there.
+//   * greedy rows (T < 1e-5 or top_p < 1e-8) and rows without a finite logit return what argmax_rows returns;
+//   * otherwise z = x / T (IEEE fp32), w = exp(z - max z), NaN and -inf logits have weight 0.  The kept set is {key >= max(tau_p, tau_k)}
+//     on the order-preserving 16-bit key of the fp16 logit: tau_k is the k-th largest key (radix select: a 256-bin count histogram of the
+//     high byte, then of the low byte inside the selected bin, summed through distributed shared memory), tau_p the smallest key whose
+//     strictly-larger weight is < top_p * sum w (the same two-level histogram over weights, restricted to keys >= tau_k);
+//   * the token is drawn by inverse CDF in index order: an ordered prefix of the per-CTA kept sums selects the CTA that holds u * S, and
+//     a block scan over contiguous per-thread ranges selects the token inside it.
+// Every weight sum is accumulated in 64-bit fixed point (40 fractional bits, w <= 1): integer addition is associative, so histograms built
+// with shared-memory atomics are exact and a call is bitwise deterministic.  Quantising each weight to 2^-41 moves a CDF by at most
+// V * 2^-41 <= 1e-7 of the largest weight, far below the fp32 exp error the tests allow for.
+//
+// Random numbers: Philox4x32-10, counter (lo(off), hi(off), row, j), key (lo(seed), hi(seed)), u = (x0 >> 8) * 2^-24; off = offsets[row],
+// which the call advances by one.  Counter-based and per row: a CUDA-graph replay draws fresh numbers and no cross-CTA atomics are needed.
+//
+// tree_accept_sampling_kernel: the sampled counterpart of tree_accept_greedy (SpecInfer multi-step speculative sampling; Leviathan / Chen
+// rejection sampling for a chain).  One cluster per sequence keeps the current target distribution p (unnormalised fp32, one V / 8 slice per
+// CTA) in shared memory.  At each node the children are tried in index order: child c with token d is accepted iff u_c * q_c(d) < p(d)
+// (u_c: draw j = c); on rejection p <- max(p - q_c, 0) (one pass over p and q_c plus a cluster reduction; for one-hot q_c only p(d) is
+// zeroed).  With no child accepted the bonus token is drawn from p with draw j = 0.  Greedy rows keep p one-hot at the argmax, which makes
+// the result exactly tree_accept_greedy(draft, mask, argmax_rows(logits)).
+//
+// Both kernels read everything a preceding kernel may write (logits, drafts, mask, parameters, offsets) after griddepcontrol.wait, need no
+// host synchronisation and can be captured in a CUDA graph.
+#include "common.cuh"
+#include "launch.h"
+
+namespace qs {
+namespace {
+
+using u64 = unsigned long long;
+
+constexpr int kCluster = 8;
+constexpr int kThreads = 256;
+constexpr int kWarps = kThreads / 32;
+constexpr int kMaxVocab = 196608;  // 24576 logits per CTA: 48 KB of fp16 (+ 96 KB of fp32 p in the tree kernel)
+constexpr int kMaxNodes = 16;
+constexpr float kFix = 1099511627776.f;  // 2^40: fixed-point scale of the weight sums
+
+// ------------------------------------------------------------------------------------------------
+// small device helpers
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+template <typename T>
+__device__ __forceinline__ T* peer(T* p, int rank) {  // the same shared-memory variable in CTA `rank` of the cluster (generic address)
+  uint64_t out;
+  asm volatile("mapa.u64 %0, %1, %2;" : "=l"(out) : "l"(reinterpret_cast<uint64_t>(p)), "r"(rank));
+  return reinterpret_cast<T*>(out);
+}
+
+// Philox4x32-10, first output word
+__device__ __forceinline__ uint32_t philox_x0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+    c0 = hi1 ^ c1 ^ k0;
+    c1 = lo1;
+    c2 = hi0 ^ c3 ^ k1;
+    c3 = lo0;
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c0;
+}
+// u in [0, 1 - 2^-24], exact in fp32
+__device__ __forceinline__ float uniform(u64 seed, long long off, int row, int j) {
+  const u64 o = static_cast<u64>(off);
+  const uint32_t x = philox_x0(static_cast<uint32_t>(o), static_cast<uint32_t>(o >> 32), static_cast<uint32_t>(row), static_cast<uint32_t>(j),
+                               static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  return __uint2float_rn(x >> 8) * 5.9604644775390625e-8f;
+}
+
+// order-preserving 16-bit key of an fp16 logit, and its inverse
+__device__ __forceinline__ uint32_t okey(uint32_t b) { return (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u); }
+__device__ __forceinline__ uint32_t key_bits(uint32_t k) { return (k & 0x8000u) ? (k & 0x7fffu) : (~k & 0xffffu); }
+__device__ __forceinline__ bool valid_bits(uint32_t b) { return (b & 0x7fffu) <= 0x7c00u && b != 0xfc00u; }  // neither NaN nor -inf
+
+__device__ __forceinline__ float weight(uint32_t b, float T, float mz) {
+  const float z = __fdiv_rn(__half2float(__ushort_as_half(static_cast<unsigned short>(b))), T);
+  return z == mz ? 1.f : expf(__fsub_rn(z, mz));
+}
+__device__ __forceinline__ u64 fix(float w) { return __float2ull_rn(__fmul_rn(w, kFix)); }
+
+struct Smem {
+  u64 hist[256];
+  u64 red[kWarps];
+  u64 part[2];      // this CTA's published value (alternating slots: one cluster barrier per gather)
+  int sel;
+  u64 sel_above;
+  int tok;
+  int2 arg[kWarps];
+};
+
+template <typename T, typename Op>
+__device__ __forceinline__ T block_reduce(T v, T* red, Op op) {
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, m));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  T r = red[0];
+#pragma unroll
+  for (int w = 1; w < kWarps; ++w) r = op(r, red[w]);  // fixed order
+  __syncthreads();
+  return r;
+}
+struct OpAdd { __device__ u64 operator()(u64 a, u64 b) const { return a + b; } };
+struct OpMax { __device__ u64 operator()(u64 a, u64 b) const { return a > b ? a : b; } };
+
+// exclusive prefix over the threads of the block in thread order
+__device__ __forceinline__ u64 block_excl_scan(u64 v, u64* red) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  u64 inc = v;
+#pragma unroll
+  for (int m = 1; m < 32; m <<= 1) {
+    const u64 o = __shfl_up_sync(0xffffffffu, inc, m);
+    if (lane >= m) inc += o;
+  }
+  if (lane == 31) red[w] = inc;
+  __syncthreads();
+  u64 off = 0;
+  for (int i = 0; i < w; ++i) off += red[i];
+  __syncthreads();
+  return off + inc - v;
+}
+
+// publish one value per CTA and read all of them, in rank order, in every thread
+__device__ __forceinline__ void gather(Smem& s, int& phase, u64 mine, u64 (&all)[kCluster]) {
+  if (threadIdx.x == 0) s.part[phase] = mine;
+  cluster_sync();
+#pragma unroll
+  for (int r = 0; r < kCluster; ++r) all[r] = *peer(&s.part[phase], r);
+  phase ^= 1;
+}
+
+// Sum the 256-bin histograms of the cluster and select a bin, scanning from the top: COUNT: the bin holding the k-th largest key;
+// WEIGHT: the lowest non-empty bin whose strictly-higher weight plus `base` is < thr.  Returns the bin and the total above it.
+template <bool COUNT>
+__device__ __forceinline__ int hist_select(Smem& s, u64 k, u64 base, double thr, u64& above_out) {
+  cluster_sync();  // every CTA's histogram is complete
+  const int t = threadIdx.x, bin = 255 - t;  // thread order = descending bins
+  u64 tot = 0;
+#pragma unroll
+  for (int r = 0; r < kCluster; ++r) tot += peer(s.hist, r)[bin];
+  if (t == 0) s.sel = -1;
+  const u64 above = block_excl_scan(tot, s.red);  // has a __syncthreads after the write of s.sel
+  bool hit;
+  if (COUNT)
+    hit = above < k && k <= above + tot;
+  else
+    hit = tot > 0 && static_cast<double>(base + above) < thr;
+  if (hit) atomicMax(&s.sel, t);  // COUNT: exactly one thread; WEIGHT: the hits are a prefix of the threads, take the lowest bin
+  __syncthreads();
+  if (t == s.sel) s.sel_above = above;
+  __syncthreads();
+  const int sel = s.sel;
+  above_out = s.sel_above;
+  cluster_sync();  // the peers are done reading this histogram
+  return 255 - sel;
+}
+
+__device__ __forceinline__ void zero_hist(Smem& s) {
+  s.hist[threadIdx.x] = 0;
+  __syncthreads();
+}
+
+// argmax_rows over the cluster (the same (value, index) order), result in every thread
+__device__ __forceinline__ int cluster_argmax(Smem& s, int& phase, const __half* xs, int n_loc, int g0) {
+  float best = __int_as_float(0xff800000);
+  int bi = 0x7fffffff;
+  for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+    const float f = __half2float(xs[i]);
+    if (argmax_better(f, g0 + i, best, bi)) { best = f; bi = g0 + i; }
+  }
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, m);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, m);
+    if (argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
+  }
+  if ((threadIdx.x & 31) == 0) s.arg[threadIdx.x >> 5] = make_int2(__float_as_int(best), bi);
+  __syncthreads();
+  best = __int_as_float(s.arg[0].x);
+  bi = s.arg[0].y;
+  for (int w = 1; w < kWarps; ++w)
+    if (argmax_better(__int_as_float(s.arg[w].x), s.arg[w].y, best, bi)) { best = __int_as_float(s.arg[w].x); bi = s.arg[w].y; }
+  __syncthreads();
+  u64 all[kCluster];
+  gather(s, phase, (static_cast<u64>(static_cast<uint32_t>(__float_as_int(best))) << 32) | static_cast<uint32_t>(bi), all);
+  best = __int_as_float(static_cast<int>(all[0] >> 32));
+  bi = static_cast<int>(all[0] & 0xffffffffu);
+#pragma unroll
+  for (int r = 1; r < kCluster; ++r) {
+    const float v = __int_as_float(static_cast<int>(all[r] >> 32));
+    const int i = static_cast<int>(all[r] & 0xffffffffu);
+    if (argmax_better(v, i, best, bi)) { best = v; bi = i; }
+  }
+  return bi;
+}
+
+struct Warped {
+  bool greedy;   // greedy row or no finite logit: the answer is `argmax`
+  int argmax;
+  uint32_t tau;  // kept: valid keys >= tau
+  float T, mz;   // weights: weight(bits, T, mz)
+};
+
+// Steps 1-5 of the sampling contract for the row slice xs[0 .. n_loc) (global index g0 + i); uniform over the cluster.
+__device__ __forceinline__ Warped warp_row(Smem& s, int& phase, const __half* xs, int n_loc, int g0, float T, int top_k, float top_p) {
+  Warped r;
+  r.T = T;
+  r.tau = 0;
+  r.mz = 0.f;
+  r.argmax = 0;
+  const uint16_t* xb = reinterpret_cast<const uint16_t*>(xs);
+  u64 mk = 0, cnt = 0;
+  for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+    const uint32_t b = xb[i];
+    if (valid_bits(b)) {
+      mk = max(mk, static_cast<u64>(okey(b)));
+      ++cnt;
+    }
+  }
+  mk = block_reduce(mk, s.red, OpMax());
+  cnt = block_reduce(cnt, s.red, OpAdd());
+  u64 all[kCluster];
+  gather(s, phase, (mk << 40) | cnt, all);
+  mk = 0;
+  cnt = 0;
+#pragma unroll
+  for (int q = 0; q < kCluster; ++q) {
+    mk = max(mk, all[q] >> 40);
+    cnt += all[q] & ((1ull << 40) - 1);
+  }
+  r.greedy = T < 1e-5f || top_p < 1e-8f || cnt == 0;
+  if (r.greedy) {
+    r.argmax = cluster_argmax(s, phase, xs, n_loc, g0);
+    return r;
+  }
+  const uint32_t kmax = static_cast<uint32_t>(mk);
+  r.mz = __fdiv_rn(__half2float(__ushort_as_half(static_cast<unsigned short>(key_bits(kmax)))), T);
+  if (top_k == 1) {
+    r.tau = kmax;
+  } else if (top_k > 1 && static_cast<u64>(top_k) < cnt) {  // radix select of the k-th largest key
+    u64 above;
+    zero_hist(s);
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t b = xb[i];
+      if (valid_bits(b)) atomicAdd(&s.hist[okey(b) >> 8], 1ull);
+    }
+    const int hi = hist_select<true>(s, static_cast<u64>(top_k), 0, 0.0, above);
+    zero_hist(s);
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t b = xb[i];
+      if (valid_bits(b) && static_cast<int>(okey(b) >> 8) == hi) atomicAdd(&s.hist[okey(b) & 255u], 1ull);
+    }
+    const int lo = hist_select<true>(s, static_cast<u64>(top_k) - above, 0, 0.0, above);
+    r.tau = static_cast<uint32_t>(hi << 8 | lo);
+  }
+  if (top_p < 1.f) {  // the two-level histogram of fixed-point weights over the keys >= tau_k; every valid weight counts towards the total
+    zero_hist(s);
+    u64 tot = 0;
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t b = xb[i];
+      if (valid_bits(b)) {
+        const u64 f = fix(weight(b, T, r.mz));
+        tot += f;
+        const uint32_t k = okey(b);
+        if (k >= r.tau && f) atomicAdd(&s.hist[k >> 8], f);
+      }
+    }
+    tot = block_reduce(tot, s.red, OpAdd());
+    gather(s, phase, tot, all);
+    tot = 0;
+#pragma unroll
+    for (int q = 0; q < kCluster; ++q) tot += all[q];
+    const double thr = static_cast<double>(top_p) * static_cast<double>(tot);
+    u64 above_hi, above_lo;
+    const int hi = hist_select<false>(s, 0, 0, thr, above_hi);
+    zero_hist(s);
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t b = xb[i];
+      if (!valid_bits(b)) continue;
+      const uint32_t k = okey(b);
+      if (static_cast<int>(k >> 8) == hi && k >= r.tau) {
+        const u64 f = fix(weight(b, T, r.mz));
+        if (f) atomicAdd(&s.hist[k & 255u], f);
+      }
+    }
+    const int lo = hist_select<false>(s, 0, above_hi, thr, above_lo);
+    r.tau = max(r.tau, static_cast<uint32_t>(hi << 8 | lo));
+  }
+  return r;
+}
+
+__device__ __forceinline__ u64 kept_fix(uint32_t b, const Warped& w) {
+  return (valid_bits(b) && okey(b) >= w.tau) ? fix(weight(b, w.T, w.mz)) : 0ull;
+}
+
+// Step 6: the smallest index t with sum_{j <= t} val(j) > u * S.  `mine` is this CTA's sum of val; returns the token in the CTA that
+// holds it and -1 in the others.
+template <typename Val>
+__device__ __forceinline__ int cluster_draw(Smem& s, int& phase, Val val, int n_loc, int g0, u64 mine, float u, int rank) {
+  u64 all[kCluster];
+  gather(s, phase, mine, all);
+  u64 pre = 0, S = 0;
+#pragma unroll
+  for (int q = 0; q < kCluster; ++q) {
+    if (q < rank) pre += all[q];
+    S += all[q];
+  }
+  const u64 target = static_cast<u64>(static_cast<double>(u) * static_cast<double>(S));  // < S: u <= 1 - 2^-24 and S >= 2^40
+  if (!(pre <= target && target < pre + mine)) return -1;  // uniform over the CTA; true in exactly one CTA
+  const u64 t = target - pre;
+  const int per = (n_loc + kThreads - 1) / kThreads;
+  const int i0 = min(static_cast<int>(threadIdx.x) * per, n_loc), i1 = min(i0 + per, n_loc);
+  u64 sum = 0;
+  for (int i = i0; i < i1; ++i) sum += val(i);
+  const u64 ex = block_excl_scan(sum, s.red);
+  if (ex <= t && t < ex + sum) {
+    u64 c = ex;
+    for (int i = i0; i < i1; ++i) {
+      c += val(i);
+      if (c > t) {
+        s.tok = g0 + i;
+        break;
+      }
+    }
+  }
+  __syncthreads();
+  return s.tok;
+}
+
+// copy this CTA's slice of an fp16 row into shared memory (128-bit loads)
+__device__ __forceinline__ void load_slice(__half* xs, const __half* row, int v0, int v1) {
+  const uint4* src = reinterpret_cast<const uint4*>(row) + v0;
+  uint4* dst = reinterpret_cast<uint4*>(xs);
+  for (int i = threadIdx.x; i < v1 - v0; i += kThreads) dst[i] = __ldg(src + i);
+  __syncthreads();
+}
+
+__device__ __forceinline__ void slice_of(int V, int rank, int& v0, int& v1) {
+  const int nvec = V / 8;  // V % 8 == 0 (checked on the host)
+  v0 = static_cast<int>((static_cast<long long>(nvec) * rank) / kCluster);
+  v1 = static_cast<int>((static_cast<long long>(nvec) * (rank + 1)) / kCluster);
+}
+
+__global__ void __launch_bounds__(kThreads, 1) sample_rows_kernel(long long* __restrict__ out, const __half* __restrict__ logits,
+                                                               const float* __restrict__ temperature, const int* __restrict__ top_k,
+                                                               const float* __restrict__ top_p, u64 seed, long long* __restrict__ offsets, int V) {
+  extern __shared__ uint4 dyn[];
+  __shared__ Smem s;
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // logits, parameters and offsets may come from the preceding kernels
+  const int row = blockIdx.x / kCluster, rank = blockIdx.x % kCluster;
+  int v0, v1;
+  slice_of(V, rank, v0, v1);
+  const int n_loc = (v1 - v0) * 8, g0 = v0 * 8;
+  __half* xs = reinterpret_cast<__half*>(dyn);
+  const long long off = offsets[row];
+  const float T = temperature[row], tp = top_p[row];
+  const int tk = top_k[row];
+  load_slice(xs, logits + static_cast<size_t>(row) * V, v0, v1);
+  int phase = 0;
+  const Warped w = warp_row(s, phase, xs, n_loc, g0, T, tk, tp);
+  if (w.greedy) {
+    if (rank == 0 && threadIdx.x == 0) out[row] = w.argmax;
+  } else {
+    const uint16_t* xb = reinterpret_cast<const uint16_t*>(xs);
+    u64 mine = 0;
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) mine += kept_fix(xb[i], w);
+    mine = block_reduce(mine, s.red, OpAdd());
+    const int tok = cluster_draw(s, phase, [&](int i) { return kept_fix(xb[i], w); }, n_loc, g0, mine, uniform(seed, off, row, 0), rank);
+    if (tok >= 0 && threadIdx.x == 0) out[row] = tok;
+  }
+  cluster_sync();  // every CTA has read `off` and is done with its peers' shared memory
+  if (rank == 0 && threadIdx.x == 0) offsets[row] = off + 1;
+}
+
+__global__ void __launch_bounds__(kThreads, 1) tree_accept_sampling_kernel(
+    const long long* __restrict__ draft, const int* __restrict__ tree_mask, const __half* __restrict__ logits, const float* __restrict__ draft_probs,
+    const float* __restrict__ temperature, const int* __restrict__ top_k, const float* __restrict__ top_p, u64 seed, long long* __restrict__ offsets,
+    int* __restrict__ accept_len, int* __restrict__ path, long long* __restrict__ bonus, int n, int V, int slice_cap) {
+  extern __shared__ uint4 dyn[];
+  __shared__ Smem s;
+  __shared__ long long s_draft[kMaxNodes];
+  __shared__ int s_parent[kMaxNodes], s_path[kMaxNodes];
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // logits, drafts, mask, q, parameters and offsets may come from the preceding kernels
+  const int b = blockIdx.x / kCluster, rank = blockIdx.x % kCluster;
+  int v0, v1;
+  slice_of(V, rank, v0, v1);
+  const int n_loc = (v1 - v0) * 8, g0 = v0 * 8;
+  __half* xs = reinterpret_cast<__half*>(dyn);
+  float* ps = reinterpret_cast<float*>(xs + slice_cap);
+  const long long off = offsets[b];
+  const float T = temperature[b], tp = top_p[b];
+  const int tk = top_k[b];
+  const size_t row0 = static_cast<size_t>(b) * n;
+  if (threadIdx.x < kMaxNodes) {
+    const int c = threadIdx.x;
+    const uint32_t anc = (c < n && c > 0) ? static_cast<uint32_t>(tree_mask[row0 + c]) & ((1u << c) - 1u) : 0u;
+    s_draft[c] = c < n ? draft[row0 + c] : -1;
+    s_parent[c] = anc ? 31 - __clz(anc) : -1;  // the root and parentless nodes are never a child
+  }
+  int phase = 0;
+  Warped w;
+  u64 mine = 0, S = 0;
+  auto enter = [&](int node) {  // p <- warp(logits[b, node])
+    load_slice(xs, logits + (row0 + node) * V, v0, v1);
+    w = warp_row(s, phase, xs, n_loc, g0, T, tk, tp);
+    if (w.greedy) return;
+    const uint16_t* xb = reinterpret_cast<const uint16_t*>(xs);
+    u64 m = 0;
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t bb = xb[i];
+      const float p = (valid_bits(bb) && okey(bb) >= w.tau) ? weight(bb, w.T, w.mz) : 0.f;
+      ps[i] = p;
+      m += fix(p);
+    }
+    mine = block_reduce(m, s.red, OpAdd());
+    u64 all[kCluster];
+    gather(s, phase, mine, all);  // also publishes ps to the peers
+    S = 0;
+#pragma unroll
+    for (int q = 0; q < kCluster; ++q) S += all[q];
+  };
+  enter(0);
+  int cur = 0, len = 1;
+  if (threadIdx.x == 0) s_path[0] = 0;
+  for (;;) {
+    int next = -1;
+    for (int c = cur + 1; c < n; ++c) {
+      if (s_parent[c] != cur) continue;
+      const long long d = s_draft[c];
+      if (d < 0 || d >= V) continue;  // padding / out of range: never accepted, p unchanged
+      const int di = static_cast<int>(d);
+      if (w.greedy) {
+        if (di == w.argmax) { next = c; break; }
+        continue;
+      }
+      const float u = uniform(seed, off, b, c);
+      const float* qrow = draft_probs ? draft_probs + (row0 + c) * V : nullptr;
+      const float qd = qrow ? qrow[di] : 1.f;
+      int owner = kCluster - 1, ov0, ov1;
+      for (int q = 0; q < kCluster - 1; ++q) {
+        slice_of(V, q, ov0, ov1);
+        if (di < ov1 * 8) {
+          owner = q;
+          break;
+        }
+      }
+      slice_of(V, owner, ov0, ov1);
+      const float pd = *peer(ps + (di - ov0 * 8), owner);
+      // p(d) = pd / (S 2^-40): accept iff u q(d) < p(d)
+      if (static_cast<double>(u) * static_cast<double>(qd) * (static_cast<double>(S) * 9.094947017729282e-13) < static_cast<double>(pd)) {
+        next = c;
+        break;
+      }
+      cluster_sync();  // every CTA has read pd: p may change
+      if (!qrow) {     // one-hot q: p - q only loses p(d)
+        if (rank == owner) {
+          if (threadIdx.x == 0) ps[di - g0] = 0.f;
+          mine -= fix(pd);
+        }
+        u64 all[kCluster];
+        gather(s, phase, mine, all);
+        S = 0;
+#pragma unroll
+    for (int q = 0; q < kCluster; ++q) S += all[q];
+      } else {  // p <- max(p / R - q, 0); kept as is when the residual mass is 0
+        const float inv = static_cast<float>(1099511627776.0 / static_cast<double>(S));
+        const float* qs = qrow + g0;
+        u64 m = 0;
+        for (int i = threadIdx.x; i < n_loc; i += kThreads) m += fix(fmaxf(__fsub_rn(__fmul_rn(ps[i], inv), __ldg(qs + i)), 0.f));
+        m = block_reduce(m, s.red, OpAdd());
+        u64 all[kCluster];
+        gather(s, phase, m, all);
+        u64 M = 0;
+#pragma unroll
+    for (int q = 0; q < kCluster; ++q) M += all[q];
+        if (M > 0) {
+          for (int i = threadIdx.x; i < n_loc; i += kThreads) ps[i] = fmaxf(__fsub_rn(__fmul_rn(ps[i], inv), __ldg(qs + i)), 0.f);
+          mine = m;
+          S = M;
+          cluster_sync();  // the new p is visible to the peers
+        }
+      }
+    }
+    if (next < 0) break;
+    cur = next;
+    if (threadIdx.x == 0) s_path[len] = cur;
+    ++len;
+    cluster_sync();  // the peers are done reading this CTA's p
+    enter(cur);
+  }
+  if (w.greedy) {
+    if (rank == 0 && threadIdx.x == 0) bonus[b] = w.argmax;
+  } else {
+    const int tok = cluster_draw(s, phase, [&](int i) { return fix(ps[i]); }, n_loc, g0, mine, uniform(seed, off, b, 0), rank);
+    if (tok >= 0 && threadIdx.x == 0) bonus[b] = tok;
+  }
+  __syncthreads();
+  if (rank == 0 && threadIdx.x < n) path[row0 + threadIdx.x] = static_cast<int>(threadIdx.x) < len ? s_path[threadIdx.x] : -1;
+  if (rank == 0 && threadIdx.x == 0) accept_len[b] = len;
+  cluster_sync();  // every CTA has read `off` and is done with its peers' shared memory
+  if (rank == 0 && threadIdx.x == 0) offsets[b] = off + 1;
+}
+
+int slice_cap_of(int V) { return ((V / 8 + kCluster - 1) / kCluster) * 8; }
+
+template <typename Kern, typename... Args>
+int launch_cluster(Kern kern, int clusters, size_t smem, void* stream, const char* what, Args... args) {
+  int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), what);
+  if (rc) return rc;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(static_cast<unsigned>(clusters) * kCluster);
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = static_cast<cudaStream_t>(stream);
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  attr[1].id = cudaLaunchAttributeClusterDimension;
+  attr[1].val.clusterDim.x = kCluster;
+  attr[1].val.clusterDim.y = 1;
+  attr[1].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 2;
+  return check_cuda(cudaLaunchKernelEx(&cfg, kern, args...), what);
+}
+
+}  // namespace
+
+int sample_rows(const SampleArgs& a) {
+  QS_REQUIRE(a.rows >= 0 && a.vocab >= 8 && a.vocab % 8 == 0 && a.vocab <= kMaxVocab, "sample_rows: rows=%d vocab=%d (a multiple of 8, 8 .. %d)",
+             a.rows, a.vocab, kMaxVocab);
+  QS_REQUIRE(a.rows <= 0x7fffffff / kCluster, "sample_rows: too many rows");
+  if (a.rows == 0) return QS_OK;
+  QS_REQUIRE(a.out && a.logits && a.temperature && a.top_k && a.top_p && a.offsets, "sample_rows: null pointer");
+  const int cap = slice_cap_of(a.vocab);
+  return launch_cluster(sample_rows_kernel, a.rows, static_cast<size_t>(cap) * 2, a.stream, "sample_rows", a.out,
+                        static_cast<const __half*>(a.logits), a.temperature, a.top_k, a.top_p, static_cast<u64>(a.seed), a.offsets, a.vocab);
+}
+
+int tree_accept_sampling(const TreeAcceptSamplingArgs& a) {
+  QS_REQUIRE(a.batch >= 0 && a.num_nodes >= 1 && a.num_nodes <= kMaxNodes, "tree_accept_sampling: batch=%d, num_nodes=%d (1 .. 16)", a.batch,
+             a.num_nodes);
+  QS_REQUIRE(a.vocab >= 8 && a.vocab % 8 == 0 && a.vocab <= kMaxVocab, "tree_accept_sampling: vocab=%d (a multiple of 8, 8 .. %d)", a.vocab,
+             kMaxVocab);
+  QS_REQUIRE(a.batch <= 0x7fffffff / kCluster, "tree_accept_sampling: batch too large");
+  if (a.batch == 0) return QS_OK;
+  QS_REQUIRE(a.draft && a.tree_mask && a.logits && a.temperature && a.top_k && a.top_p && a.offsets && a.accept_len && a.path && a.bonus,
+             "tree_accept_sampling: null pointer");
+  const int cap = slice_cap_of(a.vocab);
+  return launch_cluster(tree_accept_sampling_kernel, a.batch, static_cast<size_t>(cap) * 6, a.stream, "tree_accept_sampling", a.draft, a.tree_mask,
+                        static_cast<const __half*>(a.logits), a.draft_probs, a.temperature, a.top_k, a.top_p, static_cast<u64>(a.seed), a.offsets,
+                        a.accept_len, a.path, a.bonus, a.num_nodes, a.vocab, cap);
+}
+
+}  // namespace qs

@@ -194,6 +194,13 @@ class DecodeRunner:
         self.launches_per_step = 0
         if verify_len:
             self._alloc_verify_buffers()
+        # sampling (forward(sample=True), the sampled tree verify): per-row parameters the caller edits between replays, made with torch.full
+        # (no generator draws).  Defaults: the reference ModelRunner's SamplingParams(temperature=1.0, top_p=1.0, top_k=1).
+        self.s_seed = seed
+        self.s_temperature = torch.full((batch,), 1.0, dtype=torch.float32, device=dev)
+        self.s_top_k = torch.full((batch,), 1, dtype=torch.int32, device=dev)
+        self.s_top_p = torch.full((batch,), 1.0, dtype=torch.float32, device=dev)
+        self.s_offsets = torch.full((batch,), 0, dtype=torch.int64, device=dev)
 
     # ---------------------------------------------------------------------------------------------------------
     def _norm_quant(self, x, gamma):
@@ -219,9 +226,13 @@ class DecodeRunner:
         if self.tp_size > 1 and not self.no_comm:
             torch.distributed.all_reduce(t, group=self.pg)
 
-    def forward(self, tokens: torch.Tensor) -> torch.Tensor:
-        """One decode step for `batch` sequences; returns the greedy next tokens [batch] (device)."""
-        return self._forward_fused(tokens) if self.fused else self._forward_reference(tokens)
+    def forward(self, tokens: torch.Tensor, sample: bool = False) -> torch.Tensor:
+        """One decode step for `batch` sequences; returns the greedy next tokens [batch] (device).  sample=True ends the step in sample_rows
+        with the per-row s_temperature / s_top_k / s_top_p, seed s_seed and counters s_offsets (advanced by one) instead of argmax_rows."""
+        if not sample:
+            return self._forward_fused(tokens) if self.fused else self._forward_reference(tokens)
+        logits = self._forward_fused(tokens, True) if self.fused else self._forward_reference(tokens, True)
+        return _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets)
 
     def _attention(self, li):
         cfg, D = self.cfg, self.cfg.head_dim
@@ -352,7 +363,8 @@ class DecodeRunner:
         self.v_accept_len = torch.zeros(self.batch, dtype=torch.int32, device=dev)
         self.v_path = torch.zeros(self.batch * self.verify_len, dtype=torch.int32, device=dev)  # [:B n] viewed as [B, n] for n nodes
         self.v_bonus = torch.zeros(self.batch, dtype=torch.int64, device=dev)
-        self.v_graphs = {}  # (n, tree) -> CUDA graph
+        self.v_graphs = {}  # (n, tree) -> CUDA graph; (n, True, "sampled", draft_probs) for the sampled tree step
+        self.v_draft_probs = None  # fp32 [B * verify_len * vocab], allocated by capture_verify(..., draft_probs=True)
 
     def _verify_meta(self, n: int):
         if n not in self.v_meta:
@@ -430,8 +442,29 @@ class DecodeRunner:
         _ext.kv_cache_compact(self.block_tables, self.v_start, path, acc, self.Hkv, 64, self.size_per_token, self.kv_bits == 4)
         return acc, path, bonus
 
-    def _verify_graph_body(self, n: int, tree: bool) -> None:
+    def accept_sampled_and_compact(self, tokens: torch.Tensor, tree_mask: torch.Tensor, logits: torch.Tensor, draft_probs: Optional[torch.Tensor] = None):
+        """accept_and_compact with sampled acceptance: after verify_forward(tokens, return_logits=True, tree_mask=tree_mask) returned the logits
+        [B, n, vocab], tree_accept_sampling with the runner's per-row sampling parameters (s_temperature, s_top_k, s_top_p, s_seed,
+        s_offsets advanced by one) and draft_probs (fp32 [B, n, vocab] or None: one-hot drafts), then kv_cache_compact of the accepted path.
+        Returns (accept_len, path, bonus) in v_accept_len, v_path and v_bonus."""
+        n = tokens.size(1)
+        path = self.v_path[: self.batch * n].view(self.batch, n)
+        acc, path, bonus = _ext.tree_accept_sampling(tokens.contiguous(), tree_mask.contiguous(), logits, self.s_temperature, self.s_top_k, self.s_top_p,
+                                                     self.s_seed, self.s_offsets, draft_probs, self.v_accept_len, path, self.v_bonus)
+        _ext.kv_cache_compact(self.block_tables, self.v_start, path, acc, self.Hkv, 64, self.size_per_token, self.kv_bits == 4)
+        return acc, path, bonus
+
+    def draft_probs_view(self, n: int) -> torch.Tensor:
+        """The [B, n, vocab] fp32 draft distributions the sampled tree graph for n nodes reads (capture_verify(..., draft_probs=True))."""
+        return self.v_draft_probs[: self.batch * n * self.cfg.vocab].view(self.batch, n, self.cfg.vocab)
+
+    def _verify_graph_body(self, n: int, tree: bool, sampled: bool = False, draft_probs: bool = False) -> None:
         tin, tout = self.v_tokens_in[:, :n].contiguous(), self.v_tokens_out[:, :n]
+        if sampled:
+            mask = self.v_tree_mask[:, :n].contiguous()
+            logits = self.verify_forward(tin, return_logits=True, tree_mask=mask)
+            self.accept_sampled_and_compact(tin, mask, logits, self.draft_probs_view(n) if draft_probs else None)
+            return
         if not tree:
             tout.copy_(self.verify_forward(tin))
             return
@@ -439,25 +472,33 @@ class DecodeRunner:
         tout.copy_(self.verify_forward(tin, tree_mask=mask))
         self.accept_and_compact(tin, mask, tout)
 
-    def capture_verify(self, n: int, warmup: int = 2, tree: bool = False) -> None:
+    def _verify_key(self, n: int, tree: bool, sampled: bool, draft_probs: bool):
+        return (n, True, "sampled", bool(draft_probs)) if sampled else (n, tree)
+
+    def capture_verify(self, n: int, warmup: int = 2, tree: bool = False, sampled: bool = False, draft_probs: bool = False) -> None:
         """Capture the verify step for n draft tokens in a CUDA graph: v_tokens_in[:, :n] -> v_tokens_out[:, :n].  tree=True: the graph
-        also reads v_tree_mask[:, :n] and runs accept_and_compact (v_accept_len, v_path, v_bonus).  The warm-up runs the step eagerly, so it
-        writes the draft slots (and, with tree=True, compacts them) like a replay does."""
+        also reads v_tree_mask[:, :n] and runs accept_and_compact (v_accept_len, v_path, v_bonus).  sampled=True (needs tree=True): verify
+        -> accept_sampled_and_compact -> the same outputs, with the per-row sampling parameters; draft_probs=True allocates v_draft_probs
+        (fp32 [B, verify_len, vocab], filled through draft_probs_view(n)) and reads it as q, otherwise the drafts are one-hot.  The warm-up
+        runs the step eagerly, so it writes the draft slots (and, with tree=True, compacts them) like a replay does."""
+        assert not sampled or tree, "sampled acceptance runs on the tree step (a chain is a tree with mask (1 << i) - 1)"
+        if sampled and draft_probs and self.v_draft_probs is None:
+            self.v_draft_probs = torch.zeros(self.batch * self.verify_len * self.cfg.vocab, dtype=torch.float32, device=self.dev)
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(s), torch.no_grad():
             for _ in range(warmup):
-                self._verify_graph_body(n, tree)
+                self._verify_graph_body(n, tree, sampled, draft_probs)
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         g = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(g):
-            self._verify_graph_body(n, tree)
-        self.v_graphs[(n, tree)] = g
+            self._verify_graph_body(n, tree, sampled, draft_probs)
+        self.v_graphs[self._verify_key(n, tree, sampled, draft_probs)] = g
 
-    def verify_step(self, n: int, tree: bool = False) -> None:
+    def verify_step(self, n: int, tree: bool = False, sampled: bool = False, draft_probs: bool = False) -> None:
         """Replay the captured verify step for n draft tokens."""
-        self.v_graphs[(n, tree)].replay()
+        self.v_graphs[self._verify_key(n, tree, sampled, draft_probs)].replay()
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
@@ -528,18 +569,19 @@ class DecodeRunner:
         self.context_lens.copy_(full.context_lens)
 
     # ---------------------------------------------------------------------------------------------------------
-    def capture(self, warmup: int = 2) -> None:
-        """Warm up eagerly (allocates workspaces, sets kernel attributes) and capture the whole step in a CUDA graph."""
+    def capture(self, warmup: int = 2, sample: bool = False) -> None:
+        """Warm up eagerly (allocates workspaces, sets kernel attributes) and capture the whole step in a CUDA graph.  sample=True: the step
+        ends in sample_rows (see forward); each warm-up call and each replay advances s_offsets by one."""
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(s), torch.no_grad():
             for _ in range(warmup):
-                self.tokens_out.copy_(self.forward(self.tokens_in))
+                self.tokens_out.copy_(self.forward(self.tokens_in, sample))
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         g = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(g):
-            self.tokens_out.copy_(self.forward(self.tokens_in))
+            self.tokens_out.copy_(self.forward(self.tokens_in, sample))
         self.graph = g
 
     def step(self) -> None:
