@@ -145,6 +145,27 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// mbar_wait for code that keeps wgmma.mma_async groups in flight across the wait (the GEMM mainloop): the same 10 s bound, but the
+// timeout traps without a printf.  A call anywhere in a kernel's wgmma pipeline makes ptxas serialise every wgmma of the kernel.
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  if (mbar_test_wait(bar, parity)) return;
+  uint32_t spins = 0;
+  unsigned long long t0 = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if ((++spins & 0xFFFu) == 0) {
+      unsigned long long t;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
+      if (t0 == 0) t0 = t;
+      if (t - t0 > 10000000000ull) __trap();
+    }
+  }
+}
+// arrive if `pred`: the predicate sits on the instruction, so a single-lane release adds no divergent branch to a wgmma issue sequence
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(smem_u32(bar)),
+               "r"(static_cast<uint32_t>(pred))
+               : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------
 // bulk async copies (TMA engine): 1-D linear and 2-D tiled (tensor map)

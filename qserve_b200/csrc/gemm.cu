@@ -43,6 +43,7 @@ constexpr int kBK = 128;  // K sub-block (= one g128 group, one 128-byte swizzle
 constexpr int kSub = 2;    // sub-blocks per pipeline stage: per-stage barrier latencies are amortised over 256 K
 constexpr int kConsumers = 128;  // warps 0..3: one warpgroup (unpack, wgmma, epilogue)
 constexpr int kNumThreads = 192; // + warp 4: weight producer, warp 5: activation producer
+constexpr int kFrag = 4;         // W4: wgmma pairs whose A fragments are held in registers at once (kFrag - 1 in flight)
 
 enum { kModeW4Chn = 0, kModeW4Grp = 1, kModeW8 = 2 };
 
@@ -57,7 +58,7 @@ struct GemmParams {
   int32_t* acc_out;          // optional: raw INT32 accumulators [M, N] (parity tests)
   int M, N, K;
   int m_tiles, kb_per_tile, split;
-  unsigned long long* prof;  // optional: 16 globaltimer stamps per CTA (tools/gemm_timeline.py)
+  unsigned long long* prof;  // optional: 16 globaltimer stamps per CTA (tools/gemm_timeline.py); slot 15 holds the SM id
 };
 
 // WS = depth of the WEIGHT ring in shared memory.  Weights are static, so the producer streams them before the
@@ -76,19 +77,16 @@ struct Cfg {
   static constexpr int kOffW = kOffAct + AS * kActBytes;
   static constexpr int kOffS2 = kOffW + WS * kWBytes;
   static constexpr int kPipeBytes = kOffS2 + WS * kS2Bytes;
-  static constexpr int kRedBytes = NT * kBM * 4;  // INT32 partial tile [NT][128], aliases the pipeline buffers
+  // INT32 partials, aliasing the drained pipeline buffers: S == 1: the CTA's own tile [NT][128]; split-K (cluster) launches: the receive
+  // buffer [sender][token][128 / S channels] into which every CTA of the cluster pushes (st.shared::cluster, from the accumulator registers)
+  // the partials of the channels this CTA finishes -- only after a cluster barrier has seen every CTA's mainloop drain
+  static constexpr int kRedBytes = NT * kBM * 4;
   static constexpr int kOffRow = (kPipeBytes > kRedBytes ? kPipeBytes : kRedBytes);  // float ascales[NT], asums[NT]
   static constexpr int kOffBar = kOffRow + 2 * NT * 4;
   static constexpr int kNumBars = 2 * WS + 2 * AS;
   static constexpr int kSmemBytes = kOffBar + kNumBars * 8;
-  // split-K (cluster) launches append a dedicated receive buffer: every CTA pushes its INT32 partials of the channels another
-  // CTA of the cluster finishes straight into that CTA's buffer (st.shared::cluster from the accumulator registers); the owner then sums S rows.
-  static constexpr int kOffRx = (kSmemBytes + 127) / 128 * 128;
-  static constexpr int kRxBytes = NT * kBM * 4;  // [sender][token][128 / S channels]
-  static constexpr int kSmemBytesSplit = kOffRx + kRxBytes;
-  static constexpr bool kSplitFits = kSmemBytesSplit <= 227 * 1024;
-  // two co-resident CTAs per SM for the narrow tiles (NT accumulator registers per thread; <= 113 KB of shared memory each): one CTA's
-  // prologue / epilogue overlaps the other's weight stream.  128-token tiles keep 128 accumulators per thread and run one CTA per SM.
+  // two co-resident CTAs per SM for the narrow tiles (NT accumulator registers per thread; <= 113 KB of shared memory each), split or not:
+  // one CTA's prologue / epilogue overlaps the other's weight stream.  128-token tiles keep 128 accumulators per thread and run one CTA per SM.
   static constexpr int kCtasPerSm = (NT <= 64 && kSmemBytes <= 113 * 1024) ? 2 : 1;
   static_assert(kSmemBytes <= 227 * 1024, "shared memory overflow");
 };
@@ -107,6 +105,14 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 }
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// split phases of the same barrier (every thread of every CTA arrives once, then waits once): work between them overlaps the peers
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+__device__ __forceinline__ uint32_t smid() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(r));
+  return r;
 }
 __device__ __forceinline__ uint32_t map_to_cta(uint32_t smem_addr, uint32_t rank) {
   uint32_t r;
@@ -169,7 +175,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
   const int KB = p.kb_per_tile;
   const int kb_begin = (KB * rank) / S, kb_end = (KB * (rank + 1)) / S;
   const int n_kb = kb_end - kb_begin;
-  if (threadIdx.x == 0) QS_PROF(0);
+  if (threadIdx.x == 0) {
+    QS_PROF(0);
+    if (p.prof) p.prof[blockIdx.x * 16 + 15] = smid();
+  }
   qs_trace(QS_K_GEMM, 0);
 
   if (threadIdx.x == 0) {
@@ -199,7 +208,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
       int s = 0;
       uint32_t ph = 0;  // parity of the (it / WS - 1)-th completion of wempty[s]
       for (int it = 0; it < n_kb; ++it) {
-        if (it >= WS) mbar_wait(&bar_wempty[s], ph);
+        if (it >= WS) mbar_wait_nocall(&bar_wempty[s], ph);
         mbar_expect_tx(&bar_wfull[s], C::kWStageTx);
 #pragma unroll
         for (int u = 0; u < kSub; ++u) {
@@ -226,7 +235,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
       int s = 0;
       uint32_t ph = 0;
       for (int it = 0; it < n_kb; ++it) {
-        if (it >= AS) mbar_wait(&bar_xempty[s], ph);
+        if (it >= AS) mbar_wait_nocall(&bar_xempty[s], ph);
         mbar_expect_tx(&bar_xfull[s], C::kActBytes);
 #pragma unroll
         for (int u = 0; u < kSub; ++u)
@@ -242,12 +251,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
     for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int i = 0; i < NT / 2; ++i) acc[h][i] = 0;
-    int sw = 0, sx = 0, prev_sx = 0;
+    // No divergent branch and no call may sit between a wgmma issue and its wait (ptxas would serialise every wgmma of the kernel):
+    // the first-stage stamp is taken before the loop, stage releases are predicated arrives, barrier waits trap without a printf.
+    mbar_wait_nocall(&bar_wfull[0], 0);
+    mbar_wait_nocall(&bar_xfull[0], 0);
+    if (threadIdx.x == 0) QS_PROF(4);
+    const bool leader = lane == 0;
+    int sw = 0, sx = 0, prev_sw = WS - 1, prev_sx = AS - 1;
     uint32_t phw = 0, phx = 0;
     for (int it = 0; it < n_kb; ++it) {
-      mbar_wait(&bar_wfull[sw], phw);
-      mbar_wait(&bar_xfull[sx], phx);
-      if (it == 0 && threadIdx.x == 0) QS_PROF(4);
+      mbar_wait_nocall(&bar_wfull[sw], phw);
+      mbar_wait_nocall(&bar_xfull[sx], phx);
       if constexpr (MODE == kModeW8) {
 #pragma unroll
         for (int u = 0; u < kSub; ++u) {
@@ -263,13 +277,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
         }
         // everything but this stage's kSub groups has retired: the previous stage's weight and activation buffers are free
         wgmma_wait<kSub>();
-        __syncwarp();
-        if (it > 0 && lane == 0) {
-          mbar_arrive(&bar_wempty[sw == 0 ? WS - 1 : sw - 1]);
-          mbar_arrive(&bar_xempty[prev_sx]);
-        }
+        mbar_arrive_if(&bar_wempty[prev_sw], it > 0 && leader);
+        mbar_arrive_if(&bar_xempty[prev_sx], it > 0 && leader);
       } else {
-        uint32_t fr[2][2][4];  // [buffer][wgmma h][register]: double-buffered so that unpacking overlaps the previous wgmma pair
+        // fragment registers of the last kFrag wgmma pairs [pair % kFrag][wgmma h][register]: up to kFrag - 1 pairs stay in flight
+        // while the next one is unpacked
+        uint32_t fr[kFrag][2][4];
 #pragma unroll
         for (int u = 0; u < kSub; ++u) {
           const uint64_t bdesc = gmma_desc_sw128(smem_u32(s_act + sx * C::kActBytes + u * C::kActSub));
@@ -282,6 +295,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
           }
 #pragma unroll
           for (int t = 0; t < 4; ++t) {
+            const int j = u * 4 + t;  // pair index inside the stage
             const uint4 v = *reinterpret_cast<const uint4*>(wsrc + t * 512);
             uint32_t xl = v.x & 0x0F0F0F0Fu, xh = (v.x >> 4) & 0x0F0F0F0Fu;
             uint32_t yl = v.y & 0x0F0F0F0Fu, yh = (v.y >> 4) & 0x0F0F0F0Fu;
@@ -297,14 +311,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
               xh = __vadd4(xh * s2, z2); zh = __vadd4(zh * s2, z2);   // channel c + 16
               yh = __vadd4(yh * s3, z3); wh = __vadd4(wh * s3, z3);   // channel c + 24
             }
-            // the wgmma pair that last read this fragment buffer (two pairs back) must have retired
-            wgmma_wait<1>();
-            if (u == 0 && t == 1) {
-              // ... and with it every wgmma of the previous stage: its activation buffer is free
-              __syncwarp();
-              if (it > 0 && lane == 0) mbar_arrive(&bar_xempty[prev_sx]);
-            }
-            uint32_t(&f)[2][4] = fr[t & 1];
+            // the pair that last read this fragment buffer (kFrag pairs back) must have retired
+            wgmma_wait<kFrag - 1>();
+            // once pair kFrag - 1 of the stage may be issued, every wgmma of the previous stage has retired: its activation buffer is free
+            if (j == kFrag - 1) mbar_arrive_if(&bar_xempty[prev_sx], it > 0 && leader);
+            uint32_t(&f)[2][4] = fr[j % kFrag];
             // rows lane/4 (+8) of the band's first 16 channels -> wgmma 0, of its last 16 -> wgmma 1; 32 K per fragment
             f[0][0] = xl; f[0][1] = yl; f[0][2] = zl; f[0][3] = wl;
             f[1][0] = xh; f[1][1] = yh; f[1][2] = zh; f[1][3] = wh;
@@ -314,16 +325,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
             wgmma_commit();
           }
         }
-        // the weight stage has been consumed into registers
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_wempty[sw]);
+        // the weight stage has been consumed into registers (every lane's loads fed the last, warp-aligned, wgmma)
+        mbar_arrive_if(&bar_wempty[sw], leader);
       }
+      prev_sw = sw;
       prev_sx = sx;
       if (++sw == WS) { sw = 0; phw ^= 1; }
       if (++sx == AS) { sx = 0; phx ^= 1; }
     }
     wgmma_wait<0>();
     if (threadIdx.x == 0) QS_PROF(6);
+    // split-K: the partials go into the peers' pipeline buffers, so every CTA of the cluster must have drained its rings first
+    if (S > 1) cluster_arrive();
 
     // ------------------------------------------ epilogue ------------------------------------------
     const int epi_tid = threadIdx.x;  // 0..127
@@ -334,8 +347,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
       s_asc[j] = ok ? __half2float(p.ascales[m0 + j]) : 0.f;
       if constexpr (MODE == kModeW4Chn) s_asum[j] = ok ? __half2float(p.a_ssums[m0 + j]) : 0.f;
     }
-    // every warp's wgmmas have retired before the first partial lands in the (aliased) pipeline buffers
-    named_bar_sync(1, kConsumers);
+    // every warp's wgmmas (S > 1: every CTA's in the cluster) have retired before the first partial lands in the aliased pipeline buffers
+    if (S > 1) cluster_wait(); else named_bar_sync(1, kConsumers);
     if (epi_tid == 0) QS_PROF(8);
     const int r0 = lane >> 2, c0 = (lane & 3) * 2;
     if (S == 1) {
@@ -352,7 +365,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
       // registers -> the receive buffer of the CTA that finishes this channel: rx[sender = rank][token][channel % (128 / S)].
       // Posted remote stores; the cluster barrier below publishes them.
       const int cps = kBM / S;  // channels finished per CTA
-      const uint32_t rx_base = smem_u32(smem + C::kOffRx);
+      const uint32_t rx_base = smem_u32(s_red);
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -365,6 +378,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
     }
     if (epi_tid == 0) QS_PROF(9);
   }
+  // the producer warps take part in the cluster barrier that releases the pushes above
+  if (S > 1 && threadIdx.x >= kConsumers) { cluster_arrive(); cluster_wait(); }
 
   // ---------------- cross-CTA (cluster) reduction of the INT32 partial tiles through distributed shared memory ----------------
   if (S > 1) cluster_sync_all(); else __syncthreads();
@@ -414,7 +429,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
     } else {
       // S > 1: the partials of all S senders sit in this CTA's receive buffer; sum them locally
       const int cps = kBM / S;
-      const int32_t* rx = reinterpret_cast<const int32_t*>(smem + C::kOffRx);
+      const int32_t* rx = s_red;
       const int prl = tid % npairs;  // channel pair inside this CTA's slice
       // S is a launch constant of the cluster: specialise so that all S x tokens shared-memory loads of a thread are in flight together
       auto reduce_rows = [&](auto s_tag) {
@@ -536,19 +551,45 @@ int make_tmap_w4(CUtensorMap* m, const void* ptr, uint64_t N, uint64_t K, uint32
   return QS_OK;
 }
 
-int choose_split(int tiles, int kb_per_tile, int forced) {
+// How many clusters of `s` CTAs of `kern` the device holds at once (s == 1: CTAs): the occupancy API's answer for the exact launch
+// configuration -- clusters must fit inside one GPC, so this is less than (SMs x CTAs per SM) / s.
+int resident_clusters(const void* kern, int smem, int s) {
+  int n = 0;
+  if (s == 1) {
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kNumThreads, smem) != cudaSuccess) n = 0;
+    return n * num_sms();
+  }
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(s);
+  cfg.blockDim = dim3(kNumThreads);
+  cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = s;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) n = 0;
+  return n;
+}
+
+// Split-K plan.  Automatic: the largest S in {1, 2, 4, 8} that leaves every CTA >= 2 pipeline stages and keeps all `tiles` clusters
+// resident at once (resident(s) = the occupancy API's answer), so the launch is one wave by construction.  `forced` (tests, tuning)
+// is taken as given, halved only until every CTA has a stage.
+// Measured on an H100 80GB HBM3 (700 W, 1980 MHz max SM clock), Llama-3-8B W4A8 at M = 64, us per launch over all 32 layers in a
+// CUDA graph (tools/gemm_split_sweep.py), S = 1 / 2 / 4 / 8:  qkv 14.75 / 13.08 / 13.37 / 23.57,  o 13.31 / 11.31 / 11.45 / 20.40,
+// gate_up 26.95 / 35.73 / 50.27 / 90.83,  down 33.95 / 24.13 / 19.94 / 28.94.  The plan picks 4, 4, 1, 4: 32 clusters of 8 do not fit
+// (30 resident), so S = 8 is a second wave; where S = 2 and S = 4 are both one wave they are within 2 %.
+template <typename Resident>
+int choose_split(int tiles, int kb_per_tile, int forced, Resident resident) {
   int s = 1;
   if (forced > 0) {
     s = forced;
   } else {
-    const int sms = num_sms();
-    // smallest power of two that brings the CTA count to >= ~2/3 of the SMs; every CTA keeps >= 2 k-blocks
-    while (s < 8 && tiles * s < (2 * sms) / 3 && kb_per_tile / (2 * s) >= 1) s *= 2;
+    while (s < 8 && kb_per_tile >= 4 * s && tiles <= resident(2 * s)) s *= 2;
   }
-  if (s > 8) s = 8;
   while (s > 1 && kb_per_tile < s) s /= 2;
-  // split launches carry a receive buffer and run one CTA per SM: never more CTAs than SMs (a second wave costs more than it saves)
-  if (forced <= 0) while (s > 1 && tiles * s > num_sms()) s /= 2;
   return s;
 }
 
@@ -570,7 +611,6 @@ int launch_gemm(const GemmArgs& a) {
   p.m_tiles = (a.M + NT - 1) / NT;
   p.kb_per_tile = (a.K + kSub * kBK - 1) / (kSub * kBK);  // pipeline stages of 256 K (the last one may be half zero-filled)
   const int tiles = n_tiles * p.m_tiles;
-  p.split = C::kSplitFits ? choose_split(tiles, p.kb_per_tile, a.force_split) : 1;  // deep W8A8 rings: no room for the receive buffer
 
   CUtensorMap tm_act, tm_w;
   int rc = make_tmap_u8(&tm_act, a.act, a.M, a.K, NT);
@@ -579,18 +619,29 @@ int launch_gemm(const GemmArgs& a) {
   if (rc) return rc;
 
   auto kern = a.acc_out ? gemm_kernel<MODE, NT, WS, AS, true> : gemm_kernel<MODE, NT, WS, AS, false>;
+  const int dev = device_ordinal();
   static bool attr_set[2][kMaxDevices] = {};  // per (instantiation, device): the attribute is a per-device property of the function
-  bool& done = attr_set[a.acc_out ? 1 : 0][device_ordinal()];
+  bool& done = attr_set[a.acc_out ? 1 : 0][dev];
   if (!done) {
-    rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSplitFits ? C::kSmemBytesSplit : C::kSmemBytes),
-                    "cudaFuncSetAttribute(gemm smem)");
+    rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes), "cudaFuncSetAttribute(gemm smem)");
     if (rc) return rc;
     done = true;
   }
+  // resident clusters per (instantiation, device, split 1/2/4/8), queried once (0 = not yet asked)
+  static int resident_cache[2][kMaxDevices][4] = {};
+  auto resident = [&](int s) {
+    int& r = resident_cache[a.acc_out ? 1 : 0][dev][s == 1 ? 0 : s == 2 ? 1 : s == 4 ? 2 : 3];
+    if (r == 0) r = resident_clusters(reinterpret_cast<const void*>(kern), C::kSmemBytes, s);
+    return r;
+  };
+  p.split = choose_split(tiles, p.kb_per_tile, a.force_split, resident);
+  if (p.prof)  // profiled launches (tools/gemm_timeline.py) report their plan
+    fprintf(stderr, "qs_gemm_plan mode=%d nt=%d ws=%d as=%d M=%d N=%d K=%d tiles=%d split=%d ctas=%d smem=%d resident_clusters=%d\n", MODE, NT, WS,
+            AS, a.M, a.N, a.K, tiles, p.split, tiles * p.split, C::kSmemBytes, resident(p.split));
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(tiles * p.split);
   cfg.blockDim = dim3(kNumThreads);
-  cfg.dynamicSmemBytes = p.split > 1 ? C::kSmemBytesSplit : C::kSmemBytes;
+  cfg.dynamicSmemBytes = C::kSmemBytes;
   cfg.stream = static_cast<cudaStream_t>(a.stream);
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -612,18 +663,12 @@ int dispatch_gemm(const GemmArgs& a) {
   QS_REQUIRE((reinterpret_cast<uintptr_t>(a.act) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.weight) & 15) == 0, "gemm: operands must be 16-byte aligned");
   QS_REQUIRE(a.force_split == 0 || a.force_split == 1 || a.force_split == 2 || a.force_split == 4 || a.force_split == 8, "gemm: split must be 1, 2, 4 or 8");
   // ring depths (256-K stages): NT <= 64 fits two CTAs per SM (<= 113 KB of shared memory each); 128-token tiles run one CTA per SM and
-  // take deeper weight rings, still leaving room for the split-K receive buffer (W4A8)
+  // take deeper weight rings.  The split-K receive buffer aliases the drained rings, so it costs no shared memory.
   constexpr bool w8 = (MODE == kModeW8), grp = (MODE == kModeW4Grp);
   QS_REQUIRE(a.force_nt == 0 || a.force_nt == 32 || a.force_nt == 64 || a.force_nt == 128, "gemm: tile tokens must be 32, 64 or 128");
   const int nt = a.force_nt > 0 ? a.force_nt : a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;
   if (nt == 32) return launch_gemm<MODE, 32, (w8 ? 2 : grp ? 4 : 5), 4>(a);
   if (nt == 64) return launch_gemm<MODE, 64, (w8 ? 2 : grp ? 3 : 4), (w8 ? 2 : 3)>(a);
-  if constexpr (w8) {
-    // W8A8 at 65..128 tokens: the 4-deep weight ring (4 x 32 KB) leaves no room for the split-K receive buffer; layers with few tiles, which
-    // want a split, take a 2-deep ring
-    const int tiles = (a.N / kBM) * ((a.M + 127) / 128);
-    if (a.force_split != 1 && tiles * 2 <= num_sms()) return launch_gemm<MODE, 128, 2, 2>(a);
-  }
   return launch_gemm<MODE, 128, 4, 2>(a);
 }
 
