@@ -44,16 +44,30 @@ def quant_per_token(x, fuse_sum: bool = True):
     amax = max|x| (fp32, init 0) ; scale = half(amax/127) ; tmp = 127/amax ;
     q = cvt.rni.sat.s8(float(x)*tmp) ; sum = half(sum_fp32(x))        fused_kernels.cu:104-131
     The fp32 row sum is order dependent on the GPU; the oracle uses a float64 sum rounded to fp32.
+    Non-finite rows: the amax is taken with `if (val > amax)`, which never picks a NaN, so NaN elements are ignored
+    (and quantise to 0); the sum follows IEEE: an inf makes it inf, +inf with -inf or any NaN makes it NaN.
     """
     xf = f32(x)
-    amax = np.abs(xf).max(axis=1).astype(np.float32)
-    with np.errstate(divide="ignore", invalid="ignore"):
+    return quant_given_amax(x, _absmax(xf), fuse_sum)
+
+
+def _absmax(xf):
+    """max |x| per row, initialised to 0 and ignoring NaN (the reference's `if (val > amax) amax = val`)."""
+    return np.fmax.reduce(np.abs(f32(xf)), axis=1, initial=np.float32(0.0)).astype(np.float32)
+
+
+def quant_given_amax(x, amax_f32, fuse_sum: bool = True):
+    """The per-token quantiser with an amax supplied from outside (fp32 [M], e.g. the max over all tensor-parallel shards):
+    scale = half(amax/127) ; q = cvt.rni.sat.s8(float(x)*(127/amax)) ; sum = half(sum of this row), as in quant_per_token."""
+    xf = f32(x)
+    amax = f32(amax_f32).reshape(-1)
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
         scale = (amax / np.float32(127.0)).astype(np.float32).astype(np.float16)
         tmp = (np.float32(127.0) / amax).astype(np.float32)
         q = cvt_rni_sat_s8((xf * tmp[:, None]).astype(np.float32))
-    s = None
-    if fuse_sum:
-        s = xf.astype(np.float64).sum(axis=1).astype(np.float32).astype(np.float16)
+        s = None
+        if fuse_sum:
+            s = xf.astype(np.float64).sum(axis=1).astype(np.float32).astype(np.float16)
     return q, scale, s
 
 
@@ -108,6 +122,26 @@ def layernorm_general_quant(x, gamma, eps: float, fuse_sum: bool = True):
             acc = f16(acc.astype(np.float64) + yp[:, j].astype(np.float64))
         s = acc.astype(np.float64).sum(axis=1).astype(np.float32).astype(np.float16)
     return q, scale, s, y
+
+
+def layernorm_general_quant_per_tensor(x, gamma, eps: float, scale):
+    """rms_norm_general with use_per_token_quant=False: a static per-tensor scale (fp16, read) instead of the row amax.
+
+    mean, variance and y as in layernorm_general_quant ; q = cvt.rni.sat.s8(float(half(y)) * float(scale))
+    (layernorm_kernels.cu:153-157: the fp16-rounded y, not the fp32 y the per-token form quantises).
+    Returns (q int8 [M, H], y fp32) -- y for diagnostics.
+    """
+    xf = f32(x)
+    H = xf.shape[1]
+    g = f32(gamma)
+    mean = (xf.astype(np.float64).sum(axis=1) / H).astype(np.float32)
+    diff = (xf - mean[:, None]).astype(np.float32)
+    var = ((diff.astype(np.float64) ** 2).sum(axis=1)).astype(np.float32)
+    rstd = (1.0 / np.sqrt((var / np.float32(H) + np.float32(eps)).astype(np.float64))).astype(np.float32)
+    y = ((diff * rstd[:, None]).astype(np.float32) * g[None, :]).astype(np.float32)
+    sc = np.float32(np.float16(scale))
+    q = cvt_rni_sat_s8((y.astype(np.float16).astype(np.float32) * sc).astype(np.float32))
+    return q, y
 
 
 # ------------------------------------------------------------------------------------------------
@@ -206,3 +240,19 @@ def dequant_silu_and_mul_quant(inp_i32, scale_gate, scale_up, scale_out):
     y = (a[:, d:].astype(np.float32) * np.float32(scale_up)).astype(np.float32)
     silu = (x / (np.float32(1.0) + np.exp(-x).astype(np.float32))).astype(np.float32)
     return cvt_rni_sat_s8(((silu * y).astype(np.float32) / np.float32(scale_out)).astype(np.float32))
+
+
+def dequant_silu_and_mul_quant_per_token(inp_i32, scale_gate, scale_up):
+    """activation_kernels.cu:33-70 (per-token variant): t = silu(x)*y in fp32 ; amax = max|t| (init 0, NaN ignored) ;
+    scale_out = amax/127 (fp32) ; q = rni_sat((127/amax) * t).   Returns (q int8 [M, d], scale_out fp32 [M], tmp fp32 [M, d])."""
+    a = np.asarray(inp_i32)
+    d = a.shape[1] // 2
+    x = (a[:, :d].astype(np.float32) * np.float32(scale_gate)).astype(np.float32)
+    y = (a[:, d:].astype(np.float32) * np.float32(scale_up)).astype(np.float32)
+    with np.errstate(over="ignore", divide="ignore", invalid="ignore"):
+        silu = (x / (np.float32(1.0) + np.exp(-x).astype(np.float32))).astype(np.float32)
+        t = (silu * y).astype(np.float32)
+        amax = _absmax(t)
+        scale_out = (amax / np.float32(127.0)).astype(np.float32)
+        q = cvt_rni_sat_s8(((np.float32(127.0) / amax).astype(np.float32)[:, None] * t).astype(np.float32))
+    return q, scale_out, t

@@ -58,6 +58,20 @@ __device__ __forceinline__ long long block_sum_ll(long long v, long long* red) {
   return r;
 }
 
+// The quantisers' row sum feeds the per-channel W4A8 GEMM, and must say inf or NaN where the reference's fp32 sum does (an fp16
+// overflow of silu(g) * u, for example).  Fixed point cannot hold those (__float2ll_rn saturates and the next addition wraps), so
+// non-finite addends stay out of it and are summed apart in fp32.  That side sum is 0 for a finite row, +-inf if the row holds
+// infinities of one sign, NaN for +inf with -inf or any NaN -- exactly the IEEE sum's verdict -- and then replaces the exact sum.
+__device__ __forceinline__ long long fx_of_finite(float f) { return isfinite(f) ? fx_of_half(f) : 0ll; }
+__device__ __forceinline__ float nonfinite_part(float f) { return isfinite(f) ? 0.f : f; }
+__device__ __forceinline__ float row_sum(long long fx, float nonfinite) { return nonfinite == 0.f ? fx_to_float(fx) : nonfinite; }
+// cluster exchange of the silu_mul_quant kernels: one 64-bit word carries the CTA's amax (low half) and non-finite sum (high half)
+__device__ __forceinline__ long long pack_amax_nf(float amax, float nf) {
+  return static_cast<long long>((static_cast<unsigned long long>(__float_as_uint(nf)) << 32) | __float_as_uint(amax));
+}
+__device__ __forceinline__ float unpack_amax(long long v) { return __uint_as_float(static_cast<uint32_t>(v)); }
+__device__ __forceinline__ float unpack_nf(long long v) { return __uint_as_float(static_cast<uint32_t>(static_cast<unsigned long long>(v) >> 32)); }
+
 __device__ __forceinline__ void load_row_to_smem(__half* dst, const __half* src, int H) {
   // H % 8 == 0 guaranteed by the host wrapper
   const uint4* s = reinterpret_cast<const uint4*>(src);
@@ -395,7 +409,7 @@ __global__ void __launch_bounds__(kSiluQuantThreads) silu_mul_quant_kernel(int8_
   __half* sa = reinterpret_cast<__half*>(sm);  // this CTA's slice of the activation row (fp16)
   __shared__ float red[32];
   __shared__ long long red_ll[32];
-  __shared__ __align__(16) long long s_part[2];  // [0] = bits of the local amax (float), [1] = local fixed-point sum
+  __shared__ __align__(16) long long s_part[2];  // [0] = pack_amax_nf(local amax, local non-finite sum), [1] = local fixed-point sum
   const int row = blockIdx.x / csize;
   const int rank = blockIdx.x - row * csize;
   const int dl = d / csize;  // columns of this CTA (multiple of 8)
@@ -405,7 +419,7 @@ __global__ void __launch_bounds__(kSiluQuantThreads) silu_mul_quant_kernel(int8_
   qs_trace(QS_K_SILUQ, 1);
   const uint4* gx = reinterpret_cast<const uint4*>(in + static_cast<size_t>(row) * 2 * d + static_cast<size_t>(rank) * dl);
   const uint4* gy = reinterpret_cast<const uint4*>(in + static_cast<size_t>(row) * 2 * d + d + static_cast<size_t>(rank) * dl);
-  float amax = 0.f;
+  float amax = 0.f, nf = 0.f;
   long long s = 0;
   for (int i = threadIdx.x; i < dl / 8; i += blockDim.x) {
     const uint4 x = __ldg(gx + i), y = __ldg(gy + i);
@@ -417,35 +431,40 @@ __global__ void __launch_bounds__(kSiluQuantThreads) silu_mul_quant_kernel(int8_
     for (int j = 0; j < 8; ++j) {
       oh[j] = __hmul(silu_h_fused(xh[j]), yh[j]);
       const float f = __half2float(oh[j]);
-      if (input_sum) s += fx_of_half(f);
+      if (input_sum) { s += fx_of_finite(f); nf += nonfinite_part(f); }
       amax = fmaxf(amax, fabsf(f));
     }
     reinterpret_cast<uint4*>(sa)[i] = o;
   }
   amax = block_reduce(amax, red, OpMax(), 0.f);  // (the barriers inside also publish sa)
   long long total = 0;
-  if (input_sum) total = block_sum_ll(s, red_ll);
+  if (input_sum) {
+    total = block_sum_ll(s, red_ll);
+    nf = block_reduce(nf, red, OpSum(), 0.f);
+  }
   if (csize > 1) {
     if (threadIdx.x == 0) {
-      s_part[0] = __float_as_int(amax);
+      s_part[0] = pack_amax_nf(amax, nf);
       s_part[1] = total;
     }
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
     const uint32_t base = static_cast<uint32_t>(__cvta_generic_to_shared(s_part));
     amax = 0.f;
+    nf = 0.f;
     total = 0;
     for (int r = 0; r < csize; ++r) {
       uint32_t peer;
       asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer) : "r"(base), "r"(r));
       long long a, b;
       asm volatile("ld.shared::cluster.v2.s64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "r"(peer) : "memory");
-      amax = fmaxf(amax, __int_as_float(static_cast<int>(a)));
+      amax = fmaxf(amax, unpack_amax(a));
+      nf += unpack_nf(a);
       total += b;
     }
   }
   if (rank == 0 && threadIdx.x == 0) {
     scale[row] = __float2half_rn(__fdiv_rn(amax, 127.f));
-    if (input_sum) input_sum[row] = __float2half_rn(fx_to_float(total));
+    if (input_sum) input_sum[row] = __float2half_rn(row_sum(total, nf));
   }
   const float qs_ = __fdiv_rn(127.f, amax);
   int8_t* orow = out + static_cast<size_t>(row) * d + static_cast<size_t>(rank) * dl;
@@ -470,7 +489,8 @@ __global__ void __launch_bounds__(kSiluQuantThreads) silu_mul_quant_fast_kernel(
                                                                            __half* __restrict__ input_sum, __half* __restrict__ scale, int d, int csize) {
   __shared__ float red[32];
   __shared__ long long red_ll[32];
-  __shared__ __align__(16) long long s_rx[8][2];  // [sender]: bits of its amax, its fixed-point sum
+  __shared__ float red_nf[32];
+  __shared__ __align__(16) long long s_rx[8][2];  // [sender]: pack_amax_nf(its amax, its non-finite sum), its fixed-point sum
   const int row = blockIdx.x / csize;
   const int rank = blockIdx.x - row * csize;
   const int dl = d / csize;
@@ -488,7 +508,7 @@ __global__ void __launch_bounds__(kSiluQuantThreads) silu_mul_quant_fast_kernel(
     if (i < nvec) { xin[c] = __ldg(gx + i); yin[c] = __ldg(gy + i); }
   }
   float act[CHS][8];
-  float amax = 0.f;
+  float amax = 0.f, nf = 0.f;
   long long s = 0;
 #pragma unroll
   for (int c = 0; c < CHS; ++c) {
@@ -499,7 +519,7 @@ __global__ void __launch_bounds__(kSiluQuantThreads) silu_mul_quant_fast_kernel(
       for (int j = 0; j < 8; ++j) {
         const float f = __half2float(__hmul(silu_h_fused(xh[j]), yh[j]));
         act[c][j] = f;
-        if (input_sum) s += fx_of_half(f);
+        if (input_sum) { s += fx_of_finite(f); nf += nonfinite_part(f); }
         amax = fmaxf(amax, fabsf(f));
       }
     }
@@ -508,31 +528,35 @@ __global__ void __launch_bounds__(kSiluQuantThreads) silu_mul_quant_fast_kernel(
   amax = warp_reduce(amax, OpMax());
 #pragma unroll
   for (int m = 16; m >= 1; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
+  if (input_sum) nf = warp_reduce(nf, OpSum());
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { red[w] = amax; red_ll[w] = s; }
+  if (l == 0) { red[w] = amax; red_ll[w] = s; red_nf[w] = nf; }
   __syncthreads();
   amax = (l < (kSiluQuantThreads >> 5)) ? red[l] : 0.f;
   amax = warp_reduce(amax, OpMax());
   long long total = (l < (kSiluQuantThreads >> 5)) ? red_ll[l] : 0ll;
 #pragma unroll
   for (int m = 16; m >= 1; m >>= 1) total += __shfl_xor_sync(0xffffffffu, total, m);
+  if (input_sum) nf = warp_reduce((l < (kSiluQuantThreads >> 5)) ? red_nf[l] : 0.f, OpSum());
   if (csize > 1) {
     if (threadIdx.x < csize) {  // thread r pushes this CTA's pair into CTA r's table
       uint32_t peer;
       asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer) : "r"(static_cast<uint32_t>(__cvta_generic_to_shared(&s_rx[rank][0]))), "r"(threadIdx.x));
-      asm volatile("st.shared::cluster.v2.s64 [%0], {%1, %2};" ::"r"(peer), "l"(static_cast<long long>(__float_as_int(amax))), "l"(total) : "memory");
+      asm volatile("st.shared::cluster.v2.s64 [%0], {%1, %2};" ::"r"(peer), "l"(pack_amax_nf(amax, nf)), "l"(total) : "memory");
     }
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
     amax = 0.f;
+    nf = 0.f;
     total = 0;
     for (int r = 0; r < csize; ++r) {
-      amax = fmaxf(amax, __int_as_float(static_cast<int>(s_rx[r][0])));
+      amax = fmaxf(amax, unpack_amax(s_rx[r][0]));
+      nf += unpack_nf(s_rx[r][0]);
       total += s_rx[r][1];
     }
   }
   if (rank == 0 && threadIdx.x == 0) {
     scale[row] = __float2half_rn(__fdiv_rn(amax, 127.f));
-    if (input_sum) input_sum[row] = __float2half_rn(fx_to_float(total));
+    if (input_sum) input_sum[row] = __float2half_rn(row_sum(total, nf));
   }
   const float qs_ = __fdiv_rn(127.f, amax);
   int8_t* orow = out + static_cast<size_t>(row) * d + static_cast<size_t>(rank) * dl;
@@ -559,7 +583,7 @@ __global__ void __launch_bounds__(kThreads) quant_per_token_kernel(int8_t* __res
   qs_trace(QS_K_QUANT, 1);
   load_row_to_smem(sx, in + static_cast<size_t>(row) * H, H);
   __syncthreads();
-  float amax = 0.f;
+  float amax = 0.f, nf = 0.f;
   long long s = 0;
   for (int i = threadIdx.x; i < H / 8; i += blockDim.x) {
     const uint4 v = reinterpret_cast<const uint4*>(sx)[i];
@@ -567,14 +591,18 @@ __global__ void __launch_bounds__(kThreads) quant_per_token_kernel(int8_t* __res
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 f = __half22float2(h[j]);
-      if (input_sum) s += fx_of_half(f.x) + fx_of_half(f.y);
+      if (input_sum) {
+        s += fx_of_finite(f.x) + fx_of_finite(f.y);
+        nf += nonfinite_part(f.x) + nonfinite_part(f.y);
+      }
       amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
     }
   }
   amax = block_reduce(amax, red, OpMax(), 0.f);
   if (input_sum) {
     const long long total = block_sum_ll(s, red_ll);
-    if (threadIdx.x == 0) input_sum[row] = __float2half_rn(fx_to_float(total));
+    nf = block_reduce(nf, red, OpSum(), 0.f);
+    if (threadIdx.x == 0) input_sum[row] = __float2half_rn(row_sum(total, nf));
   }
   if (threadIdx.x == 0) scale[row] = __float2half_rn(__fdiv_rn(amax, 127.f));
   const float qs_ = __fdiv_rn(127.f, amax);
@@ -615,6 +643,7 @@ __global__ void __launch_bounds__(kThreads) row_absmax_kernel(float* __restrict_
 __global__ void __launch_bounds__(kThreads) quant_given_amax_kernel(int8_t* __restrict__ out, const __half* __restrict__ in,
                                                                    const float* __restrict__ amax_in, __half* __restrict__ input_sum,
                                                                    __half* __restrict__ scale, int H) {
+  __shared__ float red[32];
   __shared__ long long red_ll[32];
   const int row = blockIdx.x;
   if (threadIdx.x == 0) pdl_launch_dependents();
@@ -623,6 +652,7 @@ __global__ void __launch_bounds__(kThreads) quant_given_amax_kernel(int8_t* __re
   const float qs_ = __fdiv_rn(127.f, amax);
   const uint4* src = reinterpret_cast<const uint4*>(in + static_cast<size_t>(row) * H);
   long long s = 0;
+  float nf = 0.f;
   for (int i = threadIdx.x; i < H / 8; i += blockDim.x) {
     const uint4 v = src[i];
     const __half* h = reinterpret_cast<const __half*>(&v);
@@ -630,13 +660,14 @@ __global__ void __launch_bounds__(kThreads) quant_given_amax_kernel(int8_t* __re
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       x[j] = __half2float(h[j]);
-      if (input_sum) s += fx_of_half(x[j]);
+      if (input_sum) { s += fx_of_finite(x[j]); nf += nonfinite_part(x[j]); }
     }
     store_q8(out + static_cast<size_t>(row) * H, i, x, qs_);
   }
   if (input_sum) {
     const long long total = block_sum_ll(s, red_ll);
-    if (threadIdx.x == 0) input_sum[row] = __float2half_rn(fx_to_float(total));
+    nf = block_reduce(nf, red, OpSum(), 0.f);
+    if (threadIdx.x == 0) input_sum[row] = __float2half_rn(row_sum(total, nf));
   }
   if (threadIdx.x == 0) scale[row] = __float2half_rn(__fdiv_rn(amax, 127.f));
 }
@@ -647,6 +678,7 @@ template <int CH>
 __global__ void __launch_bounds__(kThreads) quant_per_token_fast_kernel(int8_t* __restrict__ out, const __half* __restrict__ in,
                                                                        __half* __restrict__ input_sum, __half* __restrict__ scale, int H) {
   __shared__ float red[32];
+  __shared__ float red_nf[32];
   __shared__ long long red_ll[32];
   const int row = blockIdx.x;
   const int nvec = H / 8;
@@ -661,7 +693,7 @@ __global__ void __launch_bounds__(kThreads) quant_per_token_fast_kernel(int8_t* 
     const int i = threadIdx.x + c * kThreads;
     xv[c] = (i < nvec) ? __ldg(src + i) : make_uint4(0u, 0u, 0u, 0u);
   }
-  float amax = 0.f;
+  float amax = 0.f, nf = 0.f;
   long long s = 0;
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
@@ -670,7 +702,10 @@ __global__ void __launch_bounds__(kThreads) quant_per_token_fast_kernel(int8_t* 
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float2 f = __half22float2(h[j]);
-        if (input_sum) s += fx_of_half(f.x) + fx_of_half(f.y);
+        if (input_sum) {
+          s += fx_of_finite(f.x) + fx_of_finite(f.y);
+          nf += nonfinite_part(f.x) + nonfinite_part(f.y);
+        }
         amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
       }
     }
@@ -678,8 +713,9 @@ __global__ void __launch_bounds__(kThreads) quant_per_token_fast_kernel(int8_t* 
   amax = warp_reduce(amax, OpMax());
 #pragma unroll
   for (int m = 16; m >= 1; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
+  if (input_sum) nf = warp_reduce(nf, OpSum());
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { red[w] = amax; red_ll[w] = s; }
+  if (l == 0) { red[w] = amax; red_ll[w] = s; red_nf[w] = nf; }
   __syncthreads();
   amax = (l < (kThreads >> 5)) ? red[l] : 0.f;
   amax = warp_reduce(amax, OpMax());
@@ -687,7 +723,8 @@ __global__ void __launch_bounds__(kThreads) quant_per_token_fast_kernel(int8_t* 
     long long total = (l < (kThreads >> 5)) ? red_ll[l] : 0ll;
 #pragma unroll
     for (int m = 16; m >= 1; m >>= 1) total += __shfl_xor_sync(0xffffffffu, total, m);
-    if (threadIdx.x == 0) input_sum[row] = __float2half_rn(fx_to_float(total));
+    nf = warp_reduce((l < (kThreads >> 5)) ? red_nf[l] : 0.f, OpSum());
+    if (threadIdx.x == 0) input_sum[row] = __float2half_rn(row_sum(total, nf));
   }
   if (threadIdx.x == 0) scale[row] = __float2half_rn(__fdiv_rn(amax, 127.f));
   const float qs_ = __fdiv_rn(127.f, amax);
