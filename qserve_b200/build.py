@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libqserve_b200.so")
 SOURCES = ["capi.cu", "gemm.cu", "attention.cu", "prefill_attention.cu", "prefix_attention.cu", "multi_token_attention.cu", "tree_verify.cu", "sampling.cu", "elementwise.cu"]
-HEADERS = ["common.cuh", "launch.h", "paged_attention.cuh", os.path.join("..", "..", "include", "qserve_b200.h")]
+HEADERS = ["common.cuh", "launch.h", "launch.cuh", "paged_attention.cuh", "prompt_attention.cuh", os.path.join("..", "..", "include", "qserve_b200.h")]
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3", "-lineinfo",

@@ -17,7 +17,7 @@
 #include <math_constants.h>
 
 #include "common.cuh"
-#include "launch.h"
+#include "launch.cuh"
 #include "paged_attention.cuh"
 
 namespace qs {
@@ -753,21 +753,6 @@ __global__ void padding_offsets_kernel(int* __restrict__ out, const int* __restr
   for (int t = beg + threadIdx.x; t < end; t += blockDim.x) out[t] = off;
 }
 
-template <typename Kern, typename... Args>
-int launch_pdl(Kern kern, dim3 grid, dim3 block, size_t smem, void* stream, const char* what, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return check_cuda(cudaLaunchKernelEx(&cfg, kern, args...), what);
-}
-
 constexpr size_t kAttnCounterBytes = 256 * 1024;  // 49152 (sequence, head-group) split counters + 16384 per-token counters
 constexpr size_t kAttnTokCounterOffset = 192 * 1024;
 
@@ -831,31 +816,13 @@ int decode_attention(const DecodeAttnArgs& a) {
   }
   dim3 grid(gx, a.batch, nsplit);
   auto run = [&](auto kern, size_t smem) {
-    static bool attr_done[2][kMaxDevices] = {};
-    bool& done = attr_done[a.int4_kv ? 0 : 1][device_ordinal()];
-    if (!done) {
-      int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), "attention smem attribute");
-      if (rc) return rc;
-      done = true;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(kAttnThreadsV2);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = static_cast<cudaStream_t>(a.stream);
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    attr[1].id = cudaLaunchAttributeClusterDimension;
-    attr[1].val.clusterDim.x = 1;
-    attr[1].val.clusterDim.y = 1;
-    attr[1].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 2;
-    return check_cuda(cudaLaunchKernelEx(&cfg, kern, static_cast<const __half*>(a.q),
-                      static_cast<const __half*>(a.k), static_cast<const __half*>(a.v), a.q_stride, a.k_stride, a.v_stride, a.kv_pointers, a.lengths,
-                      static_cast<__half*>(out), a.num_heads, a.num_kv_heads, a.max_blocks, pg, a.rotary_base, a.rotary_dim, a.timestep, nsplit,
-                      part, cnt, tok_cnt, static_cast<int8_t*>(a.q_out), static_cast<__half*>(a.q_scale), static_cast<__half*>(a.q_sum), static_cast<unsigned long long*>(a.prof)), "single_query_attention");
+    const int rc = raise_smem_limit(kern, smem, "attention smem attribute");
+    if (rc) return rc;
+    return launch(kern, grid, dim3(kAttnThreadsV2), smem, 1, a.stream, "single_query_attention", static_cast<const __half*>(a.q),
+                  static_cast<const __half*>(a.k), static_cast<const __half*>(a.v), a.q_stride, a.k_stride, a.v_stride, a.kv_pointers, a.lengths,
+                  static_cast<__half*>(out), a.num_heads, a.num_kv_heads, a.max_blocks, pg, a.rotary_base, a.rotary_dim, a.timestep, nsplit, part, cnt,
+                  tok_cnt, static_cast<int8_t*>(a.q_out), static_cast<__half*>(a.q_scale), static_cast<__half*>(a.q_sum),
+                  static_cast<unsigned long long*>(a.prof));
   };
   QS_REQUIRE(a.tokens_per_block == kPageTokens, "single_query_attention: tokens_per_block=%d, only 64 is supported (cache_engine block_size)", a.tokens_per_block);
   return a.int4_kv ? run(decode_attention_kernel<4>, static_cast<size_t>(kWarps) * StageLayout<4>::kWarpBytes)
@@ -876,9 +843,9 @@ int prefill_rope_append(const PrefillAppendArgs& a) {
   long long blocks = (work + 3) / 4;
   if (blocks > static_cast<long long>(num_sms()) * 16) blocks = static_cast<long long>(num_sms()) * 16;
   auto run = [&](auto kern) {
-    return launch_pdl(kern, dim3(static_cast<unsigned>(blocks)), dim3(128), 0, a.stream, "apply_bias_rope_update_kv_cache", static_cast<__half*>(a.qkv),
-                      a.seq_lens, a.padding_offset, a.kv_pointers, a.start_pos, a.num_tokens, a.max_blocks, a.num_heads, a.num_kv_heads, a.seq_len, pg,
-                      a.rotary_base, a.rotary_dim, a.max_positions, a.tree_mask);
+    return launch(kern, dim3(static_cast<unsigned>(blocks)), dim3(128), 0, 0, a.stream, "apply_bias_rope_update_kv_cache", static_cast<__half*>(a.qkv),
+                  a.seq_lens, a.padding_offset, a.kv_pointers, a.start_pos, a.num_tokens, a.max_blocks, a.num_heads, a.num_kv_heads, a.seq_len, pg,
+                  a.rotary_base, a.rotary_dim, a.max_positions, a.tree_mask);
   };
   if (a.tree_mask) {
     QS_REQUIRE(a.start_pos && a.seq_len <= 16, "apply_bias_rope_update_kv_cache_tree: needs start_pos and at most 16 draft nodes per sequence (seq_len=%d)",
@@ -891,7 +858,7 @@ int prefill_rope_append(const PrefillAppendArgs& a) {
 
 int padding_offsets(int* out, const int* cu_seqlens, int batch, int max_seqlen, void* stream) {
   if (batch == 0) return QS_OK;
-  return launch_pdl(padding_offsets_kernel, dim3(batch), dim3(256), 0, stream, "compute_padding_offsets", out, cu_seqlens, max_seqlen);
+  return launch(padding_offsets_kernel, dim3(batch), dim3(256), 0, 0, stream, "compute_padding_offsets", out, cu_seqlens, max_seqlen);
 }
 
 }  // namespace qs

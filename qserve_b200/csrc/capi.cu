@@ -1,10 +1,13 @@
 // qserve_b200 -- extern "C" entry points (include/qserve_b200.h) and error plumbing.
 #include <cstdarg>
 #include <cstdio>
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "../../include/qserve_b200.h"
 #include "common.cuh"
-#include "launch.h"
+#include "launch.cuh"
 
 namespace qs {
 
@@ -44,6 +47,18 @@ int num_sms() {
     sms[dev] = n > 0 ? n : 132;
   }
   return sms[dev];
+}
+
+int raise_smem_limit(const void* kern, size_t bytes, const char* what) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> limits;
+  const std::pair<const void*, int> key(kern, device_ordinal());
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& have = limits[key];
+  if (bytes <= have) return QS_OK;
+  const int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)), what);
+  if (rc == QS_OK) have = bytes;
+  return rc;
 }
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }

@@ -28,6 +28,10 @@ int check_cuda(cudaError_t e, const char* what);
     if (!(cond)) return ::qs::set_error(::qs::QS_ERR_INVALID, __VA_ARGS__); \
   } while (0)
 
+// cuTensorMapEncodeTiled from the driver, looked up once; null if the driver does not export it (prefill_attention.cu)
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                    const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+PFN_encodeTiled get_encode();
 // TMA descriptor of an fp16 [rows, cols] matrix with a row pitch of `stride` elements, box = 64 columns (128 B, 128-byte swizzle) x 128 rows
 // (prefill_attention.cu; shared by the prompt-attention kernels)
 int make_tmap_f16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t stride);
@@ -39,6 +43,13 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
+
+// 2^x on the SFU (MUFU.EX2), flush-to-zero: -inf must give 0
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;

@@ -5,7 +5,7 @@
 // accesses, IEEE fp32 arithmetic in the reference's source order, and is PDL-aware (griddepcontrol.wait /
 // launch_dependents) so back-to-back launches of the decode step overlap their prologues.
 #include "common.cuh"
-#include "launch.h"
+#include "launch.cuh"
 
 namespace qs {
 namespace {
@@ -1185,26 +1185,11 @@ __global__ void __launch_bounds__(kThreads) norm_quant_fast_kernel(int8_t* __res
   }
 }
 
-template <typename Kern, typename... Args>
-int launch(Kern kern, dim3 grid, dim3 block, size_t smem, void* stream, const char* what, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return check_cuda(cudaLaunchKernelEx(&cfg, kern, args...), what);
-}
-
 template <typename Kern>
 int ensure_smem(Kern kern, size_t bytes, const char* what) {
   if (bytes <= 40 * 1024) return QS_OK;  // static shared memory of the kernel comes on top of the dynamic row
   QS_REQUIRE(bytes <= 200 * 1024, "%s: row of %zu bytes does not fit in shared memory", what, bytes);
-  return check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024), what);
+  return raise_smem_limit(kern, 200 * 1024, what);
 }
 
 // fast path of the norm family: returns 1 if the shape is not eligible (caller falls back to the shared-memory kernels)
@@ -1217,7 +1202,7 @@ int launch_norm_fast(void* out_q, void* hidden_out, const void* x, const void* d
   ref_block = 32 * ((ref_block + 31) / 32);  // layernorm_kernels.cu:433-436
   const size_t smem = input_sum ? static_cast<size_t>(hidden) * 2 : 0;
   auto go = [&](auto kern) {
-    return launch(kern, dim3(tokens), dim3(kThreads), smem, stream, what, static_cast<int8_t*>(out_q), static_cast<__half*>(hidden_out),
+    return launch(kern, dim3(tokens), dim3(kThreads), smem, 0, stream, what, static_cast<int8_t*>(out_q), static_cast<__half*>(hidden_out),
                   static_cast<const __half*>(x), static_cast<const __half*>(delta), static_cast<const __half*>(gamma), static_cast<__half*>(input_sum),
                   static_cast<__half*>(scaling), eps, hidden, ref_block, pa);
   };
@@ -1234,7 +1219,7 @@ int rms_norm(void* out, const void* in, const void* weight, float eps, int use_q
   const size_t smem = static_cast<size_t>(hidden) * 2;
   int rc = ensure_smem(rms_norm_kernel, smem, "rms_norm");
   if (rc) return rc;
-  return launch(rms_norm_kernel, dim3(tokens), dim3(kThreads), smem, stream, "rms_norm", out, static_cast<const __half*>(in),
+  return launch(rms_norm_kernel, dim3(tokens), dim3(kThreads), smem, 0, stream, "rms_norm", out, static_cast<const __half*>(in),
                 static_cast<const __half*>(weight), eps, hidden, use_quant != 0);
 }
 
@@ -1252,7 +1237,7 @@ int layernorm_general_quant(void* out_q, const void* in, const void* gamma, void
   if (rc) return rc;
   int ref_block = hidden < 1024 ? hidden : 1024;
   ref_block = 32 * ((ref_block + 31) / 32);  // layernorm_kernels.cu:433-436
-  return launch(layernorm_quant_kernel, dim3(tokens), dim3(kThreads), smem, stream, "rms_norm_general", static_cast<int8_t*>(out_q),
+  return launch(layernorm_quant_kernel, dim3(tokens), dim3(kThreads), smem, 0, stream, "rms_norm_general", static_cast<int8_t*>(out_q),
                 static_cast<const __half*>(in), static_cast<const __half*>(gamma), static_cast<__half*>(input_sum),
                 static_cast<__half*>(scaling), eps, hidden, ref_block, per_token != 0);
 }
@@ -1263,7 +1248,7 @@ int quant_per_token(void* out_q, const void* in, void* input_sum, void* scale, i
   {
     const int nvec = hidden / 8;
     auto go = [&](auto kern) {
-      return launch(kern, dim3(tokens), dim3(kThreads), 0, stream, "invoke_quant", static_cast<int8_t*>(out_q), static_cast<const __half*>(in),
+      return launch(kern, dim3(tokens), dim3(kThreads), 0, 0, stream, "invoke_quant", static_cast<int8_t*>(out_q), static_cast<const __half*>(in),
                     static_cast<__half*>(input_sum), static_cast<__half*>(scale), hidden);
     };
     if (nvec <= kThreads) return go(quant_per_token_fast_kernel<1>);
@@ -1273,20 +1258,20 @@ int quant_per_token(void* out_q, const void* in, void* input_sum, void* scale, i
   const size_t smem = static_cast<size_t>(hidden) * 2;
   int rc = ensure_smem(quant_per_token_kernel, smem, "invoke_quant");
   if (rc) return rc;
-  return launch(quant_per_token_kernel, dim3(tokens), dim3(kThreads), smem, stream, "invoke_quant", static_cast<int8_t*>(out_q),
+  return launch(quant_per_token_kernel, dim3(tokens), dim3(kThreads), smem, 0, stream, "invoke_quant", static_cast<int8_t*>(out_q),
                 static_cast<const __half*>(in), static_cast<__half*>(input_sum), static_cast<__half*>(scale), hidden);
 }
 
 int row_absmax(void* amax_f32, const void* in, int tokens, int hidden, void* stream) {
   if (tokens == 0) return QS_OK;
   QS_REQUIRE(hidden > 0 && hidden % 8 == 0, "row_absmax: hidden=%d must be a positive multiple of 8", hidden);
-  return launch(row_absmax_kernel, dim3(tokens), dim3(kThreads), 0, stream, "row_absmax", static_cast<float*>(amax_f32), static_cast<const __half*>(in), hidden);
+  return launch(row_absmax_kernel, dim3(tokens), dim3(kThreads), 0, 0, stream, "row_absmax", static_cast<float*>(amax_f32), static_cast<const __half*>(in), hidden);
 }
 
 int quant_given_amax(void* out_q, const void* in, const void* amax_f32, void* input_sum, void* scale, int tokens, int hidden, void* stream) {
   if (tokens == 0) return QS_OK;
   QS_REQUIRE(hidden > 0 && hidden % 8 == 0, "quant_given_amax: hidden=%d must be a positive multiple of 8", hidden);
-  return launch(quant_given_amax_kernel, dim3(tokens), dim3(kThreads), 0, stream, "quant_given_amax", static_cast<int8_t*>(out_q),
+  return launch(quant_given_amax_kernel, dim3(tokens), dim3(kThreads), 0, 0, stream, "quant_given_amax", static_cast<int8_t*>(out_q),
                 static_cast<const __half*>(in), static_cast<const float*>(amax_f32), static_cast<__half*>(input_sum), static_cast<__half*>(scale), hidden);
 }
 
@@ -1294,7 +1279,7 @@ int quant_scalar(void* out_q, const void* in, float scale, int tokens, int hidde
   const size_t n = static_cast<size_t>(tokens) * hidden;
   if (n == 0) return QS_OK;
   const int grid = static_cast<int>((n + 1023) / 1024 < 2048 ? (n + 1023) / 1024 : 2048);
-  return launch(quant_scalar_kernel, dim3(grid), dim3(256), 0, stream, "invoke_quant(scalar)", static_cast<int8_t*>(out_q),
+  return launch(quant_scalar_kernel, dim3(grid), dim3(256), 0, 0, stream, "invoke_quant(scalar)", static_cast<int8_t*>(out_q),
                 static_cast<const __half*>(in), scale, n);
 }
 
@@ -1304,7 +1289,7 @@ int silu_and_mul(void* out, const void* in, int tokens, int d, void* stream) {
   const long long n_vec = static_cast<long long>(tokens) * (d / 8);
   const long long want = (n_vec + 255) / 256;  // one vector per thread up to 8 CTAs per SM (decode sizes), then two per thread and loop iteration
   const long long cap = static_cast<long long>(num_sms()) * 8;
-  return launch(silu_and_mul_kernel, dim3(static_cast<unsigned>(want < cap ? want : cap)), dim3(256), 0, stream, "silu_and_mul", static_cast<__half*>(out),
+  return launch(silu_and_mul_kernel, dim3(static_cast<unsigned>(want < cap ? want : cap)), dim3(256), 0, 0, stream, "silu_and_mul", static_cast<__half*>(out),
                 static_cast<const __half*>(in), d, n_vec);
 }
 
@@ -1312,26 +1297,26 @@ int gelu(void* out, const void* in, int tokens, int d, int fast, void* stream) {
   const size_t n = static_cast<size_t>(tokens) * d;
   if (n == 0) return QS_OK;
   const int grid = static_cast<int>((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096);
-  return launch(gelu_kernel, dim3(grid), dim3(256), 0, stream, "gelu", static_cast<__half*>(out), static_cast<const __half*>(in), n, fast != 0);
+  return launch(gelu_kernel, dim3(grid), dim3(256), 0, 0, stream, "gelu", static_cast<__half*>(out), static_cast<const __half*>(in), n, fast != 0);
 }
 
 int dequant_add_residual(void* out, const void* in_i32, const void* residual, const void* scale_vec, float scale, int tokens, int hidden,
                          void* stream) {
   if (tokens == 0) return QS_OK;
-  return launch(dequant_add_residual_kernel, dim3(tokens), dim3(kThreads), 0, stream, "invoke_dequant_add_residual", static_cast<__half*>(out),
+  return launch(dequant_add_residual_kernel, dim3(tokens), dim3(kThreads), 0, 0, stream, "invoke_dequant_add_residual", static_cast<__half*>(out),
                 static_cast<const int32_t*>(in_i32), static_cast<const __half*>(residual), static_cast<const __half*>(scale_vec), scale, hidden);
 }
 
 int dequant(void* out, const void* in_i32, float scale, int tokens, int hidden, int in_stride, int out_stride, void* stream) {
   if (tokens == 0) return QS_OK;
-  return launch(dequant_kernel, dim3(tokens), dim3(kThreads), 0, stream, "invoke_dequant", static_cast<__half*>(out),
+  return launch(dequant_kernel, dim3(tokens), dim3(kThreads), 0, 0, stream, "invoke_dequant", static_cast<__half*>(out),
                 static_cast<const int32_t*>(in_i32), scale, hidden, in_stride, out_stride);
 }
 
 int dequant_add_residual_rms_norm_quant(void* out_q, const void* in_i32, void* residual, const void* gamma, const void* scale_vec, float scale,
                                         float eps, int tokens, int hidden, void* stream) {
   if (tokens == 0) return QS_OK;
-  return launch(dequant_add_residual_rms_norm_quant_kernel, dim3(tokens), dim3(kThreads), 0, stream, "invoke_dequant_add_residual_rms_norm_quant",
+  return launch(dequant_add_residual_rms_norm_quant_kernel, dim3(tokens), dim3(kThreads), 0, 0, stream, "invoke_dequant_add_residual_rms_norm_quant",
                 static_cast<int8_t*>(out_q), static_cast<const int32_t*>(in_i32), static_cast<__half*>(residual),
                 static_cast<const __half*>(gamma), static_cast<const __half*>(scale_vec), scale, eps, hidden);
 }
@@ -1339,7 +1324,7 @@ int dequant_add_residual_rms_norm_quant(void* out_q, const void* in_i32, void* r
 int dequant_silu_and_mul_quant(void* out_q, const void* in_i32, float scale_gate, float scale_up, float scale_out, void* scale_out_vec, void* tmp,
                                int tokens, int d, void* stream) {
   if (tokens == 0) return QS_OK;
-  return launch(dequant_silu_and_mul_quant_kernel, dim3(tokens), dim3(kThreads), 0, stream, "invoke_dequant_silu_and_mul_quant",
+  return launch(dequant_silu_and_mul_quant_kernel, dim3(tokens), dim3(kThreads), 0, 0, stream, "invoke_dequant_silu_and_mul_quant",
                 static_cast<int8_t*>(out_q), static_cast<const int32_t*>(in_i32), d, scale_gate, scale_up, scale_out,
                 static_cast<float*>(scale_out_vec), static_cast<float*>(tmp));
 }
@@ -1357,24 +1342,9 @@ int silu_and_mul_quant(void* out_q, const void* in, void* input_sum, void* scale
     int rc = ensure_smem(silu_mul_quant_kernel, smem, "silu_and_mul_quant");
     if (rc) return rc;
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(tokens * csize);
-  cfg.blockDim = dim3(kSiluQuantThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  attr[1].id = cudaLaunchAttributeClusterDimension;
-  attr[1].val.clusterDim.x = csize;
-  attr[1].val.clusterDim.y = 1;
-  attr[1].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
   auto kern = !fast ? silu_mul_quant_kernel : (nvec <= kSiluQuantThreads ? silu_mul_quant_fast_kernel<1> : silu_mul_quant_fast_kernel<2>);
-  return check_cuda(cudaLaunchKernelEx(&cfg, kern, static_cast<int8_t*>(out_q), static_cast<const __half*>(in),
-                                       static_cast<__half*>(input_sum), static_cast<__half*>(scale), d, csize),
-                    "silu_and_mul_quant");
+  return launch(kern, dim3(tokens * csize), dim3(kSiluQuantThreads), smem, csize, stream, "silu_and_mul_quant", static_cast<int8_t*>(out_q),
+                static_cast<const __half*>(in), static_cast<__half*>(input_sum), static_cast<__half*>(scale), d, csize);
 }
 
 int add_layernorm_quant(void* out_q, void* hidden_out, const void* x, const void* delta, const void* gamma, void* input_sum, void* scaling,
@@ -1390,7 +1360,7 @@ int add_layernorm_quant(void* out_q, void* hidden_out, const void* x, const void
   if (rc) return rc;
   int ref_block = hidden < 1024 ? hidden : 1024;
   ref_block = 32 * ((ref_block + 31) / 32);
-  return launch(add_layernorm_quant_kernel<false>, dim3(tokens), dim3(kFusedThreads), smem, stream, "add_rms_norm_general", static_cast<int8_t*>(out_q),
+  return launch(add_layernorm_quant_kernel<false>, dim3(tokens), dim3(kFusedThreads), smem, 0, stream, "add_rms_norm_general", static_cast<int8_t*>(out_q),
                 static_cast<__half*>(hidden_out), static_cast<const __half*>(x), static_cast<const __half*>(delta),
                 static_cast<const __half*>(gamma), static_cast<__half*>(input_sum), static_cast<__half*>(scaling), eps, hidden, ref_block, PeerArgs{});
 }
@@ -1417,7 +1387,7 @@ int add_layernorm_quant_peer(void* out_q, void* hidden_out, const void* x, const
   if (rc) return rc;
   int ref_block = hidden < 1024 ? hidden : 1024;
   ref_block = 32 * ((ref_block + 31) / 32);
-  return launch(add_layernorm_quant_kernel<true>, dim3(tokens), dim3(kFusedThreads), smem, stream, "add_rms_norm_general_peer", static_cast<int8_t*>(out_q),
+  return launch(add_layernorm_quant_kernel<true>, dim3(tokens), dim3(kFusedThreads), smem, 0, stream, "add_rms_norm_general_peer", static_cast<int8_t*>(out_q),
                 static_cast<__half*>(hidden_out), static_cast<const __half*>(x), static_cast<const __half*>(nullptr),
                 static_cast<const __half*>(gamma), static_cast<__half*>(input_sum), static_cast<__half*>(scaling), eps, hidden, ref_block, pa);
 }
@@ -1425,21 +1395,8 @@ int add_layernorm_quant_peer(void* out_q, void* hidden_out, const void* x, const
 int argmax_rows(void* out, const void* logits, int rows, int vocab, void* stream) {
   if (rows == 0) return QS_OK;
   QS_REQUIRE(vocab > 0 && vocab % 8 == 0, "argmax_rows: vocab=%d must be a positive multiple of 8", vocab);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(rows * kArgmaxCluster);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  attr[1].id = cudaLaunchAttributeClusterDimension;
-  attr[1].val.clusterDim.x = kArgmaxCluster;
-  attr[1].val.clusterDim.y = 1;
-  attr[1].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  return check_cuda(cudaLaunchKernelEx(&cfg, argmax_rows_kernel, static_cast<long long*>(out), static_cast<const __half*>(logits), vocab), "argmax_rows");
+  return launch(argmax_rows_kernel, dim3(rows * kArgmaxCluster), dim3(kThreads), 0, kArgmaxCluster, stream, "argmax_rows", static_cast<long long*>(out),
+                static_cast<const __half*>(logits), vocab);
 }
 
 }  // namespace qs

@@ -32,7 +32,7 @@
 #include <unordered_map>
 
 #include "common.cuh"
-#include "launch.h"
+#include "launch.cuh"
 
 namespace qs {
 
@@ -469,20 +469,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
 // host side
 // ---------------------------------------------------------------------------------------------
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-PFN_encodeTiled get_encode() {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && p) fn = reinterpret_cast<PFN_encodeTiled>(p);
-  }
-  return fn;
-}
-
 // Tensor maps are pure functions of (address, shape, box): cuTensorMapEncodeTiled costs ~1 us of host time and an eager decode step issues
 // ~260 of them, so they are memoised (weights: one entry per layer and projection; activations: a handful of buffers).
 struct TmapKey {
@@ -619,14 +605,9 @@ int launch_gemm(const GemmArgs& a) {
   if (rc) return rc;
 
   auto kern = a.acc_out ? gemm_kernel<MODE, NT, WS, AS, true> : gemm_kernel<MODE, NT, WS, AS, false>;
+  rc = raise_smem_limit(kern, C::kSmemBytes, "cudaFuncSetAttribute(gemm smem)");
+  if (rc) return rc;
   const int dev = device_ordinal();
-  static bool attr_set[2][kMaxDevices] = {};  // per (instantiation, device): the attribute is a per-device property of the function
-  bool& done = attr_set[a.acc_out ? 1 : 0][dev];
-  if (!done) {
-    rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes), "cudaFuncSetAttribute(gemm smem)");
-    if (rc) return rc;
-    done = true;
-  }
   // resident clusters per (instantiation, device, split 1/2/4/8), queried once (0 = not yet asked)
   static int resident_cache[2][kMaxDevices][4] = {};
   auto resident = [&](int s) {
@@ -638,21 +619,7 @@ int launch_gemm(const GemmArgs& a) {
   if (p.prof)  // profiled launches (tools/gemm_timeline.py) report their plan
     fprintf(stderr, "qs_gemm_plan mode=%d nt=%d ws=%d as=%d M=%d N=%d K=%d tiles=%d split=%d ctas=%d smem=%d resident_clusters=%d\n", MODE, NT, WS,
             AS, a.M, a.N, a.K, tiles, p.split, tiles * p.split, C::kSmemBytes, resident(p.split));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(tiles * p.split);
-  cfg.blockDim = dim3(kNumThreads);
-  cfg.dynamicSmemBytes = C::kSmemBytes;
-  cfg.stream = static_cast<cudaStream_t>(a.stream);
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  attr[1].id = cudaLaunchAttributeClusterDimension;
-  attr[1].val.clusterDim.x = p.split;
-  attr[1].val.clusterDim.y = 1;
-  attr[1].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  return check_cuda(cudaLaunchKernelEx(&cfg, kern, tm_act, tm_w, p), "gemm launch");
+  return launch(kern, dim3(tiles * p.split), dim3(kNumThreads), C::kSmemBytes, p.split, a.stream, "gemm launch", tm_act, tm_w, p);
 }
 
 template <int MODE>

@@ -20,7 +20,7 @@
 #include <math_constants.h>
 
 #include "common.cuh"
-#include "launch.h"
+#include "launch.cuh"
 #include "paged_attention.cuh"
 
 namespace qs {
@@ -328,7 +328,7 @@ int resident_ctas() {
   if (r == 0) {
     const int smem = kWarps * StageLayout<BITS>::kWarpBytes;
     int n = 0;
-    if (cudaFuncSetAttribute(multi_token_attention_kernel<BITS, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||
+    if (raise_smem_limit(multi_token_attention_kernel<BITS, NT, false>, smem, "multi_token_decode_attention smem attribute") != QS_OK ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, multi_token_attention_kernel<BITS, NT, false>, kAttnConsumers, smem) != cudaSuccess || n < 1) {
       cudaGetLastError();
       n = 1;
@@ -336,20 +336,6 @@ int resident_ctas() {
     r = n;
   }
   return r;
-}
-
-// The tree instantiations run with the chain kernel's launch plan; they only need the dynamic shared memory attribute (once per device).
-template <int BITS, int NT>
-int tree_smem_attribute() {
-  static bool done[kMaxDevices] = {};
-  bool& d = done[device_ordinal()];
-  if (!d) {
-    const int rc = check_cuda(cudaFuncSetAttribute(multi_token_attention_kernel<BITS, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                   kWarps * StageLayout<BITS>::kWarpBytes), "tree_decode_attention smem attribute");
-    if (rc) return rc;
-    d = true;
-  }
-  return QS_OK;
 }
 
 MultiTokenPlan plan_multi_token(int bits, int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads) {
@@ -432,27 +418,14 @@ int multi_token_attention(const MultiTokenAttnArgs& a) {
   p.tree_mask = a.tree_mask;
   const dim3 grid(static_cast<unsigned>(gx), a.batch, pl.nsplit);
   auto run = [&](auto kern, size_t smem) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(kAttnConsumers);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = static_cast<cudaStream_t>(a.stream);
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return check_cuda(cudaLaunchKernelEx(&cfg, kern, p), "multi_token_decode_attention");
+    const int rc = raise_smem_limit(kern, smem, "multi_token_decode_attention smem attribute");
+    if (rc) return rc;
+    return launch(kern, grid, dim3(kAttnConsumers), smem, 0, a.stream, "multi_token_decode_attention", p);
   };
   const size_t smem4 = static_cast<size_t>(kWarps) * StageLayout<4>::kWarpBytes, smem8 = static_cast<size_t>(kWarps) * StageLayout<8>::kWarpBytes;
   if (a.tree_mask) {
-    int rc;
-    if (a.int4_kv) {
-      if (pl.ntile == 1) return (rc = tree_smem_attribute<4, 1>()) ? rc : run(multi_token_attention_kernel<4, 1, true>, smem4);
-      return (rc = tree_smem_attribute<4, 2>()) ? rc : run(multi_token_attention_kernel<4, 2, true>, smem4);
-    }
-    if (pl.ntile == 1) return (rc = tree_smem_attribute<8, 1>()) ? rc : run(multi_token_attention_kernel<8, 1, true>, smem8);
-    return (rc = tree_smem_attribute<8, 2>()) ? rc : run(multi_token_attention_kernel<8, 2, true>, smem8);
+    if (a.int4_kv) return pl.ntile == 1 ? run(multi_token_attention_kernel<4, 1, true>, smem4) : run(multi_token_attention_kernel<4, 2, true>, smem4);
+    return pl.ntile == 1 ? run(multi_token_attention_kernel<8, 1, true>, smem8) : run(multi_token_attention_kernel<8, 2, true>, smem8);
   }
   if (a.int4_kv) return pl.ntile == 1 ? run(multi_token_attention_kernel<4, 1, false>, smem4) : run(multi_token_attention_kernel<4, 2, false>, smem4);
   return pl.ntile == 1 ? run(multi_token_attention_kernel<8, 1, false>, smem8) : run(multi_token_attention_kernel<8, 2, false>, smem8);

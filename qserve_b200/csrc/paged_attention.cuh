@@ -33,11 +33,6 @@ __device__ __forceinline__ uint32_t pack_f2h2(float lo, float hi) {
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
   return d;
 }
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 constexpr uint32_t kMagic = 0x64006400u;      // half2(1024, 1024)
 constexpr uint32_t kOnesH2 = 0x3c003c00u;     // half2(1, 1)
 

@@ -10,35 +10,27 @@
 //        page into registers and writes 256 B of fp16 into the K or V ring slot in exactly the 128-byte-swizzled [128 rows][64 halfs] x 2 layout
 //        a TMA box produces (16-byte chunk c of row r at chunk c ^ (r & 7)); rows >= P_b are written as zeros (unwritten page slots hold
 //        arbitrary bytes, and NaN * 0 is NaN).  For a chunk block one elected thread issues the TMA loads, as prefill_attention.cu does.
-//   WG1, WG2  consumers (setmaxnreg 224), the two warpgroups of prefill_attention.cu unchanged: S = Q K^T from shared memory, online softmax
-//        in registers, O += P V with P from registers and V as the MN-major operand.
+//   WG1, WG2  consumers (setmaxnreg 224), the two warpgroups of prompt_attention.cuh that prefill_attention.cu runs too: S = Q K^T from
+//        shared memory, online softmax in registers, O += P V with P from registers and V as the MN-major operand.
 // Key blocks: first the ceil(P_b / 128) prefix blocks (keys >= P_b of the last one masked to -inf), then the chunk blocks aligned to the chunk
 // start, so that no block mixes prefix and chunk keys and the diagonal mask of the prompt kernel applies unchanged.  No atomics: the result is
 // deterministic run to run.  Shared memory: the Q tile and the two-deep K / V ring, 160 KB, as in prefill_attention.cu.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
-#include <math_constants.h>
 
 #include <climits>
 
 #include "common.cuh"
-#include "launch.h"
+#include "launch.cuh"
+#include "prompt_attention.cuh"
 
 namespace qs {
 namespace {
 
-constexpr int kD = 128;         // head dim
-constexpr int kBQ = 128;        // query rows per CTA (two consumer warpgroups x m64)
-constexpr int kBKV = 128;       // keys per block
-constexpr int kStages = 2;      // K / V ring depth
 constexpr int kThreads = 384;   // warps 0..3: producer warpgroup, warps 4..11: two consumer warpgroups
 constexpr int kProducers = 128;
 constexpr int kPageTokens = 64;
-constexpr int kTileBytes = kBQ * kD * 2;      // 32 KB: two swizzled [128 rows x 64 halfs] sub-tiles
-constexpr int kSubBytes = kTileBytes / 2;     // 16 KB
-constexpr int kOffQ = 0, kOffK = kTileBytes, kOffV = kOffK + kStages * kTileBytes, kOffBar = kOffV + kStages * kTileBytes;
-constexpr int kSmemBytes = kOffBar + 128;
 // register split of the 64 K-register file: 128 x 56 + 256 x 224 = 64512
 constexpr int kProducerRegs = 56, kConsumerRegs = 224;
 
@@ -46,18 +38,6 @@ template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ uint32_t pack_half2(float a, float b, float& sum) {
-  const __half2 h2 = __floats2half2_rn(a, b);
-  const float2 f = __half22float2(h2);  // the row sum is taken over the ROUNDED probabilities, as in prefill_attention.cu
-  sum += f.x + f.y;
-  return *reinterpret_cast<const uint32_t*>(&h2);
-}
 
 struct PrefixAttnParams {
   const int* cu_seqlens;          // [B + 1] chunk token offsets
@@ -156,27 +136,9 @@ prefix_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   uint8_t* s_q = smem + kOffQ;
   uint8_t* s_k = smem + kOffK;
   uint8_t* s_v = smem + kOffV;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  uint64_t* bar_q = bar;                      // Q tile landed
-  uint64_t* bar_kfull = bar + 1;              // [kStages] K block ready: 128 producer arrivals (+ TMA bytes for a chunk block)
-  uint64_t* bar_kfree = bar_kfull + kStages;  // [kStages] S = Q K^T retired in all eight consumer warps
-  uint64_t* bar_vfull = bar_kfree + kStages;
-  uint64_t* bar_vfree = bar_vfull + kStages;  // O += P V retired in all eight consumer warps
-
+  const RingBarriers bar = ring_barriers(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-    mbar_init(bar_q, 1);
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&bar_kfull[i], kProducers);
-      mbar_init(&bar_kfree[i], 8);
-      mbar_init(&bar_vfull[i], kProducers);
-      mbar_init(&bar_vfree[i], 8);
-    }
-    fence_barrier_init();
-  }
+  if (threadIdx.x == 0) init_ring(bar, kProducers, &tmap_q, &tmap_k, &tmap_v);  // K / V block ready: 128 arrivals (+ TMA bytes for a chunk block)
   __syncthreads();
   if (threadIdx.x == 0) pdl_launch_dependents();
 
@@ -194,9 +156,9 @@ prefix_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     pdl_wait();  // page contents and q / k / v are written by the preceding kernel (RoPE + KV append)
     if (r == 0) {
       const int q_row = seq_start + qb * kBQ;
-      mbar_expect_tx(bar_q, kTileBytes);
-      tma_load_2d(s_q, &tmap_q, h * kD, q_row, bar_q);
-      tma_load_2d(s_q + kSubBytes, &tmap_q, h * kD + 64, q_row, bar_q);
+      mbar_expect_tx(bar.q, kTileBytes);
+      tma_load_2d(s_q, &tmap_q, h * kD, q_row, bar.q);
+      tma_load_2d(s_q + kSubBytes, &tmap_q, h * kD + 64, q_row, bar.q);
     }
     for (int j = 0; j < n_kb; ++j) {
       const int st = j % kStages;
@@ -207,14 +169,14 @@ prefix_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
         const int t = j * kBKV + r;
         const bool live = t < P;
         const int slot = t & (kPageTokens - 1);
-        if (j >= kStages) mbar_wait(&bar_kfree[st], ph ^ 1u);
+        if (j >= kStages) mbar_wait(&bar.kfree[st], ph ^ 1u);
         dequant_row<BITS>(sk, r, live ? reinterpret_cast<const uint8_t*>(kpg) : nullptr, slot, hkv, p);
         fence_proxy_async();  // generic-proxy writes, read by wgmma through the async proxy
-        mbar_arrive(&bar_kfull[st]);
-        if (j >= kStages) mbar_wait(&bar_vfree[st], ph ^ 1u);
+        mbar_arrive(&bar.kfull[st]);
+        if (j >= kStages) mbar_wait(&bar.vfree[st], ph ^ 1u);
         dequant_row<BITS>(sv, r, live ? reinterpret_cast<const uint8_t*>(vpg) : nullptr, slot, hkv, p);
         fence_proxy_async();
-        mbar_arrive(&bar_vfull[st]);
+        mbar_arrive(&bar.vfull[st]);
         const int tn = t + kBKV;
         if (tn < P) {
           kpg = kptrs[tn / kPageTokens];
@@ -222,141 +184,40 @@ prefix_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
         }
       } else {
         const int k_row = seq_start + (j - n_pb) * kBKV;
-        if (j >= kStages) mbar_wait(&bar_kfree[st], ph ^ 1u);
+        if (j >= kStages) mbar_wait(&bar.kfree[st], ph ^ 1u);
         if (r == 0) {
-          mbar_expect_tx(&bar_kfull[st], kTileBytes);
-          tma_load_2d(sk, &tmap_k, hkv * kD, k_row, &bar_kfull[st]);
-          tma_load_2d(sk + kSubBytes, &tmap_k, hkv * kD + 64, k_row, &bar_kfull[st]);
+          mbar_expect_tx(&bar.kfull[st], kTileBytes);
+          tma_load_2d(sk, &tmap_k, hkv * kD, k_row, &bar.kfull[st]);
+          tma_load_2d(sk + kSubBytes, &tmap_k, hkv * kD + 64, k_row, &bar.kfull[st]);
         } else {
-          mbar_arrive(&bar_kfull[st]);
+          mbar_arrive(&bar.kfull[st]);
         }
-        if (j >= kStages) mbar_wait(&bar_vfree[st], ph ^ 1u);
+        if (j >= kStages) mbar_wait(&bar.vfree[st], ph ^ 1u);
         if (r == 0) {
-          mbar_expect_tx(&bar_vfull[st], kTileBytes);
-          tma_load_2d(sv, &tmap_v, hkv * kD, k_row, &bar_vfull[st]);
-          tma_load_2d(sv + kSubBytes, &tmap_v, hkv * kD + 64, k_row, &bar_vfull[st]);
+          mbar_expect_tx(&bar.vfull[st], kTileBytes);
+          tma_load_2d(sv, &tmap_v, hkv * kD, k_row, &bar.vfull[st]);
+          tma_load_2d(sv + kSubBytes, &tmap_v, hkv * kD + 64, k_row, &bar.vfull[st]);
         } else {
-          mbar_arrive(&bar_vfull[st]);
+          mbar_arrive(&bar.vfull[st]);
         }
       }
     }
     return;
   }
 
-  // ===================================== consumers: warpgroup g owns query rows [64 g, 64 g + 64) of the block =====================================
+  // ---- consumers.  Masks: keys >= P of the last prefix block; the causal diagonal of the chunk ----
   setmaxnreg_inc<kConsumerRegs>();
-  const int cw = warp - 4;
-  const int g = cw >> 2;
-  const int row_a = g * 64 + (cw & 3) * 16 + (lane >> 2);  // this thread's two rows: row_a and row_a + 8
-  const int q_pos_a = qb * kBQ + row_a, q_pos_b = q_pos_a + 8;  // positions within the chunk
-  const int col0 = (lane & 3) * 2;
-  float o[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) o[i] = 0.f;
-  float m_a = -CUDART_INF_F, m_b = -CUDART_INF_F;  // running maxima (log2 domain, scaled)
-  float l_a = 0.f, l_b = 0.f;                      // this thread's share of the row sums
-  mbar_wait(bar_q, 0);
-  for (int j = 0; j < n_kb; ++j) {
-    const int st = j % kStages;
-    const uint32_t ph = static_cast<uint32_t>(j / kStages) & 1u;
-    const uint8_t* sk = s_k + st * kTileBytes;
-    const uint8_t* sv = s_v + st * kTileBytes;
-    mbar_wait(&bar_kfull[st], ph);
-    float s[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) s[i] = 0.f;
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < kD / 16; ++ks) {
-      const uint32_t off = (ks >> 2) * kSubBytes;
-      const uint64_t adesc = gmma_desc_sw128(smem_u32(s_q + off + g * 64 * 128)) + (ks & 3) * 2;
-      const uint64_t bdesc = gmma_desc_sw128(smem_u32(sk + off)) + (ks & 3) * 2;
-      wgmma_f16_ss_n128(s, adesc, bdesc, 1u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bar_kfree[st]);
-
-    // ---- masks: keys >= P of the last prefix block; the causal diagonal of the chunk.  Key k is visible to a row iff k <= lim ----
+  consume(smem, warp - 4, lane, qb, n_kb, p.scale_log2, p.out, p.out_stride, seq_start, seq_len, h, [&](int j, int q_pos_a, int q_pos_b) {
     const bool pre = j < n_pb;
     const int kbase = (pre ? j : j - n_pb) * kBKV;
-    const bool masked = pre ? (kbase + kBKV > P) : (j - n_pb == qb);
-    const int lim_a = pre ? P - 1 : q_pos_a, lim_b = pre ? P - 1 : q_pos_b;
-    float mx_a = -CUDART_INF_F, mx_b = -CUDART_INF_F;
-#pragma unroll
-    for (int c = 0; c < kBKV / 8; ++c)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = kbase + c * 8 + col0 + (e & 1);
-        float& v = s[c * 4 + e];
-        if (e < 2) {
-          if (masked && key > lim_a) v = -CUDART_INF_F;  // -inf: exp2 turns it into an exact 0
-          mx_a = fmaxf(mx_a, v);
-        } else {
-          if (masked && key > lim_b) v = -CUDART_INF_F;
-          mx_b = fmaxf(mx_b, v);
-        }
-      }
-#pragma unroll
-    for (int sh = 1; sh <= 2; sh <<= 1) {
-      mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, sh));
-      mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, sh));
-    }
-    // the first key of every block (prefix key 128 j < P, or chunk key 128 jj <= q_pos) is visible: the maxima are finite from block 0 on
-    const float mn_a = fmaxf(m_a, mx_a * p.scale_log2), mn_b = fmaxf(m_b, mx_b * p.scale_log2);
-    const float alpha_a = ex2_approx(m_a - mn_a), alpha_b = ex2_approx(m_b - mn_b);  // 0 on the first block (m = -inf)
-    m_a = mn_a;
-    m_b = mn_b;
-    l_a *= alpha_a;
-    l_b *= alpha_b;
-#pragma unroll
-    for (int c = 0; c < kD / 8; ++c) {
-      o[c * 4 + 0] *= alpha_a; o[c * 4 + 1] *= alpha_a;
-      o[c * 4 + 2] *= alpha_b; o[c * 4 + 3] *= alpha_b;
-    }
-    uint32_t pa[kBKV / 16][4];
-#pragma unroll
-    for (int kk = 0; kk < kBKV / 16; ++kk)
-#pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
-        const float* sc = s + (2 * kk + hf) * 4;
-        pa[kk][2 * hf + 0] = pack_half2(ex2_approx(fmaf(sc[0], p.scale_log2, -m_a)), ex2_approx(fmaf(sc[1], p.scale_log2, -m_a)), l_a);
-        pa[kk][2 * hf + 1] = pack_half2(ex2_approx(fmaf(sc[2], p.scale_log2, -m_b)), ex2_approx(fmaf(sc[3], p.scale_log2, -m_b)), l_b);
-      }
-    mbar_wait(&bar_vfull[st], ph);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < kBKV / 16; ++kk) wgmma_f16_rs_n128_tb(o, pa[kk], gmma_desc_sw128(smem_u32(sv + kk * 2048), kSubBytes));
-    wgmma_commit();
-    wgmma_wait<0>();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bar_vfree[st]);
-  }
-  // ---- epilogue: O / l -> fp16 ----
-#pragma unroll
-  for (int sh = 1; sh <= 2; sh <<= 1) {
-    l_a += __shfl_xor_sync(0xffffffffu, l_a, sh);
-    l_b += __shfl_xor_sync(0xffffffffu, l_b, sh);
-  }
-  const float inv_a = 1.f / l_a, inv_b = 1.f / l_b;
-  __half* dst_a = p.out + static_cast<long long>(seq_start + q_pos_a) * p.out_stride + h * kD + col0;
-  __half* dst_b = dst_a + 8 * p.out_stride;
-  const bool valid_a = q_pos_a < seq_len, valid_b = q_pos_b < seq_len;
-#pragma unroll
-  for (int c = 0; c < kD / 8; ++c) {
-    if (valid_a) *reinterpret_cast<__half2*>(dst_a + c * 8) = __floats2half2_rn(o[c * 4 + 0] * inv_a, o[c * 4 + 1] * inv_a);
-    if (valid_b) *reinterpret_cast<__half2*>(dst_b + c * 8) = __floats2half2_rn(o[c * 4 + 2] * inv_b, o[c * 4 + 3] * inv_b);
-  }
+    return BlockMask{pre ? (kbase + kBKV > P) : (j - n_pb == qb), kbase, pre ? P - 1 : q_pos_a, pre ? P - 1 : q_pos_b};
+  });
 }
 
 }  // namespace
 
 int prefix_attention(const PrefixAttnArgs& a) {
-  QS_REQUIRE(a.head_dim == kD, "prefix_prefill_attention: head_dim=%d (only 128 is built)", a.head_dim);
-  QS_REQUIRE(a.num_heads > 0 && a.num_kv_heads > 0 && a.num_heads % a.num_kv_heads == 0, "prefix_prefill_attention: heads=%d kv_heads=%d", a.num_heads,
-             a.num_kv_heads);
-  QS_REQUIRE(a.batch >= 0 && a.num_tokens >= 0 && a.max_seqlen >= 0 && a.max_prefix_len >= 0, "prefix_prefill_attention: negative size");
+  QS_REQUIRE(a.max_prefix_len >= 0, "prefix_prefill_attention: negative size");
   QS_REQUIRE(a.tokens_per_block == kPageTokens, "prefix_prefill_attention: tokens_per_block=%d, only 64 is supported", a.tokens_per_block);
   const int bits = a.int4_kv ? 4 : 8;
   QS_REQUIRE(a.size_per_token == a.num_kv_heads * kD * bits / 8, "prefix_prefill_attention: size_per_token=%d does not match %d kv heads x %d bits",
@@ -364,22 +225,11 @@ int prefix_attention(const PrefixAttnArgs& a) {
   QS_REQUIRE(static_cast<long long>(a.max_prefix_len) + a.max_seqlen <= static_cast<long long>(a.max_blocks) * kPageTokens,
              "prefix_prefill_attention: max_prefix_len %d + max_seqlen %d exceed the page table (%d blocks of %d tokens)", a.max_prefix_len, a.max_seqlen,
              a.max_blocks, kPageTokens);
-  if (a.batch == 0 || a.num_tokens == 0 || a.max_seqlen == 0) return QS_OK;
-  QS_REQUIRE(a.batch <= 65535 && a.num_heads <= 65535, "prefix_prefill_attention: batch=%d / heads=%d exceed the grid limits", a.batch, a.num_heads);
-  QS_REQUIRE(a.q && a.k && a.v && a.out && a.cu_seqlens && a.prefix_lens && a.kv_pointers, "prefix_prefill_attention: null pointer");
-  QS_REQUIRE(a.q_stride % 8 == 0 && a.k_stride % 8 == 0 && a.v_stride % 8 == 0 && a.out_stride % 8 == 0,
-             "prefix_prefill_attention: row strides must be multiples of 8 halfs");
-  QS_REQUIRE(((reinterpret_cast<uintptr_t>(a.q) | reinterpret_cast<uintptr_t>(a.k) | reinterpret_cast<uintptr_t>(a.v) | reinterpret_cast<uintptr_t>(a.out)) & 15) == 0,
-             "prefix_prefill_attention: q, k, v, out must be 16-byte aligned");
-  QS_REQUIRE(a.q_stride >= a.num_heads * kD && a.k_stride >= a.num_kv_heads * kD && a.v_stride >= a.num_kv_heads * kD && a.out_stride >= a.num_heads * kD,
-             "prefix_prefill_attention: row stride smaller than the row");
+  bool empty = false;
   CUtensorMap tq, tk, tv;
-  int rc = make_tmap_f16(&tq, a.q, a.num_tokens, static_cast<uint64_t>(a.num_heads) * kD, a.q_stride);
-  if (rc) return rc;
-  rc = make_tmap_f16(&tk, a.k, a.num_tokens, static_cast<uint64_t>(a.num_kv_heads) * kD, a.k_stride);
-  if (rc) return rc;
-  rc = make_tmap_f16(&tv, a.v, a.num_tokens, static_cast<uint64_t>(a.num_kv_heads) * kD, a.v_stride);
-  if (rc) return rc;
+  int rc = prompt_attention_prepare(a, "prefix_prefill_attention", &empty, &tq, &tk, &tv);
+  if (rc || empty) return rc;
+  QS_REQUIRE(a.prefix_lens && a.kv_pointers, "prefix_prefill_attention: null pointer");
   PrefixAttnParams p{};
   p.cu_seqlens = a.cu_seqlens;
   p.prefix_lens = a.prefix_lens;
@@ -391,27 +241,11 @@ int prefix_attention(const PrefixAttnArgs& a) {
   p.max_blocks = a.max_blocks;
   p.code_bytes = kPageTokens * a.size_per_token;
   p.scale_log2 = a.softmax_scale * 1.4426950408889634f;
-  auto run = [&](auto kern) {
-    static bool attr_set[2][kMaxDevices] = {};
-    bool& done = attr_set[a.int4_kv ? 0 : 1][device_ordinal()];
-    if (!done) {
-      const int r = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes), "cudaFuncSetAttribute(prefix attention)");
-      if (r) return r;
-      done = true;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((a.max_seqlen + kBQ - 1) / kBQ, a.num_heads, a.batch);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = kSmemBytes;
-    cfg.stream = static_cast<cudaStream_t>(a.stream);
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return check_cuda(cudaLaunchKernelEx(&cfg, kern, tq, tk, tv, p), "prefix prefill attention launch");
-  };
-  return a.int4_kv ? run(prefix_attention_kernel<4>) : run(prefix_attention_kernel<8>);
+  auto kern = a.int4_kv ? prefix_attention_kernel<4> : prefix_attention_kernel<8>;
+  rc = raise_smem_limit(kern, kSmemBytes, "cudaFuncSetAttribute(prefix attention)");
+  if (rc) return rc;
+  return launch(kern, dim3((a.max_seqlen + kBQ - 1) / kBQ, a.num_heads, a.batch), dim3(kThreads), kSmemBytes, 0, a.stream,
+                "prefix prefill attention launch", tq, tk, tv, p);
 }
 
 }  // namespace qs

@@ -26,7 +26,7 @@
 // Both kernels read everything a preceding kernel may write (logits, drafts, mask, parameters, offsets) after griddepcontrol.wait, need no
 // host synchronisation and can be captured in a CUDA graph.
 #include "common.cuh"
-#include "launch.h"
+#include "launch.cuh"
 
 namespace qs {
 namespace {
@@ -514,27 +514,6 @@ __global__ void __launch_bounds__(kThreads, 1) tree_accept_sampling_kernel(
 
 int slice_cap_of(int V) { return ((V / 8 + kCluster - 1) / kCluster) * 8; }
 
-template <typename Kern, typename... Args>
-int launch_cluster(Kern kern, int clusters, size_t smem, void* stream, const char* what, Args... args) {
-  int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), what);
-  if (rc) return rc;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(clusters) * kCluster);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  attr[1].id = cudaLaunchAttributeClusterDimension;
-  attr[1].val.clusterDim.x = kCluster;
-  attr[1].val.clusterDim.y = 1;
-  attr[1].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  return check_cuda(cudaLaunchKernelEx(&cfg, kern, args...), what);
-}
-
 }  // namespace
 
 int sample_rows(const SampleArgs& a) {
@@ -544,8 +523,11 @@ int sample_rows(const SampleArgs& a) {
   if (a.rows == 0) return QS_OK;
   QS_REQUIRE(a.out && a.logits && a.temperature && a.top_k && a.top_p && a.offsets, "sample_rows: null pointer");
   const int cap = slice_cap_of(a.vocab);
-  return launch_cluster(sample_rows_kernel, a.rows, static_cast<size_t>(cap) * 2, a.stream, "sample_rows", a.out,
-                        static_cast<const __half*>(a.logits), a.temperature, a.top_k, a.top_p, static_cast<u64>(a.seed), a.offsets, a.vocab);
+  const size_t smem = static_cast<size_t>(cap) * 2;
+  const int rc = raise_smem_limit(sample_rows_kernel, smem, "sample_rows");
+  if (rc) return rc;
+  return launch(sample_rows_kernel, dim3(static_cast<unsigned>(a.rows) * kCluster), dim3(kThreads), smem, kCluster, a.stream, "sample_rows", a.out,
+                static_cast<const __half*>(a.logits), a.temperature, a.top_k, a.top_p, static_cast<u64>(a.seed), a.offsets, a.vocab);
 }
 
 int tree_accept_sampling(const TreeAcceptSamplingArgs& a) {
@@ -558,9 +540,12 @@ int tree_accept_sampling(const TreeAcceptSamplingArgs& a) {
   QS_REQUIRE(a.draft && a.tree_mask && a.logits && a.temperature && a.top_k && a.top_p && a.offsets && a.accept_len && a.path && a.bonus,
              "tree_accept_sampling: null pointer");
   const int cap = slice_cap_of(a.vocab);
-  return launch_cluster(tree_accept_sampling_kernel, a.batch, static_cast<size_t>(cap) * 6, a.stream, "tree_accept_sampling", a.draft, a.tree_mask,
-                        static_cast<const __half*>(a.logits), a.draft_probs, a.temperature, a.top_k, a.top_p, static_cast<u64>(a.seed), a.offsets,
-                        a.accept_len, a.path, a.bonus, a.num_nodes, a.vocab, cap);
+  const size_t smem = static_cast<size_t>(cap) * 6;  // above the default 48 KB for V > 65536
+  const int rc = raise_smem_limit(tree_accept_sampling_kernel, smem, "tree_accept_sampling");
+  if (rc) return rc;
+  return launch(tree_accept_sampling_kernel, dim3(static_cast<unsigned>(a.batch) * kCluster), dim3(kThreads), smem, kCluster, a.stream,
+                "tree_accept_sampling", a.draft, a.tree_mask, static_cast<const __half*>(a.logits), a.draft_probs, a.temperature, a.top_k, a.top_p,
+                static_cast<u64>(a.seed), a.offsets, a.accept_len, a.path, a.bonus, a.num_nodes, a.vocab, cap);
 }
 
 }  // namespace qs

@@ -12,7 +12,7 @@
 #include <type_traits>
 
 #include "common.cuh"
-#include "launch.h"
+#include "launch.cuh"
 
 namespace qs {
 namespace {
@@ -119,20 +119,6 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) kv_compact_kernel(const lon
   }
 }
 
-template <typename Kern, typename... Args>
-int launch(Kern kern, long long ctas, void* stream, const char* what, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(ctas));
-  cfg.blockDim = dim3(kWarpsPerCta * 32);
-  cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return check_cuda(cudaLaunchKernelEx(&cfg, kern, args...), what);
-}
-
 }  // namespace
 
 int tree_accept_greedy(const long long* draft, const int* tree_mask, const long long* target, int* accept_len, int* path, long long* bonus,
@@ -140,8 +126,8 @@ int tree_accept_greedy(const long long* draft, const int* tree_mask, const long 
   QS_REQUIRE(batch >= 0 && num_nodes >= 1 && num_nodes <= kMaxNodes, "tree_accept_greedy: batch=%d, num_nodes=%d (1 .. 16)", batch, num_nodes);
   if (batch == 0) return QS_OK;
   QS_REQUIRE(draft && tree_mask && target && accept_len && path && bonus, "tree_accept_greedy: null pointer");
-  return launch(tree_accept_kernel, (batch + kWarpsPerCta - 1) / kWarpsPerCta, stream, "tree_accept_greedy", draft, tree_mask, target, accept_len,
-                path, bonus, batch, num_nodes);
+  return launch(tree_accept_kernel, dim3((batch + kWarpsPerCta - 1) / kWarpsPerCta), dim3(kWarpsPerCta * 32), 0, 0, stream, "tree_accept_greedy", draft,
+                tree_mask, target, accept_len, path, bonus, batch, num_nodes);
 }
 
 int kv_cache_compact(const KvCompactArgs& a) {
@@ -158,11 +144,9 @@ int kv_cache_compact(const KvCompactArgs& a) {
   const long long ctas = (n_warps + kWarpsPerCta - 1) / kWarpsPerCta;
   QS_REQUIRE(ctas <= 0x7fffffffLL, "kv_cache_compact: grid too large");
   const int code_bytes = kTokensPerPage * a.size_per_token;
-  if (a.int4_kv)
-    return launch(kv_compact_kernel<4>, ctas, a.stream, "kv_cache_compact", a.kv_pointers, a.start_pos, a.path, a.accept_len, a.batch, a.num_nodes,
-                  a.max_blocks, a.num_kv_heads, code_bytes, n_warps);
-  return launch(kv_compact_kernel<8>, ctas, a.stream, "kv_cache_compact", a.kv_pointers, a.start_pos, a.path, a.accept_len, a.batch, a.num_nodes,
-                a.max_blocks, a.num_kv_heads, code_bytes, n_warps);
+  return launch(a.int4_kv ? kv_compact_kernel<4> : kv_compact_kernel<8>, dim3(static_cast<unsigned>(ctas)), dim3(kWarpsPerCta * 32), 0, 0, a.stream,
+                "kv_cache_compact", a.kv_pointers, a.start_pos, a.path, a.accept_len, a.batch, a.num_nodes, a.max_blocks, a.num_kv_heads, code_bytes,
+                n_warps);
 }
 
 }  // namespace qs
