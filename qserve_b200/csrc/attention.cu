@@ -54,11 +54,8 @@ __device__ __forceinline__ uint32_t kv_quant_code(float x, float inv_s, float z)
 //   side, output rows rescaled at the end on the V side); sum_d (1024 + w_d u_d) q'_d = B(q) + sum_d u_d q_d with B(q) computed
 //   once per head, and sum_t p'_t (1024 + u_t) = 1024 sum_t p'_t + ... with sum_t p'_t from one MMA against an all-ones tile.
 // ------------------------------------------------------------------------------------------------
-// Page geometry, stage layout, biased-operand and MMA helpers, and the main-loop pieces shared with multi_token_attention_kernel:
-// paged_attention.cuh.  This kernel calls q_operand and merge_warps from there.  The other pieces (slice_ptrs / issue_slice, slice_meta,
-// qk_chunk, chunk_logits, softmax_tile, pv_chunk, reduce_tile_sums / store_partial / own_logit, merge_weights, arrive_last / merge_splits)
-// are the same arithmetic as the inline code below, which is kept as it is: calling any one of them here changes the SASS ptxas emits for
-// this kernel (DESIGN.md 3.6), and its code is pinned.  A fix to one of them must be made in both places.
+// This kernel and multi_token_attention_kernel are both built on paged_attention.cuh (one n8 tile here: the <= 8 heads of the group); the
+// output bits of this kernel are pinned by tests/test_gpu_attention.py::test_decode_attention_output_bits_are_pinned.
 constexpr int kAttnThreadsV2 = kAttnConsumers;  // no dedicated producer warp: every warp streams its own half pages
 
 template <int BITS>
@@ -125,29 +122,10 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
   uint8_t* my_ring = s_ring + warp * SL::kWarpBytes;
   uint64_t* my_full = &s_full[warp][0];
   const int zoff = pg.num_kv_heads * pg.tokens_per_block * 2;  // bytes from a scale row to the zero row
-  long long kp_l = 0, vp_l = 0;  // lane l: page pointers of this warp's page (batch * 32 + l)
-  auto load_ptr_batch = [&](int j0) {
-    const int pidx = my_first + 2 * (j0 + lane);
-    kp_l = (pidx < p_end) ? kptrs[pidx] : 0;
-    vp_l = (pidx < p_end) ? vptrs[pidx] : 0;
-  };
-  auto issue = [&](int j, int slot) {  // all lanes call; lane 0 issues the six copies of this warp's j-th slice into `slot`
-    const long long kp_j = __shfl_sync(0xffffffffu, kp_l, j & 31), vp_j = __shfl_sync(0xffffffffu, vp_l, j & 31);
-    if (lane == 0) {
-      const uint8_t* kpage = reinterpret_cast<const uint8_t*>(kp_j);
-      const uint8_t* vpage = reinterpret_cast<const uint8_t*>(vp_j);
-      uint8_t* dst = my_ring + slot * SL::kBytes;
-      fence_proxy_async();  // the slot was last read through the generic proxy
-      mbar_expect_tx(&my_full[slot], SL::kBytes);
-      bulk_copy_g2s(dst + SL::kOffK, kpage + static_cast<size_t>(hk) * SL::kCodes + hslice * SL::kSliceCodes, SL::kSliceCodes, &my_full[slot]);
-      bulk_copy_g2s(dst + SL::kOffV, vpage + static_cast<size_t>(hk) * SL::kCodes + hslice * SL::kSliceCodes, SL::kSliceCodes, &my_full[slot]);
-      const uint8_t* kmeta = kpage + pg.code_bytes + hk * 128 + hslice * 64;
-      const uint8_t* vmeta = vpage + pg.code_bytes + hk * 128 + hslice * 64;
-      bulk_copy_g2s(dst + SL::kOffKs, kmeta, 64, &my_full[slot]);
-      bulk_copy_g2s(dst + SL::kOffKz, kmeta + zoff, 64, &my_full[slot]);
-      bulk_copy_g2s(dst + SL::kOffVs, vmeta, 64, &my_full[slot]);
-      bulk_copy_g2s(dst + SL::kOffVz, vmeta + zoff, 64, &my_full[slot]);
-    }
+  long long kp_l = 0, vp_l = 0;  // lane l: page pointers of this warp's slice (batch * 32 + l)
+  auto load_ptr_batch = [&](int j0) { slice_ptrs(kptrs, vptrs, my_first + 2 * (j0 + lane), p_end, kp_l, vp_l); };
+  auto issue = [&](int j, int slot) {
+    issue_slice<BITS>(lane, kp_l, vp_l, j, my_ring + slot * SL::kBytes, &my_full[slot], hk, hslice, pg.code_bytes, zoff);
   };
   load_ptr_batch(0);
   pdl_wait();
@@ -235,15 +213,18 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
     uint32_t qb0[8], qb1[8];
     float sumq[1][2], biasq[1][2];  // heads 2*q4 and 2*q4+1 (this thread's S^T columns)
     q_operand<BITS>(s_q + g * kD + 32 * q4, q4, qb0, qb1, sumq[0], biasq[0]);
+    auto qb = [&](int, int ks, uint32_t& b0, uint32_t& b1) {  // the Q fragments stay in registers
+      b0 = qb0[ks];
+      b1 = qb1[ks];
+    };
 
-    const float sumq0 = sumq[0][0], sumq1 = sumq[0][1], biasq0 = biasq[0][0], biasq1 = biasq[0][1];  // heads 2q4, 2q4+1
     const float sm_scale = rsqrtf(static_cast<float>(kD)) * 1.4426950408889634f;  // 1/sqrt(D) * log2(e)
     // O^T accumulators: m-tile i (dims 16g + 2i, 16g + 2i + 1) x heads (2q4, 2q4+1)
-    float o[8][4];
+    float o[1][8][4];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+    for (int i = 0; i < 8; ++i) o[0][i][0] = o[0][i][1] = o[0][i][2] = o[0][i][3] = 0.f;
     // running max, sum p, sum p*c (zero-point correction), sum p' (bias correction of the V operand) per head
-    float m0 = -CUDART_INF_F, m1 = -CUDART_INF_F, l0 = 0.f, l1 = 0.f, cr0 = 0.f, cr1 = 0.f;
+    float m[2] = {-CUDART_INF_F, -CUDART_INF_F}, l[2] = {0.f, 0.f}, cr[2] = {0.f, 0.f};
     float spa[4] = {0.f, 0.f, 0.f, 0.f};  // [0], [1]: sum p' of heads 2q4, 2q4+1 over ALL tokens this warp has seen
 
     // S^T = K Q^T: A rows g / g+8 <-> chunk tokens tokA / 8+tokA (the permutation keeps the V row reads at a 2-way conflict)
@@ -261,160 +242,32 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
       if (threadIdx.x == 0 && j == 0) ATTN_PROF(5);
       const uint8_t* st = my_ring + s * SL::kBytes;
       const int t0 = pidx * kPageTokens + hbase;  // first token of this warp's 32-token slice
-      if (t0 < tlen) {
-        // per-token (scale, c = -scale * zero) pairs of the 32 K and 32 V tokens, converted to fp32 ONCE per token here
-        // (fp16 -> fp32 conversions run on the slow XU pipe: the logit code below must not repeat them per thread)
-        {
-          const __half* kp = reinterpret_cast<const __half*>(st + SL::kOffKs) + lane;
-          const __half* vp = reinterpret_cast<const __half*>(st + SL::kOffVs) + lane;
-          const __half ksc = kp[0], kzp = kp[32], vsc = vp[0], vzp = vp[32];
-          float2 fk, fv;
-          if constexpr (BITS == 4) {
-            // c = half(-s * z): the fp16 product of two fp16 values, rounded once
-            fk = __half22float2(__halves2half2(ksc, __hmul(__hneg(ksc), kzp)));
-            fv = __half22float2(__halves2half2(vsc, __hmul(__hneg(vsc), vzp)));
-          } else {
-            fk = __half22float2(__halves2half2(ksc, kzp));
-            fv = __half22float2(__halves2half2(vsc, vzp));
-            fk.y = -fk.x * fk.y;  // aux holds the zero point: c = -s * z in fp32
-            fv.y = -fv.x * fv.y;
-          }
-          fk.x *= sm_scale;
-          fk.y *= sm_scale;
-          if (t0 + lane >= tlen) fk = fv = make_float2(0.f, 0.f);  // unwritten slots: force finite zeros (their logits are masked below)
-          s_meta[warp][0][lane] = fk;
-          s_meta[warp][1][lane] = fv;
-        }
+      if (t0 < tlen) {  // every processed slice holds at least one valid token, so no column's running max stays -inf
+        slice_meta<BITS>(st, lane, t0 + lane >= tlen, sm_scale, s_meta[warp][0], s_meta[warp][1]);
         __syncwarp();
         // ---- S^T (2 x 16 tokens x 8 heads) on biased codes: 16 MMAs ----
-        float sc[2][4];
+        float sc[2][1][4];
 #pragma unroll
         for (int c = 0; c < 2; ++c) {
-          sc[c][0] = sc[c][1] = sc[c][2] = sc[c][3] = 0.f;
-          const uint8_t* krow = st + SL::kOffK + (c * kChunk + tokA) * kRow;
-          if constexpr (BITS == 4) {
-            const uint4 ka = *reinterpret_cast<const uint4*>(krow + q4 * 16);
-            const uint4 kb = *reinterpret_cast<const uint4*>(krow + 8 * kRow + q4 * 16);
-            const uint32_t wa[4] = {ka.x, ka.y, ka.z, ka.w}, wb[4] = {kb.x, kb.y, kb.z, kb.w};
-#pragma unroll
-            for (int w = 0; w < 4; ++w) {
-              const uint32_t xa = wa[w], xb = wb[w], ta = xa >> 8, tb = xb >> 8;
-              mma_full(sc[c][0], sc[c][1], sc[c][2], sc[c][3], lop3_and_or(xa, 0x000f000fu, kMagic), lop3_and_or(xb, 0x000f000fu, kMagic),
-                       lop3_and_or(xa, 0x00f000f0u, kMagic), lop3_and_or(xb, 0x00f000f0u, kMagic), qb0[2 * w], qb1[2 * w]);
-              mma_full(sc[c][0], sc[c][1], sc[c][2], sc[c][3], lop3_and_or(ta, 0x000f000fu, kMagic), lop3_and_or(tb, 0x000f000fu, kMagic),
-                       lop3_and_or(ta, 0x00f000f0u, kMagic), lop3_and_or(tb, 0x00f000f0u, kMagic), qb0[2 * w + 1], qb1[2 * w + 1]);
-            }
-          } else {
-            const uint4 ka0 = *reinterpret_cast<const uint4*>(krow + q4 * 32), ka1 = *reinterpret_cast<const uint4*>(krow + q4 * 32 + 16);
-            const uint4 kb0 = *reinterpret_cast<const uint4*>(krow + 8 * kRow + q4 * 32), kb1 = *reinterpret_cast<const uint4*>(krow + 8 * kRow + q4 * 32 + 16);
-            const uint32_t wa[8] = {ka0.x, ka0.y, ka0.z, ka0.w, ka1.x, ka1.y, ka1.z, ka1.w};
-            const uint32_t wb[8] = {kb0.x, kb0.y, kb0.z, kb0.w, kb1.x, kb1.y, kb1.z, kb1.w};
-#pragma unroll
-            for (int w = 0; w < 8; ++w) {
-              // bytes -> fp16: 0x6400 | u = 1024 + u
-              mma_full(sc[c][0], sc[c][1], sc[c][2], sc[c][3], __byte_perm(wa[w], kMagic, 0x7150), __byte_perm(wb[w], kMagic, 0x7150),
-                       __byte_perm(wa[w], kMagic, 0x7352), __byte_perm(wb[w], kMagic, 0x7352), qb0[w], qb1[w]);
-            }
-          }
+          sc[c][0][0] = sc[c][0][1] = sc[c][0][2] = sc[c][0][3] = 0.f;
+          qk_chunk<BITS, 1>(st + SL::kOffK + (c * kChunk + tokA) * kRow, q4, sc[c], qb);
         }
         // ---- logits (log2 units) of tokens A = tokA, B = 8 + tokA of both chunks for heads 2q4, 2q4+1 ----
-        float tl[2][4], vs[2][2], vc[2][2];
-        const bool partial = (t0 + 2 * kChunk > tlen);  // only the last page of a sequence
+        float tl[2][1][4], vs[2][2], vc[2][2];
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const float2 fkA = s_meta[warp][0][c * kChunk + tokA], fkB = s_meta[warp][0][c * kChunk + 8 + tokA];
-          const float2 fvA = s_meta[warp][1][c * kChunk + tokA], fvB = s_meta[warp][1][c * kChunk + 8 + tokA];
-          vs[c][0] = fvA.x; vs[c][1] = fvB.x; vc[c][0] = fvA.y; vc[c][1] = fvB.y;
-          tl[c][0] = fmaf(fkA.x, sc[c][0] - biasq0, fkA.y * sumq0);
-          tl[c][1] = fmaf(fkA.x, sc[c][1] - biasq1, fkA.y * sumq1);
-          tl[c][2] = fmaf(fkB.x, sc[c][2] - biasq0, fkB.y * sumq0);
-          tl[c][3] = fmaf(fkB.x, sc[c][3] - biasq1, fkB.y * sumq1);
-        }
-        if (partial) {
+        for (int c = 0; c < 2; ++c) chunk_logits<1>(s_meta[warp][0], s_meta[warp][1], c, tokA, sc[c], biasq, sumq, tl[c], vs[c], vc[c]);
+        if (t0 + 2 * kChunk > tlen) {  // only the last page of a sequence
 #pragma unroll
           for (int c = 0; c < 2; ++c) {
-            if (t0 + c * kChunk + tokA >= tlen) tl[c][0] = tl[c][1] = -CUDART_INF_F;
-            if (t0 + c * kChunk + 8 + tokA >= tlen) tl[c][2] = tl[c][3] = -CUDART_INF_F;
+            if (t0 + c * kChunk + tokA >= tlen) tl[c][0][0] = tl[c][0][1] = -CUDART_INF_F;
+            if (t0 + c * kChunk + 8 + tokA >= tlen) tl[c][0][2] = tl[c][0][3] = -CUDART_INF_F;
           }
         }
-        // online softmax with lazy rescale
-        float mh0 = fmaxf(fmaxf(tl[0][0], tl[0][2]), fmaxf(tl[1][0], tl[1][2]));
-        float mh1 = fmaxf(fmaxf(tl[0][1], tl[0][3]), fmaxf(tl[1][1], tl[1][3]));
-#pragma unroll
-        for (int m = 4; m <= 16; m <<= 1) {
-          mh0 = fmaxf(mh0, __shfl_xor_sync(0xffffffffu, mh0, m));
-          mh1 = fmaxf(mh1, __shfl_xor_sync(0xffffffffu, mh1, m));
-        }
-        const bool n0 = mh0 > m0 + 8.f, n1 = mh1 > m1 + 8.f;  // rescale only when a running max moves by more than 2^8
-        if (__any_sync(0xffffffffu, n0 || n1)) {
-          const float a0 = n0 ? exp2f(m0 - mh0) : 1.f, a1 = n1 ? exp2f(m1 - mh1) : 1.f;
-          if (n0) m0 = mh0;
-          if (n1) m1 = mh1;
-          l0 *= a0; cr0 *= a0; l1 *= a1; cr1 *= a1;
-          spa[0] *= a0; spa[2] *= a0; spa[1] *= a1; spa[3] *= a1;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            o[i][0] *= a0; o[i][2] *= a0;
-            o[i][1] *= a1; o[i][3] *= a1;
-          }
-        }
-        uint32_t bp[2][2];
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const float pA0 = ex2_approx(tl[c][0] - m0), pA1 = ex2_approx(tl[c][1] - m1);
-          const float pB0 = ex2_approx(tl[c][2] - m0), pB1 = ex2_approx(tl[c][3] - m1);
-          l0 += pA0 + pB0; l1 += pA1 + pB1;
-          cr0 = fmaf(pA0, vc[c][0], fmaf(pB0, vc[c][1], cr0));
-          cr1 = fmaf(pA1, vc[c][0], fmaf(pB1, vc[c][1], cr1));
-          // P' = p * s_v rounded to fp16 (the MMA operand); its exact sum removes the 1024 bias of the V operand afterwards
-          const uint32_t hA = pack_f2h2(pA0 * vs[c][0], pA1 * vs[c][0]), hB = pack_f2h2(pB0 * vs[c][1], pB1 * vs[c][1]);
-          // P'^T fragments: transpose the (token, head) tiles so that tokens become the MMA k index
-          bp[c][0] = movmatrix_trans(hA);  // k = 2q4, 2q4+1  <-> chunk tokens q4, 4+q4
-          bp[c][1] = movmatrix_trans(hB);  // k = 2q4+8, +9   <-> chunk tokens 8+q4, 12+q4
-          // sum_t p'_t per head, from the very operand the V MMAs consume: an all-ones A tile (every output row is the sum)
-          mma_full(spa[0], spa[1], spa[2], spa[3], kOnesH2, kOnesH2, kOnesH2, kOnesH2, bp[c][0], bp[c][1]);
-        }
+        uint32_t bp[2][1][2];
+        softmax_tile<1, false>(0, tl, vs, vc, m, l, cr, spa, o[0], bp);
         // ---- O^T += V^T P'^T on biased codes: 2 x 8 MMAs (m-tile = 16 dims) ----
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const uint8_t* vbase = st + SL::kOffV + (c * kChunk + q4) * kRow;
-          if constexpr (BITS == 4) {
-            const uint2 va = *reinterpret_cast<const uint2*>(vbase + g * 8);
-            const uint2 vb = *reinterpret_cast<const uint2*>(vbase + 4 * kRow + g * 8);
-            const uint2 vcw = *reinterpret_cast<const uint2*>(vbase + 8 * kRow + g * 8);
-            const uint2 vd = *reinterpret_cast<const uint2*>(vbase + 12 * kRow + g * 8);
-#pragma unroll
-            for (int ww = 0; ww < 2; ++ww) {
-              const uint32_t a = ww ? va.y : va.x, bb = ww ? vb.y : vb.x, cc = ww ? vcw.y : vcw.x, dd = ww ? vd.y : vd.x;
-#pragma unroll
-              for (int kb = 0; kb < 4; ++kb) {
-                const uint32_t sel = static_cast<uint32_t>(kb) | (static_cast<uint32_t>(kb) << 4) | (static_cast<uint32_t>(4 + kb) << 8) |
-                                     (static_cast<uint32_t>(4 + kb) << 12);  // bytes [a_kb, a_kb, b_kb, b_kb]
-                const uint32_t m01 = __byte_perm(a, bb, sel), m89 = __byte_perm(cc, dd, sel);
-                const int i = 4 * ww + kb;
-                mma_full(o[i][0], o[i][1], o[i][2], o[i][3], lop3_and_or(m01, 0x000f000fu, kMagic), lop3_and_or(m01, 0x00f000f0u, kMagic),
-                         lop3_and_or(m89, 0x000f000fu, kMagic), lop3_and_or(m89, 0x00f000f0u, kMagic), bp[c][0], bp[c][1]);
-              }
-            }
-          } else {
-            const uint4 va = *reinterpret_cast<const uint4*>(vbase + g * 16);
-            const uint4 vb = *reinterpret_cast<const uint4*>(vbase + 4 * kRow + g * 16);
-            const uint4 vcw = *reinterpret_cast<const uint4*>(vbase + 8 * kRow + g * 16);
-            const uint4 vd = *reinterpret_cast<const uint4*>(vbase + 12 * kRow + g * 16);
-            const uint32_t wa[4] = {va.x, va.y, va.z, va.w}, wb[4] = {vb.x, vb.y, vb.z, vb.w};
-            const uint32_t wc[4] = {vcw.x, vcw.y, vcw.z, vcw.w}, wd[4] = {vd.x, vd.y, vd.z, vd.w};
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              // dims 16g + 2i (row g) and 16g + 2i + 1 (row g+8): bytes 2i, 2i+1 of the 16-byte row chunk
-              const int w = i >> 1, b0 = 2 * (i & 1), b1 = b0 + 1;
-              const uint32_t sel0 = static_cast<uint32_t>(b0) | (static_cast<uint32_t>(b0) << 4) | (static_cast<uint32_t>(4 + b0) << 8) | (static_cast<uint32_t>(4 + b0) << 12);
-              const uint32_t sel1 = static_cast<uint32_t>(b1) | (static_cast<uint32_t>(b1) << 4) | (static_cast<uint32_t>(4 + b1) << 8) | (static_cast<uint32_t>(4 + b1) << 12);
-              mma_full(o[i][0], o[i][1], o[i][2], o[i][3], lop3_and_or(__byte_perm(wa[w], wb[w], sel0), 0x00ff00ffu, kMagic),
-                       lop3_and_or(__byte_perm(wa[w], wb[w], sel1), 0x00ff00ffu, kMagic), lop3_and_or(__byte_perm(wc[w], wd[w], sel0), 0x00ff00ffu, kMagic),
-                       lop3_and_or(__byte_perm(wc[w], wd[w], sel1), 0x00ff00ffu, kMagic), bp[c][0], bp[c][1]);
-            }
-          }
-        }
+        for (int c = 0; c < 2; ++c) pv_chunk<BITS, 1>(st + SL::kOffV + (c * kChunk + q4) * kRow, g, o, bp[c]);
       }
       __syncwarp();
       // refill the slot just consumed with the slice R iterations ahead
@@ -427,40 +280,17 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
 
     if (threadIdx.x == 0) ATTN_PROF(6);
     // ---- per-warp partials -> the warp's own (drained) ring: no need to wait for the other warps ----
-#pragma unroll
-    for (int m = 4; m <= 16; m <<= 1) {
-      l0 += __shfl_xor_sync(0xffffffffu, l0, m);
-      l1 += __shfl_xor_sync(0xffffffffu, l1, m);
-      cr0 += __shfl_xor_sync(0xffffffffu, cr0, m);
-      cr1 += __shfl_xor_sync(0xffffffffu, cr1, m);
-    }
+    reduce_tile_sums(l, cr);
     if (g == 0) {
-      s_m[warp][2 * q4] = m0; s_m[warp][2 * q4 + 1] = m1;
-      s_l[warp][2 * q4] = l0; s_l[warp][2 * q4 + 1] = l1;
+      s_m[warp][2 * q4] = m[0]; s_m[warp][2 * q4 + 1] = m[1];
+      s_l[warp][2 * q4] = l[0]; s_l[warp][2 * q4 + 1] = l[1];
     }
-    {
-      // layout [warp][head][(d % 16) * 8 + d / 16] with a head stride of 132 floats: conflict-free for these stores and for the
-      // merge reads below (thread t owns dim 16 (t % 8) + t / 8)
-      __syncwarp();  // every lane is done with the ring slots this overwrites
-      float* so0 = reinterpret_cast<float*>(my_ring) + (2 * q4) * kOStride + g;  // head 2q4, dims 16g + j at offset 8 j
-      float* so1 = so0 + kOStride;                                // head 2q4+1
-      constexpr float hs = (BITS == 4) ? 0.0625f : 1.f;
-      const float b0 = 1024.f * spa[0], b1 = 1024.f * spa[1];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        // remove the operand bias (1024 sum p'); KV4: the odd dims came from the high nibbles, i.e. 16 x the code
-        so0[8 * (2 * i)] = (o[i][0] - b0) + cr0; so0[8 * (2 * i + 1)] = (o[i][2] - b0) * hs + cr0;
-        so1[8 * (2 * i)] = (o[i][1] - b1) + cr1; so1[8 * (2 * i + 1)] = (o[i][3] - b1) * hs + cr1;
-      }
-    }
-    // new token logit: fp32 dot of the rotated, un-quantised q and k  (Template.hpp:1410-1441)
+    __syncwarp();  // every lane is done with the ring slots this overwrites
+    store_partial<BITS>(reinterpret_cast<float*>(my_ring) + (2 * q4) * kOStride + g, o[0], spa, cr);
+    // new token logit: fp32 dot of the rotated, un-quantised q and k
     if (split == 0) {
       for (int r = warp; r < Gc; r += kWarps) {
-        float acc = 0.f;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc = fmaf(__half2float(s_q[r * kD + lane * 4 + j]), __half2float(s_k[lane * 4 + j]), acc);
-#pragma unroll
-        for (int m = 16; m >= 1; m >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, m);
+        const float acc = own_logit(s_q + r * kD, s_k, lane);
         if (lane == 0) {
           s_m[kWarps][r] = acc * sm_scale;
           s_l[kWarps][r] = 1.f;
@@ -472,26 +302,8 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
   if (threadIdx.x == 0) ATTN_PROF(7);
 
   // ---------------- merge the warps (and the un-quantised new token) ----------------
-  const bool owner = (split == 0);
-  const int nparts = kWarps + (owner ? 1 : 0);
-  if (threadIdx.x < kMaxG) {
-    // one thread per head: weights exp2(m_w - M), normalised by 1 / (sum + 1e-6) when this CTA produces the final output
-    const int r = threadIdx.x;
-    float M = -CUDART_INF_F;
-    for (int w = 0; w < nparts; ++w) M = fmaxf(M, s_m[w][r]);
-    float e[kWarps + 1], L = 0.f;
-#pragma unroll
-    for (int w = 0; w < kWarps + 1; ++w) {
-      e[w] = (w < nparts && s_m[w][r] != -CUDART_INF_F) ? exp2f(s_m[w][r] - M) : 0.f;
-      if (w < nparts) L += s_l[w][r] * e[w];
-    }
-    // reference normalisation: 1 / (sum + 1e-6)   (Template.hpp:1818)
-    const float inv = (nsplit == 1) ? __fdividef(1.f, L + 1.e-6f) : 1.f;
-#pragma unroll
-    for (int w = 0; w < kWarps + 1; ++w) s_f[w][r] = e[w] * inv;
-    s_m[0][r] = M;   // only read back by the split path below
-    s_l[0][r] = L;
-  }
+  const int nparts = kWarps + (split == 0 ? 1 : 0);
+  if (threadIdx.x < kMaxG) merge_weights<kMaxG>(threadIdx.x, nparts, nsplit, s_m, s_l, s_f);
   __syncthreads();
   if (threadIdx.x < kD) {
     const int d = 16 * (threadIdx.x & 7) + (threadIdx.x >> 3);  // the dim whose partials sit at offset threadIdx.x
@@ -519,32 +331,13 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
   if (threadIdx.x == 0) ATTN_PROF(8);
   bool final_written = (nsplit == 1);  // this CTA produced the final fp16 outputs of its head group
   if (nsplit > 1) {
-    __threadfence();
-    __syncthreads();
-    uint32_t* cnt = ws_cnt + static_cast<size_t>(b) * gridDim.x + blockIdx.x;
-    if (threadIdx.x == 0) {
-      const uint32_t old = atomicAdd(cnt, 1u);
-      const bool last = (old == static_cast<uint32_t>(nsplit - 1));
-      if (last) *cnt = 0;
-      s_last = last ? 1u : 0u;
-    }
-    __syncthreads();
-    final_written = (s_last != 0);
-    if (s_last && threadIdx.x < kD) {
+    final_written = arrive_last(ws_cnt + static_cast<size_t>(b) * gridDim.x + blockIdx.x, nsplit, s_last);
+    if (final_written && threadIdx.x < kD) {
       const int d = threadIdx.x;
       __threadfence();
       for (int r = 0; r < Gc; ++r) {
         const float* pr = ws_part + (static_cast<size_t>(b) * num_heads + h0 + r) * nsplit * (kD + 2);
-        float M = -CUDART_INF_F;
-        for (int sp = 0; sp < nsplit; ++sp) M = fmaxf(M, __ldcg(pr + sp * (kD + 2) + kD));
-        float L = 0.f, acc = 0.f;
-        for (int sp = 0; sp < nsplit; ++sp) {
-          const float ms = __ldcg(pr + sp * (kD + 2) + kD);
-          const float e = (ms == -CUDART_INF_F) ? 0.f : exp2f(ms - M);
-          L += __ldcg(pr + sp * (kD + 2) + kD + 1) * e;
-          acc += __ldcg(pr + sp * (kD + 2) + d) * e;
-        }
-        out[(static_cast<size_t>(b) * num_heads + h0 + r) * kD + d] = __float2half_rn(acc * __fdividef(1.f, L + 1.e-6f));
+        out[(static_cast<size_t>(b) * num_heads + h0 + r) * kD + d] = __float2half_rn(merge_splits(pr, nsplit, d));
       }
     }
   }
@@ -553,7 +346,7 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
     //      `out` is an fp16 scratch row in the workspace (L2 resident); the last head-group CTA of a token to finish
     //      re-reads the row and quantises it: same arithmetic as quant_per_token_kernel ----
     __shared__ uint32_t s_last_tok;
-    __shared__ float s_red_f[8];
+    __shared__ float s_red_f[8], s_red_nf[8];
     __shared__ long long s_red_l[8];
     __threadfence();
     __syncthreads();
@@ -572,14 +365,17 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
       constexpr int kRowRegs = 8;
       const bool in_regs = nvec <= kRowRegs * kAttnThreadsV2;
       uint4 rv[kRowRegs];
-      float amax = 0.f;
+      float amax = 0.f, nf = 0.f;
       long long sum = 0;
       auto stats = [&](const uint4& v) {
         const __half2* h = reinterpret_cast<const __half2*>(&v);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const float2 f = __half22float2(h[j]);
-          if (q_sum) sum += __float2ll_rn(f.x * 16777216.f) + __float2ll_rn(f.y * 16777216.f);
+          if (q_sum) {
+            sum += fx_of_finite(f.x) + fx_of_finite(f.y);
+            nf += f.x + f.y;  // a thread's fp32 sum of fp16 values cannot overflow: it is non-finite only where the side sum is, and then equals it
+          }
           amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
         }
       };
@@ -595,32 +391,31 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
       } else {
         for (int i = threadIdx.x; i < nvec; i += kAttnThreadsV2) stats(__ldcg(row + i));
       }
+      nf = nonfinite_part(nf);
 #pragma unroll
       for (int m = 16; m >= 1; m >>= 1) {
         amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, m));
         sum += __shfl_xor_sync(0xffffffffu, sum, m);
+        nf += __shfl_xor_sync(0xffffffffu, nf, m);
       }
-      if (lane == 0) { s_red_f[warp] = amax; s_red_l[warp] = sum; }
+      if (lane == 0) { s_red_f[warp] = amax; s_red_l[warp] = sum; s_red_nf[warp] = nf; }
       __syncthreads();
       amax = 0.f;
       sum = 0;
-      for (int w = 0; w < kAttnThreadsV2 / 32; ++w) { amax = fmaxf(amax, s_red_f[w]); sum += s_red_l[w]; }
+      nf = 0.f;
+      for (int w = 0; w < kAttnThreadsV2 / 32; ++w) { amax = fmaxf(amax, s_red_f[w]); sum += s_red_l[w]; nf += s_red_nf[w]; }
       if (threadIdx.x == 0) {
         q_scale[b] = __float2half_rn(__fdiv_rn(amax, 127.f));
-        if (q_sum) q_sum[b] = __float2half_rn(__ll2float_rn(sum) * (1.f / 16777216.f));
+        if (q_sum) q_sum[b] = __float2half_rn(row_sum(sum, nf));
       }
       const float qs_ = __fdiv_rn(127.f, amax);
-      uint2* qrow = reinterpret_cast<uint2*>(q_out + static_cast<size_t>(b) * num_heads * kD);
+      int8_t* qrow = q_out + static_cast<size_t>(b) * num_heads * kD;
       auto quantise = [&](int i, const uint4& v) {
         const __half* h = reinterpret_cast<const __half*>(&v);
-        uint32_t w[2] = {0u, 0u};
+        float x[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          int32_t c;
-          asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(c) : "f"(__fmul_rn(__half2float(h[j]), qs_)));
-          w[j >> 2] |= (static_cast<uint32_t>(c) & 0xffu) << ((j & 3) * 8);
-        }
-        qrow[i] = make_uint2(w[0], w[1]);
+        for (int j = 0; j < 8; ++j) x[j] = __half2float(h[j]);
+        store_q8(qrow, i, x, qs_);
       };
       if (in_regs) {
 #pragma unroll

@@ -70,6 +70,39 @@ __device__ __forceinline__ bool argmax_better(float v, int i, float bv, int bi) 
   return v > bv || (v == bv && i < bi);
 }
 
+// ---------------------------------------------------------------------------------------------
+// per-token INT8 quantisation (the quantisers of elementwise.cu and the fused epilogue of decode_attention_kernel)
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ int8_t cvt_s8(float x) {
+  int32_t r;
+  asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return static_cast<int8_t>(r);
+}
+// 8 int8 codes cvt_s8(v[j] * scale) = one 64-bit store to vector i8 of the row
+__device__ __forceinline__ void store_q8(int8_t* dst, int i8, const float (&v)[8], float scale) {
+  uint32_t lo = 0, hi = 0;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    lo |= (static_cast<uint32_t>(static_cast<uint8_t>(cvt_s8(__fmul_rn(v[j], scale)))) << (8 * j));
+    hi |= (static_cast<uint32_t>(static_cast<uint8_t>(cvt_s8(__fmul_rn(v[4 + j], scale)))) << (8 * j));
+  }
+  reinterpret_cast<uint2*>(dst)[i8] = make_uint2(lo, hi);
+}
+
+// Exact, order-independent row sums of fp16 values: every fp16 is an integer multiple of 2^-24, so a row of up to 2^14
+// values sums exactly in int64 fixed point; the result is rounded ONCE to fp32 (then to fp16 by the caller).  Bit-identical
+// for every thread count / decomposition and to the oracle's float64 sum.
+__device__ __forceinline__ long long fx_of_half(float f) { return __float2ll_rn(f * 16777216.f); }
+__device__ __forceinline__ float fx_to_float(long long v) { return __ll2float_rn(v) * (1.f / 16777216.f); }
+
+// The quantisers' row sum feeds the per-channel W4A8 GEMM, and must say inf or NaN where the reference's fp32 sum does (an fp16
+// overflow of silu(g) * u, for example).  Fixed point cannot hold those (__float2ll_rn saturates and the next addition wraps), so
+// non-finite addends stay out of it and are summed apart in fp32.  That side sum is 0 for a finite row, +-inf if the row holds
+// infinities of one sign, NaN for +inf with -inf or any NaN -- exactly the IEEE sum's verdict -- and then replaces the exact sum.
+__device__ __forceinline__ long long fx_of_finite(float f) { return isfinite(f) ? fx_of_half(f) : 0ll; }
+__device__ __forceinline__ float nonfinite_part(float f) { return isfinite(f) ? 0.f : f; }
+__device__ __forceinline__ float row_sum(long long fx, float nonfinite) { return nonfinite == 0.f ? fx_to_float(fx) : nonfinite; }
+
 // Programmatic dependent launch (PDL)
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

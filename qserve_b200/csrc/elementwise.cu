@@ -12,12 +12,6 @@ namespace {
 
 constexpr int kThreads = 512;
 
-__device__ __forceinline__ int8_t cvt_s8(float x) {
-  int32_t r;
-  asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return static_cast<int8_t>(r);
-}
-
 template <typename Op>
 __device__ __forceinline__ float warp_reduce(float v, Op op) {
 #pragma unroll
@@ -40,11 +34,7 @@ __device__ __forceinline__ float block_reduce(float v, float* red, Op op, float 
   return r;
 }
 
-// Exact, order-independent row sums of fp16 values: every fp16 is an integer multiple of 2^-24, so a row of up to 2^14
-// values sums exactly in int64 fixed point; the result is rounded ONCE to fp32 (then to fp16 by the caller).  Bit-identical
-// for every thread count / decomposition and to the oracle's float64 sum.
-__device__ __forceinline__ long long fx_of_half(float f) { return __float2ll_rn(f * 16777216.f); }
-__device__ __forceinline__ float fx_to_float(long long v) { return __ll2float_rn(v) * (1.f / 16777216.f); }
+// block-wide sum of the fixed-point row sums (fx_of_half, common.cuh)
 __device__ __forceinline__ long long block_sum_ll(long long v, long long* red) {
 #pragma unroll
   for (int m = 16; m >= 1; m >>= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
@@ -58,13 +48,6 @@ __device__ __forceinline__ long long block_sum_ll(long long v, long long* red) {
   return r;
 }
 
-// The quantisers' row sum feeds the per-channel W4A8 GEMM, and must say inf or NaN where the reference's fp32 sum does (an fp16
-// overflow of silu(g) * u, for example).  Fixed point cannot hold those (__float2ll_rn saturates and the next addition wraps), so
-// non-finite addends stay out of it and are summed apart in fp32.  That side sum is 0 for a finite row, +-inf if the row holds
-// infinities of one sign, NaN for +inf with -inf or any NaN -- exactly the IEEE sum's verdict -- and then replaces the exact sum.
-__device__ __forceinline__ long long fx_of_finite(float f) { return isfinite(f) ? fx_of_half(f) : 0ll; }
-__device__ __forceinline__ float nonfinite_part(float f) { return isfinite(f) ? 0.f : f; }
-__device__ __forceinline__ float row_sum(long long fx, float nonfinite) { return nonfinite == 0.f ? fx_to_float(fx) : nonfinite; }
 // cluster exchange of the silu_mul_quant kernels: one 64-bit word carries the CTA's amax (low half) and non-finite sum (high half)
 __device__ __forceinline__ long long pack_amax_nf(float amax, float nf) {
   return static_cast<long long>((static_cast<unsigned long long>(__float_as_uint(nf)) << 32) | __float_as_uint(amax));
@@ -77,17 +60,6 @@ __device__ __forceinline__ void load_row_to_smem(__half* dst, const __half* src,
   const uint4* s = reinterpret_cast<const uint4*>(src);
   uint4* d = reinterpret_cast<uint4*>(dst);
   for (int i = threadIdx.x; i < H / 8; i += blockDim.x) d[i] = __ldg(s + i);
-}
-
-__device__ __forceinline__ void store_q8(int8_t* dst, int i8, const float (&v)[8], float scale) {
-  // 8 int8 values = one 64-bit store
-  uint32_t lo = 0, hi = 0;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    lo |= (static_cast<uint32_t>(static_cast<uint8_t>(cvt_s8(__fmul_rn(v[j], scale)))) << (8 * j));
-    hi |= (static_cast<uint32_t>(static_cast<uint8_t>(cvt_s8(__fmul_rn(v[4 + j], scale)))) << (8 * j));
-  }
-  reinterpret_cast<uint2*>(dst)[i8] = make_uint2(lo, hi);
 }
 
 // ------------------------------------------------------------------------------------------------

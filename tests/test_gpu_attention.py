@@ -9,6 +9,8 @@ Stated tolerances (floating point, SURVEY.md 8c: the reference itself is order d
   * K pages: RoPE uses sincosf/powf whose last fp32 bit differs from numpy's; scales / zeros within 1 fp16 ulp and
     codes within 1 LSB, with at most 3% of the codes of a token differing.
 """
+import os
+
 import numpy as np
 import pytest
 import torch
@@ -105,6 +107,55 @@ def test_decode_attention(dev, bits, B, Hq, Hkv, lens):
         err_f = np.abs(faithful - exact).max()
         assert err_f <= 1e-2 * scale
         assert err_g <= 1.5 * err_f + 1e-3 * scale, (err_g, err_f)
+
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "decode_attn_bits.npz")
+GOLDEN_CASES = [  # (B, Hq, Hkv, lens): G = 4 with a length-1 sequence, G = 1, G = 16 (two head groups), and context splits at small batch
+    (3, 8, 2, [1, 65, 200]),
+    (2, 4, 4, [300, 31]),
+    (2, 16, 1, [90, 257]),
+    (2, 32, 8, [1025, 700]),
+    (1, 16, 1, [1500]),
+    (1, 64, 64, [2048]),
+]
+
+
+def decode_attn_outputs(dev, case, bits):
+    """The outputs of single_query_attention (fp16 out) and single_query_attention_quant (int8 codes, scale, sum) for GOLDEN_CASES[case],
+    each on a fresh copy of the cache built from a fixed seed, as int16 / int8 tensors on the host."""
+    import qserve_backend.fused_attention as fa
+    from qserve_b200 import backend as ext
+    B, Hq, Hkv, lens = GOLDEN_CASES[case]
+    D = 128
+    kp, vp, bt, q, k, v = _mk(np.random.default_rng(9000 + 10 * case + bits), B, Hq, Hkv, lens, bits)
+    res = {}
+    for fused in (False, True):
+        gk, gv = GpuPool(kp, dev), GpuPool(vp, dev)
+        table = kv_pointer_table(gk, gv, bt, dev)
+        qd, kd, vd = to_dev(q, dev), to_dev(k, dev), to_dev(v, dev)
+        lens_d = torch.tensor(lens, dtype=torch.int32, device=dev)
+        args = (8192, 64, Hkv * D * bits // 8, int(max(lens)), D, ROPE)
+        if fused:
+            oq = torch.empty((B, Hq * D), dtype=torch.int8, device=dev)
+            sc = torch.empty(B, dtype=torch.half, device=dev)
+            sm = torch.empty(B, dtype=torch.half, device=dev)
+            ext.single_query_attention_quant(qd, kd, vd, table, lens_d, *args, bits == 4, True, oq, sc, sm)
+            res.update(codes=oq, scale=sc.view(torch.int16), sum=sm.view(torch.int16))
+        else:
+            res["out"] = fa.single_query_attention(qd, kd, vd, table, lens_d, None, *args, True, bits == 4, True).view(torch.int16)
+    torch.cuda.synchronize()
+    return {key: t.cpu() for key, t in res.items()}
+
+
+@pytest.mark.parametrize("bits", [4, 8])
+@pytest.mark.parametrize("case", range(len(GOLDEN_CASES)))
+def test_decode_attention_output_bits_are_pinned(dev, case, bits):
+    """The output bits of both decode-attention ops equal the stored fixture (tests/golden/make_golden_decode_attn.py, written on an H100
+    with 132 SMs: the context-split count, and so the summation order, depends on the SM count)."""
+    want = np.load(GOLDEN)
+    got = decode_attn_outputs(dev, case, bits)
+    for key, t in got.items():
+        assert torch.equal(t, torch.from_numpy(want[f"kv{bits}_{case}_{key}"])), key
 
 
 def test_decode_attention_config2_properties(dev):

@@ -62,15 +62,23 @@ def test_fused_runner_matches_reference_sequence(dev, precision):
     assert torch.equal(outs[0], outs[1])
 
 
+INF, NAN = float("inf"), float("nan")
+QUANT_CASES = [  # (B, Hq, Hkv, lens, with_sum, non-finite entries (sequence, kv head, dim, value) of the new token's V)
+    (4, 32, 8, [17, 16, 64, 129], True, ()),  # Llama-3 head geometry, no context split -> bit identical to the two-op sequence
+    (3, 8, 2, [1, 65, 200], False, ()),
+    (2, 16, 1, [90, 257], True, ()),          # two head groups per kv head
+    (2, 32, 8, [1025, 700], True, ()),        # context splits: two-level last-CTA merge
+    (1, 64, 64, [2048], True, ()),            # 64 CTAs per token
+    # an overflowed qkv GEMM: the output rows hold inf / NaN, and the row sum must say so as invoke_quant_fuse_sum does
+    (4, 32, 8, [17, 16, 64, 129], True, ((0, 1, 5, INF), (2, 3, 7, NAN))),
+    (2, 32, 8, [1025, 700], True, ((0, 2, 9, INF), (1, 0, 3, INF), (1, 5, 100, -INF))),
+]
+
+
 @pytest.mark.parametrize("bits", [4, 8])
-@pytest.mark.parametrize("B,Hq,Hkv,lens,with_sum", [
-    (4, 32, 8, [17, 16, 64, 129], True),      # Llama-3 head geometry, no context split -> bit identical to the two-op sequence
-    (3, 8, 2, [1, 65, 200], False),
-    (2, 16, 1, [90, 257], True),              # two head groups per kv head
-    (2, 32, 8, [1025, 700], True),            # context splits: two-level last-CTA merge
-    (1, 64, 64, [2048], True),                # 64 CTAs per token
-])
-def test_attention_quant_equals_attention_then_quant(dev, bits, B, Hq, Hkv, lens, with_sum):
+@pytest.mark.parametrize("B,Hq,Hkv,lens,with_sum,bad_v", [
+    pytest.param(*c, id=f"{c[0]}-{c[1]}-{c[2]}-lens{i}-{c[4]}" + ("-nonfinite" if c[5] else "")) for i, c in enumerate(QUANT_CASES)])
+def test_attention_quant_equals_attention_then_quant(dev, bits, B, Hq, Hkv, lens, with_sum, bad_v):
     """single_query_attention_quant == invoke_quant[_fuse_sum](single_query_attention(...)); KV pages updated identically."""
     from oracle import kv
     from qserve_b200 import backend as ext
@@ -80,6 +88,8 @@ def test_attention_quant_equals_attention_then_quant(dev, bits, B, Hq, Hkv, lens
     from tests.util import GpuPool, kv_pointer_table
     rng = np.random.default_rng(B + Hq + sum(lens) + bits)
     kp, vp, bt, q, k, v = _mk(rng, B, Hq, Hkv, lens, bits)
+    for b, h, d, x in bad_v:
+        v[b, h, d] = x
     D = 128
     res = []
     for fused in (False, True):
@@ -105,7 +115,7 @@ def test_attention_quant_equals_attention_then_quant(dev, bits, B, Hq, Hkv, lens
         res.append((oq.cpu(), sc.cpu(), sm.cpu(), gk.download(), gv.download()))
     (q1, s1, m1, k1, v1), (q2, s2, m2, k2, v2) = res
     assert np.array_equal(k1, k2) and np.array_equal(v1, v2)
-    assert torch.equal(q1, q2) and torch.equal(s1, s2) and torch.equal(m1, m2)
+    assert torch.equal(q1, q2) and torch.equal(s1.view(torch.int16), s2.view(torch.int16)) and torch.equal(m1.view(torch.int16), m2.view(torch.int16))
 
 
 @pytest.mark.parametrize("rows,vocab", [(64, 128256), (3, 32000), (1, 1024), (5, 152064)])
