@@ -19,9 +19,9 @@
 //   * weights and activations travel in separate rings with separate producer warps: the weight producer never waits for the previous
 //     kernel, so with programmatic dependent launch the weight ring fills while the preceding norm / quant kernel runs.
 //   * decode shapes have too few 128-channel tiles to fill 132 SMs, so K is split across a thread-block CLUSTER
-//     (2/4/8 CTAs); every CTA pushes its INT32 partials of the channels a peer finishes into that peer's receive buffer
-//     through DISTRIBUTED SHARED MEMORY (st.shared::cluster) and each CTA sums and finishes a 1/S slice of the channels --
-//     integer adds, so the result is bit-identical for every split.
+//     (2/4/8 CTAs); every CTA stages its INT32 partials in its own shared memory and sends each peer the channels that peer finishes
+//     with one bulk copy through DISTRIBUTED SHARED MEMORY (cp.async.bulk.shared::cluster, completing on the peer's mbarrier); each
+//     CTA sums and finishes a 1/S slice of the channels -- integer adds, so the result is bit-identical for every split.
 //   * epilogue fused: acc*s1[n]*sa[m] - s1z[n]*asum[m] (per-channel) or acc*(s1[n]*sa[m]) (per-group, W8A8) -> fp16,
 //     IEEE fp32 in the reference's source order (bit-exact against the oracle).
 #include <cstdarg>
@@ -58,7 +58,7 @@ struct GemmParams {
   int32_t* acc_out;          // optional: raw INT32 accumulators [M, N] (parity tests)
   int M, N, K;
   int m_tiles, kb_per_tile, split;
-  unsigned long long* prof;  // optional: 16 globaltimer stamps per CTA (tools/gemm_timeline.py); slot 15 holds the SM id
+  unsigned long long* prof;  // optional: 16 globaltimer stamps per CTA (tools/gemm_timeline.py); slots 13 / 14 / 15 hold NT, the split, the SM id
 };
 
 // WS = depth of the WEIGHT ring in shared memory.  Weights are static, so the producer streams them before the
@@ -77,13 +77,16 @@ struct Cfg {
   static constexpr int kOffW = kOffAct + AS * kActBytes;
   static constexpr int kOffS2 = kOffW + WS * kWBytes;
   static constexpr int kPipeBytes = kOffS2 + WS * kS2Bytes;
-  // INT32 partials, aliasing the drained pipeline buffers: S == 1: the CTA's own tile [NT][128]; split-K (cluster) launches: the receive
-  // buffer [sender][token][128 / S channels] into which every CTA of the cluster pushes (st.shared::cluster, from the accumulator registers)
-  // the partials of the channels this CTA finishes -- only after a cluster barrier has seen every CTA's mainloop drain
+  // INT32 partials, aliasing the drained pipeline buffers.  S == 1: the CTA's own tile [NT][128] at offset 0.  Split-K (cluster) launches:
+  // at offset 0 the receive buffer [sender][token][128 / S channels], into which the peers copy the partials of the channels this CTA
+  // finishes -- only after a cluster barrier has seen every CTA's mainloop drain; behind it the staging buffer [owner][token][128 / S
+  // channels], which only this CTA writes, so it may be filled as soon as this CTA's own rings have drained.
   static constexpr int kRedBytes = NT * kBM * 4;
+  static constexpr int kOffTx = kRedBytes;
+  static_assert(2 * kRedBytes <= kPipeBytes, "receive and staging buffer must both fit in the drained rings");
   static constexpr int kOffRow = (kPipeBytes > kRedBytes ? kPipeBytes : kRedBytes);  // float ascales[NT], asums[NT]
   static constexpr int kOffBar = kOffRow + 2 * NT * 4;
-  static constexpr int kNumBars = 2 * WS + 2 * AS;
+  static constexpr int kNumBars = 2 * WS + 2 * AS + 1;  // + the split-K receive barrier
   static constexpr int kSmemBytes = kOffBar + kNumBars * 8;
   // two co-resident CTAs per SM for the narrow tiles (NT accumulator registers per thread; <= 113 KB of shared memory each), split or not:
   // one CTA's prologue / epilogue overlaps the other's weight stream.  128-token tiles keep 128 accumulators per thread and run one CTA per SM.
@@ -103,9 +106,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 // split phases of the same barrier (every thread of every CTA arrives once, then waits once): work between them overlaps the peers
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
@@ -119,9 +119,14 @@ __device__ __forceinline__ uint32_t map_to_cta(uint32_t smem_addr, uint32_t rank
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
   return r;
 }
-__device__ __forceinline__ void st_dsmem_u32(uint32_t addr, uint32_t v) {
-  asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+// bulk copy from this CTA's shared memory into a peer's (dst and bar are shared::cluster addresses of the same peer); the peer's mbarrier
+// receives the byte count
+__device__ __forceinline__ void bulk_copy_s2peer(uint32_t dst, uint32_t src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "r"(src), "r"(bytes), "r"(bar)
+               : "memory");
 }
+// word swizzle of a row of `width` (16 .. 128) INT32 partials of token `tok`
+__device__ __forceinline__ int red_swizzle(int tok, int width) { return (((tok >> 1) & 3) << 3) & (width - 1); }
 
 template <int V>
 struct IntTag { static constexpr int value = V; };
@@ -164,6 +169,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
   uint64_t* bar_wempty = bar_wfull + WS;                                   // consumers (4 warps) -> weight producer
   uint64_t* bar_xfull = bar_wempty + WS;                                   // activation TMA -> consumers
   uint64_t* bar_xempty = bar_xfull + AS;                                   // consumers (4 warps) -> activation producer
+  uint64_t* bar_red = bar_xempty + AS;                                     // split-K: the peers' bulk copies -> consumers
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -177,7 +183,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
   const int n_kb = kb_end - kb_begin;
   if (threadIdx.x == 0) {
     QS_PROF(0);
-    if (p.prof) p.prof[blockIdx.x * 16 + 15] = smid();
+    if (p.prof) {
+      p.prof[blockIdx.x * 16 + 13] = NT;
+      p.prof[blockIdx.x * 16 + 14] = S;
+      p.prof[blockIdx.x * 16 + 15] = smid();
+    }
   }
   qs_trace(QS_K_GEMM, 0);
 
@@ -192,6 +202,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
       mbar_init(&bar_xfull[i], 1);
       mbar_init(&bar_xempty[i], 4);
     }
+    // split-K: one phase per launch, complete when the S - 1 peer slices (NT x 128 / S partials each) have landed.  The peers copy only
+    // after cluster barrier A, which this thread joins after the fence below.
+    mbar_init(bar_red, 1);
+    if (S > 1) mbar_expect_tx(bar_red, static_cast<uint32_t>((S - 1) * NT * (kBM / S) * 4));
     fence_barrier_init();
   }
   __syncthreads();
@@ -335,74 +349,72 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
     }
     wgmma_wait<0>();
     if (threadIdx.x == 0) QS_PROF(6);
-    // split-K: the partials go into the peers' pipeline buffers, so every CTA of the cluster must have drained its rings first
+    // Cluster barrier A (split-K): the partials of the peers land in this CTA's pipeline buffers, so every CTA of the cluster must have
+    // drained its rings before any partial is sent.  Arrive now; the wait comes after the work below, which touches this CTA only.
     if (S > 1) cluster_arrive();
 
     // ------------------------------------------ epilogue ------------------------------------------
-    const int epi_tid = threadIdx.x;  // 0..127
-    pdl_wait();  // ascales / a_ssums / out belong to the dependency chain
+    // every warp's wgmmas and weight reads are done: this CTA's own rings are free
+    named_bar_sync(1, kConsumers);
+    const int tid = threadIdx.x;  // 0..127
+    const int cps_log2 = 8 - __ffs(S), cps = 1 << cps_log2;  // channels finished per CTA: 128 / S, S a power of two
+    // registers -> this CTA's shared memory, [owner][token][channel % cps] (S == 1: [token][channel]), 8-word groups of a token row swizzled
+    // by the token so that the four tokens and eight channels of a warp's store fall in 32 banks
+    int32_t* s_tx = s_red + (S > 1 ? C::kOffTx / 4 : 0);
+    {
+      const int r0 = lane >> 2, c0 = (lane & 3) * 2;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < NT / 2; ++i) {
+          const int ch = acc_channel<MODE>(h, warp, r0 + 8 * ((i >> 1) & 1));
+          const int tok = (i >> 2) * 8 + c0 + (i & 1);
+          s_tx[(((ch >> cps_log2) * NT + tok) << cps_log2) + ((ch & (cps - 1)) ^ red_swizzle(tok, cps))] = acc[h][i];
+        }
+    }
+    // this CTA finishes channel pairs [64 rank / S, 64 (rank + 1) / S) of the tile for all NT tokens: npairs divides 128, so a thread keeps
+    // one channel pair and walks the tokens.  Its weight scales are static; the loads are in flight across the waits below.
+    const int npairs = 64 / S;
+    const int prl = tid % npairs;  // channel pair inside this CTA's slice
+    const int n = n_tile * kBM + 2 * ((64 * rank) / S + prl);
+    const float ws0 = __half2float(__ldg(p.wscales + n)), ws1 = __half2float(__ldg(p.wscales + n + 1));
+    float wz0 = 0.f, wz1 = 0.f;
+    if constexpr (MODE == kModeW4Chn) {
+      wz0 = __half2float(__ldg(p.w_szs + n));
+      wz1 = __half2float(__ldg(p.w_szs + n + 1));
+    }
+    pdl_wait();  // ascales / a_ssums / out belong to the dependency chain; every storing thread observes it
     const int m0 = m_tile * NT;
-    for (int j = epi_tid; j < NT; j += kConsumers) {
+    for (int j = tid; j < NT; j += kConsumers) {
       const bool ok = (m0 + j) < p.M;
       s_asc[j] = ok ? __half2float(p.ascales[m0 + j]) : 0.f;
       if constexpr (MODE == kModeW4Chn) s_asum[j] = ok ? __half2float(p.a_ssums[m0 + j]) : 0.f;
     }
-    // every warp's wgmmas (S > 1: every CTA's in the cluster) have retired before the first partial lands in the aliased pipeline buffers
-    if (S > 1) cluster_wait(); else named_bar_sync(1, kConsumers);
-    if (epi_tid == 0) QS_PROF(8);
-    const int r0 = lane >> 2, c0 = (lane & 3) * 2;
-    if (S == 1) {
-      // registers -> shared memory, [token][channel] so that channel pairs are contiguous
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int i = 0; i < NT / 2; ++i) {
-          const int ch = acc_channel<MODE>(h, warp, r0 + 8 * ((i >> 1) & 1));
-          const int tok = (i >> 2) * 8 + c0 + (i & 1);
-          s_red[tok * kBM + ch] = acc[h][i];
-        }
-    } else {
-      // registers -> the receive buffer of the CTA that finishes this channel: rx[sender = rank][token][channel % (128 / S)].
-      // Posted remote stores; the cluster barrier below publishes them.
-      const int cps = kBM / S;  // channels finished per CTA
-      const uint32_t rx_base = smem_u32(s_red);
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int i = 0; i < NT / 2; ++i) {
-          const int ch = acc_channel<MODE>(h, warp, r0 + 8 * ((i >> 1) & 1));
-          const int tok = (i >> 2) * 8 + c0 + (i & 1);
-          const uint32_t owner = static_cast<uint32_t>(ch / cps);
-          st_dsmem_u32(map_to_cta(rx_base, owner) + static_cast<uint32_t>(((rank * NT + tok) * cps + ch % cps) * 4), static_cast<uint32_t>(acc[h][i]));
-        }
+    if (S > 1) {
+      fence_proxy_async();  // the staged partials are read by bulk copies
+      cluster_wait();       // barrier A: every ring of the cluster has drained
     }
-    if (epi_tid == 0) QS_PROF(9);
-  }
-  // the producer warps take part in the cluster barrier that releases the pushes above
-  if (S > 1 && threadIdx.x >= kConsumers) { cluster_arrive(); cluster_wait(); }
-
-  // ---------------- cross-CTA (cluster) reduction of the INT32 partial tiles through distributed shared memory ----------------
-  if (S > 1) cluster_sync_all(); else __syncthreads();
-  if (threadIdx.x < kConsumers) {
-    // the consumer warpgroup: this CTA finishes channel pairs [64 rank / S, 64 (rank + 1) / S) of the tile for all NT tokens
-    pdl_wait();  // already resolved; makes every storing thread an observer of the dependency
-    const int tid = threadIdx.x;
+    if (tid == 0) QS_PROF(8);
+    named_bar_sync(1, kConsumers);  // staged partials and row scales are visible to the warpgroup
+    if (S > 1) {
+      // one bulk copy per peer: its slice of the staging buffer -> slot `rank` of its receive buffer, completing on ITS mbarrier
+      if (tid < S && tid != rank) {
+        const uint32_t slice = static_cast<uint32_t>(NT * cps * 4);
+        bulk_copy_s2peer(map_to_cta(smem_u32(s_red) + rank * slice, tid), smem_u32(s_tx) + tid * slice, slice, map_to_cta(smem_u32(bar_red), tid));
+      }
+      if (tid == 0) QS_PROF(9);
+      mbar_wait_nocall(bar_red, 0);  // the S - 1 peer slices have landed
+      // Cluster barrier B: a CTA may exit only when the peers' copies have read its staging buffer.  Every CTA arrives after it has
+      // received all its slices, so once all have arrived every copy of the cluster is complete.  The wait is at the end of the kernel.
+      cluster_arrive();
+    } else if (tid == 0) {
+      QS_PROF(9);
+    }
     if (tid == 0) QS_PROF(10);
-    const int npairs = 64 / S;
-    const int pr = (64 * rank) / S + tid % npairs;
-    const float ws0 = __half2float(__ldg(p.wscales + n_tile * kBM + 2 * pr)), ws1 = __half2float(__ldg(p.wscales + n_tile * kBM + 2 * pr + 1));
-    float wz0 = 0.f, wz1 = 0.f;
-    if constexpr (MODE == kModeW4Chn) {
-      wz0 = __half2float(__ldg(p.w_szs + n_tile * kBM + 2 * pr));
-      wz1 = __half2float(__ldg(p.w_szs + n_tile * kBM + 2 * pr + 1));
-    }
-    const int m0 = m_tile * NT;
-    // npairs divides 128, so a thread keeps one channel pair and walks the tokens
-    const int tstep = kConsumers / npairs;    // 2 * S tokens are finished per pass of the warpgroup
-    const int n = n_tile * kBM + 2 * pr;
+
+    const int tstep = kConsumers / npairs;  // 2 * S tokens are finished per pass of the warpgroup
     const int tok_end = min(NT, p.M - m0);  // tokens of this tile that exist
     const int tok0 = tid / npairs;
-    const uint32_t off0 = static_cast<uint32_t>((tok0 * kBM + 2 * pr) * 4), off_step = static_cast<uint32_t>(tstep * kBM * 4);
     __half* optr = p.out + static_cast<size_t>(m0 + tok0) * p.N + n;
     const size_t ostep = static_cast<size_t>(tstep) * p.N;
     auto finish = [&](int tok, int2 acc, __half* dst) {
@@ -412,57 +424,56 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_act, const __grid_constant_
       *reinterpret_cast<__half2*>(dst) = __floats2half2_rn(o0, o1);  // one packed conversion, each half rounded to nearest even
       if constexpr (ACC) *reinterpret_cast<int2*>(p.acc_out + (dst - p.out)) = acc;
     };
-    if (S == 1) {
-      constexpr int kPerThread = NT / 2;  // tstep = 2
+    // S is a launch constant of the cluster: specialise so that the S partials of several tokens are loaded together, then summed
+    auto reduce_rows = [&](auto s_tag) {
+      constexpr int SS = decltype(s_tag)::value;
+      constexpr int CPS = kBM / SS;
+      constexpr int TPT = NT / (2 * SS) > 0 ? NT / (2 * SS) : 1;
+      constexpr int kChunk = TPT * SS > 16 ? 16 / SS : TPT;  // at most 16 int2 loads in flight per thread
 #pragma unroll 1
-      for (int i0 = 0; i0 < kPerThread; i0 += 16) {
-        int2 v[16];
+      for (int i0 = 0; i0 < TPT; i0 += kChunk) {
+        int2 v[kChunk][SS];
 #pragma unroll
-        for (int e = 0; e < 16; ++e)
-          if (kPerThread > e) v[e] = *reinterpret_cast<const int2*>(reinterpret_cast<const uint8_t*>(s_red) + off0 + (i0 + e) * off_step);
+        for (int i = 0; i < kChunk; ++i) {
+          const int tok = tok0 + (i0 + i) * tstep;
 #pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int tok = tok0 + (i0 + e) * tstep;
-          if (kPerThread > e && tok < tok_end) finish(tok, v[e], optr + (i0 + e) * ostep);
-        }
-      }
-    } else {
-      // S > 1: the partials of all S senders sit in this CTA's receive buffer; sum them locally
-      const int cps = kBM / S;
-      const int32_t* rx = s_red;
-      const int prl = tid % npairs;  // channel pair inside this CTA's slice
-      // S is a launch constant of the cluster: specialise so that all S x tokens shared-memory loads of a thread are in flight together
-      auto reduce_rows = [&](auto s_tag) {
-        constexpr int SS = decltype(s_tag)::value;
-        constexpr int TPT = NT / (2 * SS) > 0 ? NT / (2 * SS) : 1;
-        int2 v[TPT][SS];
-#pragma unroll
-        for (int i = 0; i < TPT; ++i) {
-          const int tok = tok0 + i * tstep;
-#pragma unroll
-          for (int r = 0; r < SS; ++r)
-            v[i][r] = (tok < NT) ? *reinterpret_cast<const int2*>(rx + (r * NT + tok) * cps + 2 * prl) : make_int2(0, 0);
+          for (int r = 0; r < SS; ++r) {
+            // sender r's partials: in the receive buffer, but this CTA's own never left its staging buffer
+            const int32_t* src = (SS > 1 && r != rank) ? s_red + r * NT * CPS : s_tx + rank * NT * CPS;
+            v[i][r] = (tok < NT) ? *reinterpret_cast<const int2*>(src + tok * CPS + ((2 * prl) ^ red_swizzle(tok, CPS))) : make_int2(0, 0);
+          }
         }
 #pragma unroll
-        for (int i = 0; i < TPT; ++i) {
-          const int tok = tok0 + i * tstep;
+        for (int i = 0; i < kChunk; ++i) {
+          const int tok = tok0 + (i0 + i) * tstep;
           int2 acc = v[i][0];
 #pragma unroll
           for (int r = 1; r < SS; ++r) { acc.x += v[i][r].x; acc.y += v[i][r].y; }
-          if (tok < tok_end) finish(tok, acc, optr + i * ostep);
+          if (tok < tok_end) finish(tok, acc, optr + (i0 + i) * ostep);
         }
-      };
-      if (S == 2) reduce_rows(IntTag<2>{});
-      else if (S == 4) reduce_rows(IntTag<4>{});
-      else reduce_rows(IntTag<8>{});
-    }
+      }
+    };
+    if (S == 1) reduce_rows(IntTag<1>{});
+    else if (S == 2) reduce_rows(IntTag<2>{});
+    else if (S == 4) reduce_rows(IntTag<4>{});
+    else reduce_rows(IntTag<8>{});
     if (tid == 0) QS_PROF(11);
-  } else {
-    pdl_wait();
+    if (S > 1) cluster_wait();  // barrier B
+    if (tid == 0) QS_PROF(12);
+    qs_trace(QS_K_GEMM, 2);
+    return;
   }
-  // S > 1: every remote store into this CTA's receive buffer was ordered before the cluster barrier above; none follows
-  if (threadIdx.x == 0) QS_PROF(12);
-  qs_trace(QS_K_GEMM, 2);
+  // the producer warps take part in both cluster barriers (every thread of the cluster arrives at each) and otherwise stay out of the tail
+  if (S > 1) {
+    cluster_arrive();
+    cluster_wait();
+    cluster_arrive();
+    cluster_wait();
+  }
+  // griddepcontrol.wait holds the whole warp: lanes 1..31 get here at once, and the weight producer's lane 0 must go on streaming weights
+  // while the previous kernel runs, so the warp reconverges first
+  __syncwarp();
+  pdl_wait();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -560,27 +571,20 @@ int resident_clusters(const void* kern, int smem, int s) {
   return n;
 }
 
-// Split-K plan.  Automatic: the largest S in {1, 2, 4, 8} that leaves every CTA >= 2 pipeline stages and keeps all `tiles` clusters
-// resident at once (resident(s) = the occupancy API's answer), so the launch is one wave by construction.  `forced` (tests, tuning)
-// is taken as given, halved only until every CTA has a stage.
-// Measured on an H100 80GB HBM3 (700 W, 1980 MHz max SM clock), Llama-3-8B W4A8 at M = 64, us per launch over all 32 layers in a
-// CUDA graph (tools/gemm_split_sweep.py), S = 1 / 2 / 4 / 8:  qkv 14.75 / 13.08 / 13.37 / 23.57,  o 13.31 / 11.31 / 11.45 / 20.40,
-// gate_up 26.95 / 35.73 / 50.27 / 90.83,  down 33.95 / 24.13 / 19.94 / 28.94.  The plan picks 4, 4, 1, 4: 32 clusters of 8 do not fit
-// (30 resident), so S = 8 is a second wave; where S = 2 and S = 4 are both one wave they are within 2 %.
-template <typename Resident>
-int choose_split(int tiles, int kb_per_tile, int forced, Resident resident) {
-  int s = 1;
-  if (forced > 0) {
-    s = forced;
-  } else {
-    while (s < 8 && kb_per_tile >= 4 * s && tiles <= resident(2 * s)) s *= 2;
-  }
-  while (s > 1 && kb_per_tile < s) s /= 2;
-  return s;
+// resident clusters of `s` CTAs of one instantiation on the current device, queried once per (instantiation, accumulator dump, device, s)
+template <int MODE, int NT, int WS, int AS>
+int resident_gemm(const GemmArgs& a, int s) {
+  using C = Cfg<MODE, NT, WS, AS>;
+  auto kern = a.acc_out ? gemm_kernel<MODE, NT, WS, AS, true> : gemm_kernel<MODE, NT, WS, AS, false>;
+  static int cache[2][kMaxDevices][4] = {};  // 0 = not yet asked
+  int& r = cache[a.acc_out ? 1 : 0][device_ordinal()][s == 1 ? 0 : s == 2 ? 1 : s == 4 ? 2 : 3];
+  if (r == 0 && raise_smem_limit(kern, C::kSmemBytes, "cudaFuncSetAttribute(gemm smem)") == QS_OK)
+    r = resident_clusters(reinterpret_cast<const void*>(kern), C::kSmemBytes, s);
+  return r;
 }
 
 template <int MODE, int NT, int WS, int AS>
-int launch_gemm(const GemmArgs& a) {
+int launch_gemm(const GemmArgs& a, int split) {
   using C = Cfg<MODE, NT, WS, AS>;
   GemmParams p{};
   p.s2_scales = static_cast<const uint8_t*>(a.s2_scales);
@@ -607,20 +611,40 @@ int launch_gemm(const GemmArgs& a) {
   auto kern = a.acc_out ? gemm_kernel<MODE, NT, WS, AS, true> : gemm_kernel<MODE, NT, WS, AS, false>;
   rc = raise_smem_limit(kern, C::kSmemBytes, "cudaFuncSetAttribute(gemm smem)");
   if (rc) return rc;
-  const int dev = device_ordinal();
-  // resident clusters per (instantiation, device, split 1/2/4/8), queried once (0 = not yet asked)
-  static int resident_cache[2][kMaxDevices][4] = {};
-  auto resident = [&](int s) {
-    int& r = resident_cache[a.acc_out ? 1 : 0][dev][s == 1 ? 0 : s == 2 ? 1 : s == 4 ? 2 : 3];
-    if (r == 0) r = resident_clusters(reinterpret_cast<const void*>(kern), C::kSmemBytes, s);
-    return r;
-  };
-  p.split = choose_split(tiles, p.kb_per_tile, a.force_split, resident);
+  p.split = split;
   if (p.prof)  // profiled launches (tools/gemm_timeline.py) report their plan
     fprintf(stderr, "qs_gemm_plan mode=%d nt=%d ws=%d as=%d M=%d N=%d K=%d tiles=%d split=%d ctas=%d smem=%d resident_clusters=%d\n", MODE, NT, WS,
-            AS, a.M, a.N, a.K, tiles, p.split, tiles * p.split, C::kSmemBytes, resident(p.split));
+            AS, a.M, a.N, a.K, tiles, p.split, tiles * p.split, C::kSmemBytes, resident_gemm<MODE, NT, WS, AS>(a, p.split));
   return launch(kern, dim3(tiles * p.split), dim3(kNumThreads), C::kSmemBytes, p.split, a.stream, "gemm launch", tm_act, tm_w, p);
 }
+
+// one (MODE, NT) instantiation with its ring depths, as the planner sees it
+struct TileImpl {
+  int nt;
+  int (*resident)(const GemmArgs&, int);
+  int (*launch)(const GemmArgs&, int);
+};
+
+// The plan of a launch: tokens per tile NT in {32, 64, 128} x cluster split S in {1, 2, 4, 8}.  Candidates: every NT up to the smallest
+// one that covers M in one tile (a larger one would be mostly empty), every S that leaves each CTA >= 2 pipeline stages, and only plans
+// whose clusters are all resident at once by the occupancy API's answer for that exact instantiation -- one wave by construction.
+// `force_nt` / `force_split` (tests, tuning) restrict the candidates to the given value, a forced S without the stage rule (it is
+// halved only until every CTA has a stage).  Without a one-wave candidate (prompt-sized M) the launch is the covering tile, unsplit.
+// Rule, in this order: fewest stages per CTA, then fewest token tiles (larger NT), then smaller S.
+// Measured on an H100 80GB HBM3 (700 W, 1980 MHz max SM clock), us per launch over 32 weight sets in a CUDA graph
+// (tools/gemm_split_sweep.py), as NT/S: us.  Llama-3-8B W4A8 per-channel, M = 64:
+//   qkv      32/2: 11.17  64/2: 12.12  64/4: 11.19  64/8: 17.05    o     32/2: 10.14  64/2: 10.19  64/4:  9.66  64/8: 15.42
+//   gate_up  32/1: 33.97  64/1: 27.78  64/2: 33.18  128/1: 45.49   down  32/2: 22.40  32/4: 25.73  64/2: 23.51  64/4: 18.51  64/8: 24.41
+// g128, M = 64:  qkv 32/2: 15.12  64/4: 11.71;  o 32/2: 13.88  64/4: 11.58;  gate_up 64/1: 29.59;  down 32/4: 32.91  64/4: 25.17.
+// W8A8, M = 128:  qkv 32/1: 23.70  64/2: 17.10  128/2: 16.94;  o 32/2: 15.17  64/2: 14.77  128/2: 15.00;
+//   gate_up 64/1: 60.20 (two waves)  128/1: 61.32;  down 32/2: 41.89  64/2: 40.93  128/2: 39.78.
+// Qwen1.5-72B TP = 4 shards, per-channel, M = 64:  qkv (6144 x 8192) 32/2: 15.89  64/4: 15.08;  o (8192 x 2048) 32/2: 9.72  64/2: 9.65;
+//   gate_up (12288 x 8192) 32/1: 26.78  64/2: 23.73;  down (8192 x 6144) 32/2: 15.74  64/2: 15.47.
+// The rule picks the fastest plan of each of these shapes or one within 2 % of it.  Two token tiles unpack every weight twice, so a
+// smaller NT pays only where it buys a deeper split; 32 clusters of 8 do not fit (30 resident), so S = 8 is a second wave.  With the
+// scalar remote-store tail this kernel had before, 32/2 measured 1.5 (qkv) and 0.9 us (o) faster than 64/4; the bulk-copy tail removed
+// that difference.
+inline long plan_cost(int nt, int s, int stages) { return stages * 1000L + (128 - nt) + s; }
 
 template <int MODE>
 int dispatch_gemm(const GemmArgs& a) {
@@ -629,14 +653,36 @@ int dispatch_gemm(const GemmArgs& a) {
   QS_REQUIRE(a.K % kBK == 0, "gemm: K=%d must be a multiple of %d", a.K, kBK);
   QS_REQUIRE((reinterpret_cast<uintptr_t>(a.act) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.weight) & 15) == 0, "gemm: operands must be 16-byte aligned");
   QS_REQUIRE(a.force_split == 0 || a.force_split == 1 || a.force_split == 2 || a.force_split == 4 || a.force_split == 8, "gemm: split must be 1, 2, 4 or 8");
-  // ring depths (256-K stages): NT <= 64 fits two CTAs per SM (<= 113 KB of shared memory each); 128-token tiles run one CTA per SM and
-  // take deeper weight rings.  The split-K receive buffer aliases the drained rings, so it costs no shared memory.
-  constexpr bool w8 = (MODE == kModeW8), grp = (MODE == kModeW4Grp);
   QS_REQUIRE(a.force_nt == 0 || a.force_nt == 32 || a.force_nt == 64 || a.force_nt == 128, "gemm: tile tokens must be 32, 64 or 128");
-  const int nt = a.force_nt > 0 ? a.force_nt : a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;
-  if (nt == 32) return launch_gemm<MODE, 32, (w8 ? 2 : grp ? 4 : 5), 4>(a);
-  if (nt == 64) return launch_gemm<MODE, 64, (w8 ? 2 : grp ? 3 : 4), (w8 ? 2 : 3)>(a);
-  return launch_gemm<MODE, 128, 4, 2>(a);
+  // ring depths (256-K stages): NT <= 64 fits two CTAs per SM (<= 113 KB of shared memory each); 128-token tiles run one CTA per SM and
+  // take deeper weight rings.  The split-K receive and staging buffers alias the drained rings, so they cost no shared memory.
+  constexpr bool w8 = (MODE == kModeW8), grp = (MODE == kModeW4Grp);
+  constexpr int kWs32 = w8 ? 2 : grp ? 4 : 5, kWs64 = w8 ? 2 : grp ? 3 : 4, kAs64 = w8 ? 2 : 3;
+  static const TileImpl impls[3] = {{32, resident_gemm<MODE, 32, kWs32, 4>, launch_gemm<MODE, 32, kWs32, 4>},
+                                    {64, resident_gemm<MODE, 64, kWs64, kAs64>, launch_gemm<MODE, 64, kWs64, kAs64>},
+                                    {128, resident_gemm<MODE, 128, 4, 2>, launch_gemm<MODE, 128, 4, 2>}};
+  const int kb = (a.K + kSub * kBK - 1) / (kSub * kBK);
+  const int nt_cover = a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;  // the smallest tile that covers M, or the largest there is
+  int forced_s = a.force_split;
+  while (forced_s > 1 && kb < forced_s) forced_s /= 2;
+  const TileImpl* best = nullptr;
+  int best_s = 0;
+  long best_cost = 0;
+  for (const TileImpl& t : impls) {
+    if (a.force_nt > 0 ? t.nt != a.force_nt : t.nt > nt_cover) continue;
+    const int tiles = (a.N / kBM) * ((a.M + t.nt - 1) / t.nt);
+    for (int s = 1; s <= 8; s *= 2) {
+      if (forced_s > 0 ? s != forced_s : (s > 1 && kb < 2 * s)) continue;
+      if (tiles > t.resident(a, s)) continue;
+      const long cost = plan_cost(t.nt, s, (kb + s - 1) / s);
+      if (best == nullptr || cost < best_cost) best = &t, best_s = s, best_cost = cost;
+    }
+  }
+  if (best == nullptr) {  // no one-wave plan (prompt-sized M, or a forced value that does not fit): the widest tile, unsplit unless forced
+    best = &impls[(a.force_nt > 0 ? a.force_nt : nt_cover) == 32 ? 0 : (a.force_nt > 0 ? a.force_nt : nt_cover) == 64 ? 1 : 2];
+    best_s = forced_s > 0 ? forced_s : 1;
+  }
+  return best->launch(a, best_s);
 }
 
 }  // namespace

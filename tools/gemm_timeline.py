@@ -2,9 +2,10 @@
 """Per-CTA phase timeline of the decode GEMM (Llama-3-8B, M = 64) from the kernel's %globaltimer stamps (qs_gemm_set_profile_buffer).
 
 For each of the four decode shapes: the number of waves (CTAs that enter only after the first CTA has exited ran in a later wave), CTAs
-per SM, and the median per-CTA phase times: entry -> first stage on chip, PDL wait, mainloop (and per 256-K stage), epilogue up to the
-partial push, the cluster barrier, the finish.  A profiled launch prints its plan, with the occupancy API's answer for it, on stderr
-(qs_gemm_plan ... resident_clusters=N).
+per SM, the planned tokens per tile and split, and the median per-CTA phase times: entry -> first stage on chip, PDL wait, mainloop (and
+per 256-K stage), epilogue up to the issue of the split-K bulk copies (staging the partials, row loads and the ring-drain cluster barrier
+included), the wait for the peers' partials, the finish.  A profiled launch prints its plan, with the occupancy API's answer for it, on
+stderr (qs_gemm_plan ... resident_clusters=N).
 
   python tools/gemm_timeline.py [--reps 5] [--out DIR]
 """
@@ -20,7 +21,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from qserve_b200._lib import lib  # noqa: E402
 from qserve_b200.decode import DecodeRunner  # noqa: E402
 
-# stamp slots written by gemm_kernel (slot 15: SM id)
+# stamp slots written by gemm_kernel (slots 13 / 14 / 15: tokens per tile, split, SM id)
 ENTRY, PDL, FIRST_STAGE, MAIN_DONE, ROWS, PUSHED, CLUSTER, FINISHED, EXIT = 0, 2, 4, 6, 8, 9, 10, 11, 12
 
 ap = argparse.ArgumentParser()
@@ -37,7 +38,6 @@ prof = torch.zeros(8192 * 16, dtype=torch.int64, device="cuda")
 summary = {}
 for name, (xq, buf) in ops.items():
     lin = run.layers[0][name]
-    tiles = (lin.N // 128) * 1  # M = 64: one 64-token tile
     stages = -(-lin.K // 256)
     reps = []
     for r in range(args.reps):
@@ -53,12 +53,11 @@ for name, (xq, buf) in ops.items():
         p = p[p[:, ENTRY] > 0]
         sm = p[:, 15].copy()
         t = (p[:, :15] - p[:, ENTRY].min()).astype(np.float64) / 1e3  # us from the first CTA's entry
-        ctas = len(p)
-        split = max(1, ctas // tiles)
+        ctas, nt, split = len(p), int(p[0, 13]), int(p[0, 14])
         late = int((t[:, ENTRY] > t[:, EXIT].min()).sum())
         med = lambda a, b: float(np.median(t[:, b] - t[:, a]))  # noqa: E731
         reps.append({
-            "ctas": ctas, "split": split, "stages_per_cta": stages / split, "ctas_after_first_exit": late, "waves": 1 if late == 0 else 2,
+            "ctas": ctas, "tile_tokens": nt, "split": split, "stages_per_cta": stages / split, "ctas_after_first_exit": late, "waves": 1 if late == 0 else 2,
             "max_ctas_per_sm": int(np.bincount(sm.astype(np.int64)).max()) if sm.any() else None,
             "span_us": float(t[:, EXIT].max()), "entry_spread_us": float(t[:, ENTRY].max()),
             "entry_to_first_stage_us": med(ENTRY, FIRST_STAGE), "pdl_wait_us": med(ENTRY, PDL),
