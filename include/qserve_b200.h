@@ -320,6 +320,29 @@ QS_API int qs_tree_accept_sampling(const int64_t* draft_tokens, const int32_t* t
                                    const float* temperature, const int32_t* top_k, const float* top_p, uint64_t seed, int64_t* offsets,
                                    int32_t* accept_len, int32_t* path, int64_t* bonus, int batch, int num_nodes, int vocab, void* stream);
 
+/* Penalties and log-probabilities (SamplingParams.repetition_penalty / presence_penalty / frequency_penalty, logprobs / prompt_logprobs).
+ * Both read everything after the PDL dependency wait, need no host synchronisation and are CUDA-graph capturable; vocab % 8 == 0,
+ * vocab <= 196608.  Parameter arrays are trusted (not read on the host).
+ *
+ * qs_apply_penalties: fp16 logits [rows, vocab] modified in place before sampling (vLLM's semantics).  history int64 [rows, history_len]:
+ *   the prompt at [0, prompt_lens[r]), the generated tokens at [prompt_lens[r], seq_lens[r]); prompt_lens / seq_lens int32 [rows] are clamped
+ *   to 0 <= prompt_lens <= seq_lens <= history_len before any read; ids outside [0, vocab) (-1: padding) are ignored.  repetition fp32 (in
+ *   (0, 2]), presence and frequency fp32 (in [-2, 2]), [rows].  For every token t that occurs in the row's history, with c = its count among
+ *   the generated tokens, x = float(logit[t]) in IEEE fp32 without FMA contraction: (1) if repetition != 1, x = x > 0 ? x / repetition :
+ *   x * repetition; (2) if c > 0, x = (x - (frequency * c)) - presence; then one rounding to fp16.  Each distinct token is written once (no
+ *   atomics: bitwise deterministic) and only when its bits change; NaN logits and rows with (1, 0, 0) are not written, and no logit outside
+ *   the history is touched.  history_len <= 32768.
+ * qs_logprobs_rows: for fp16 logits [rows, vocab] and tokens int64 [rows] (the sampled token, or the next prompt token): logprob fp32 [rows]
+ *   = the token's log-probability and, for 0 <= n <= 20, top_ids int64 [rows, n] / top_logprobs fp32 [rows, n] = the n largest logits by
+ *   (logit descending, index ascending; -0 ties with +0).  The distribution is the sampler's softmax at T = 1: NaN and -inf weigh 0,
+ *   w = exp(x - max) with w = 1 where x == max (+inf logits share the mass), the weight sum in 64-bit fixed point.  A row without weight
+ *   gives NaN log-probabilities and top_ids -1; an out-of-range token gives NaN; with fewer than n non-NaN logits the remaining slots get -1
+ *   and -inf.  top_ids / top_logprobs may be NULL when n = 0.                                                                          */
+QS_API int qs_apply_penalties(void* logits, const int64_t* history, const int32_t* prompt_lens, const int32_t* seq_lens, const float* repetition,
+                              const float* presence, const float* frequency, int rows, int vocab, int history_len, void* stream);
+QS_API int qs_logprobs_rows(float* logprob, int64_t* top_ids, float* top_logprobs, const void* logits, const int64_t* tokens, int rows, int vocab,
+                            int n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

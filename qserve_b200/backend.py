@@ -655,16 +655,21 @@ def kv_cache_compact(kv_pointers, start_pos, path, accept_len, num_kv_heads: int
           kv_pointers.size(-1), int(num_kv_heads), int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)))
 
 
+def _row_vec(v, n: int, dev, dt, name: str, ok, what: str) -> torch.Tensor:
+    """A per-row parameter as a device tensor: a scalar broadcasts (and is checked on the host); a tensor is used as given (its values are
+    trusted: checking them would synchronise with the device)."""
+    if isinstance(v, torch.Tensor):
+        _cuda(v, name)
+        _require(v.dtype == dt and v.is_contiguous() and tuple(v.shape) == (n,) and v.device == dev, f"{name} must be contiguous {dt} [{n}]")
+        return v
+    _require(ok(v), f"{name}={v}: {what}")
+    return torch.full((n,), v, dtype=dt, device=dev)
+
+
 def _row_params(n: int, dev, temperature, top_k, top_p, offsets):
-    """Per-row sampling parameters as device tensors: scalars broadcast (and are checked on the host); tensors are used as given (their
-    values are trusted: checking them would synchronise with the device)."""
+    """Per-row sampling parameters as device tensors (see _row_vec)."""
     def vec(v, dt, name, ok, what):
-        if isinstance(v, torch.Tensor):
-            _cuda(v, name)
-            _require(v.dtype == dt and v.is_contiguous() and tuple(v.shape) == (n,) and v.device == dev, f"{name} must be contiguous {dt} [{n}]")
-            return v
-        _require(ok(v), f"{name}={v}: {what}")
-        return torch.full((n,), v, dtype=dt, device=dev)
+        return _row_vec(v, n, dev, dt, name, ok, what)
     T = vec(temperature, torch.float32, "temperature", lambda v: float(v) >= 0, "must be >= 0")
     K = vec(top_k, torch.int32, "top_k", lambda v: int(v) == -1 or int(v) >= 1, "must be -1 (off) or >= 1")
     P = vec(top_p, torch.float32, "top_p", lambda v: 0 < float(v) <= 1, "must lie in (0, 1]")
@@ -743,6 +748,73 @@ def tree_accept_sampling(draft_tokens, tree_mask, logits, temperature, top_k, to
               draft_probs.data_ptr() if draft_probs is not None else None, T.data_ptr(), K.data_ptr(), P.data_ptr(), _seed(seed), offsets.data_ptr(),
               accept_len.data_ptr(), path.data_ptr(), bonus.data_ptr(), B, n, V)
     return accept_len, path, bonus
+
+
+MAX_PENALTY_HISTORY = 32768  # history tokens per row apply_penalties supports
+MAX_TOP_LOGPROBS = 20
+
+
+def _logit_rows(logits) -> tuple:
+    _cuda(logits, "logits")
+    _require(logits.dtype == _HALF and logits.dim() == 2 and logits.is_contiguous(), "logits must be contiguous float16 [rows, vocab]")
+    rows, V = logits.shape
+    _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
+    return rows, V
+
+
+def apply_penalties(logits, history, prompt_lens, seq_lens, repetition, presence, frequency) -> torch.Tensor:
+    """Repetition / presence / frequency penalties (SamplingParams.repetition_penalty / presence_penalty / frequency_penalty, vLLM's
+    semantics) applied in place to fp16 logits [rows, V] before sample_rows / argmax_rows; returns logits.  history int64 [rows, H] holds
+    the prompt at [0, prompt_lens[r]) and the generated tokens at [prompt_lens[r], seq_lens[r]) (prompt_lens / seq_lens int32 [rows], clamped
+    to 0 <= prompt_lens <= seq_lens <= H on the device; -1 and other out-of-range ids are ignored), H <= 32768.  repetition (in (0, 2]),
+    presence and frequency (in [-2, 2]) are fp32 per-row tensors (trusted) or scalars (checked).  For each token t of the history, with c its
+    count among the generated tokens, in fp32: x = x / rep if x > 0 else x * rep (rep != 1); if c > 0: x = (x - frequency * c) - presence;
+    one rounding to fp16.  Only history tokens whose value changes are written: neutral rows (1, 0, 0) and NaN logits stay as they are, and
+    the call is bitwise deterministic.  See include/qserve_b200.h."""
+    rows, V = _logit_rows(logits)
+    dev = logits.device
+    _cuda(history, "history")
+    _require(history.dtype == torch.int64 and history.dim() == 2 and history.is_contiguous() and history.size(0) == rows and history.device == dev,
+             f"history must be contiguous int64 [{rows}, H] on the device of the logits")
+    H = history.size(1)
+    _require(H <= MAX_PENALTY_HISTORY, f"history of {H} tokens per row: at most {MAX_PENALTY_HISTORY}")
+    for t, nm in ((prompt_lens, "prompt_lens"), (seq_lens, "seq_lens")):
+        _cuda(t, nm)
+        _require(t.dtype == torch.int32 and t.is_contiguous() and tuple(t.shape) == (rows,) and t.device == dev, f"{nm} must be contiguous int32 [{rows}]")
+    R = _row_vec(repetition, rows, dev, torch.float32, "repetition", lambda v: 0 < float(v) <= 2, "must lie in (0, 2]")
+    P = _row_vec(presence, rows, dev, torch.float32, "presence", lambda v: -2 <= float(v) <= 2, "must lie in [-2, 2]")
+    F = _row_vec(frequency, rows, dev, torch.float32, "frequency", lambda v: -2 <= float(v) <= 2, "must lie in [-2, 2]")
+    if rows and H:
+        _call(logits, lib.qs_apply_penalties, logits.data_ptr(), history.data_ptr(), prompt_lens.data_ptr(), seq_lens.data_ptr(), R.data_ptr(),
+              P.data_ptr(), F.data_ptr(), rows, V, H)
+    return logits
+
+
+def logprobs_rows(logits, tokens, n: int, logprob: Optional[torch.Tensor] = None, top_ids: Optional[torch.Tensor] = None,
+                  top_logprobs: Optional[torch.Tensor] = None):
+    """Log-probabilities for SamplingParams.logprobs / prompt_logprobs in one launch: for fp16 logits [rows, V] and tokens int64 [rows] (the
+    sampled token, or the next prompt token), returns (logprob fp32 [rows], top_ids int64 [rows, n], top_logprobs fp32 [rows, n]) with
+    0 <= n <= 20, the top tokens ordered by logit descending, ties by ascending index.  The distribution is the row's softmax at T = 1 with the
+    sampler's conventions (NaN and -inf weigh 0, +inf logits share the mass); pass the penalised logits to get the distribution before the
+    temperature / top-k / top-p warpers.  A row without weight gives NaN and top_ids -1; an out-of-range token gives NaN; with fewer than n
+    non-NaN logits the remaining slots are -1 / -inf.  The optional out tensors are written in place (CUDA-graph capture).  Deterministic."""
+    rows, V = _logit_rows(logits)
+    dev = logits.device
+    n = int(n)
+    _require(0 <= n <= MAX_TOP_LOGPROBS, f"n={n}: 0 .. {MAX_TOP_LOGPROBS} top log-probabilities")
+    _cuda(tokens, "tokens")
+    _require(tokens.dtype == torch.int64 and tokens.is_contiguous() and tuple(tokens.shape) == (rows,) and tokens.device == dev,
+             f"tokens must be contiguous int64 [{rows}]")
+    logprob = torch.empty(rows, dtype=torch.float32, device=dev) if logprob is None else logprob
+    top_ids = torch.empty((rows, n), dtype=torch.int64, device=dev) if top_ids is None else top_ids
+    top_logprobs = torch.empty((rows, n), dtype=torch.float32, device=dev) if top_logprobs is None else top_logprobs
+    for t, nm, dt, shape in ((logprob, "logprob", torch.float32, (rows,)), (top_ids, "top_ids", torch.int64, (rows, n)),
+                             (top_logprobs, "top_logprobs", torch.float32, (rows, n))):
+        _require(t.device == dev and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, f"{nm} must be contiguous {dt} {shape}")
+    if rows:
+        _call(logits, lib.qs_logprobs_rows, logprob.data_ptr(), top_ids.data_ptr() if n else None, top_logprobs.data_ptr() if n else None,
+              logits.data_ptr(), tokens.data_ptr(), rows, V, n)
+    return logprob, top_ids, top_logprobs
 
 
 class PeerContext:

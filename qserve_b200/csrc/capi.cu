@@ -303,6 +303,24 @@ int qs_tree_accept_sampling(const int64_t* draft_tokens, const int32_t* tree_mas
   return tree_accept_sampling(a);
 }
 
+int qs_apply_penalties(void* logits, const int64_t* history, const int32_t* prompt_lens, const int32_t* seq_lens, const float* repetition,
+                       const float* presence, const float* frequency, int rows, int vocab, int history_len, void* stream) {
+  PenaltyArgs a;
+  a.logits = logits; a.history = reinterpret_cast<const long long*>(history); a.prompt_lens = prompt_lens; a.seq_lens = seq_lens;
+  a.repetition = repetition; a.presence = presence; a.frequency = frequency; a.rows = rows; a.vocab = vocab; a.history_len = history_len;
+  a.stream = stream;
+  return apply_penalties(a);
+}
+
+int qs_logprobs_rows(float* logprob, int64_t* top_ids, float* top_logprobs, const void* logits, const int64_t* tokens, int rows, int vocab, int n,
+                     void* stream) {
+  QS_REQUIRE(logits == nullptr || aligned16(logits), "logprobs_rows: logits must be 16-byte aligned");
+  LogprobArgs a;
+  a.logprob = logprob; a.top_ids = reinterpret_cast<long long*>(top_ids); a.top_logprobs = top_logprobs; a.logits = logits;
+  a.tokens = reinterpret_cast<const long long*>(tokens); a.rows = rows; a.vocab = vocab; a.n = n; a.stream = stream;
+  return logprobs_rows(a);
+}
+
 int qs_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
                          int64_t out_stride, const int32_t* cu_seqlens, int batch, int num_tokens, int max_seqlen, int num_heads, int num_kv_heads,
                          int head_dim, float softmax_scale, void* stream) {

@@ -206,5 +206,29 @@ struct TreeAcceptSamplingArgs {
   void* stream = nullptr;
 };
 int tree_accept_sampling(const TreeAcceptSamplingArgs& a);
+// repetition / presence / frequency penalties applied in place to fp16 logits before sampling
+struct PenaltyArgs {
+  void* logits = nullptr;               // fp16 [rows, vocab], modified in place
+  const long long* history = nullptr;   // [rows, history_len] token ids: prompt, then generated tokens; -1 / out of range ignored
+  const int* prompt_lens = nullptr;     // [rows]
+  const int* seq_lens = nullptr;        // [rows], clamped to 0 <= prompt_lens <= seq_lens <= history_len on the device
+  const float* repetition = nullptr;    // [rows]
+  const float* presence = nullptr;
+  const float* frequency = nullptr;
+  int rows = 0, vocab = 0, history_len = 0;
+  void* stream = nullptr;
+};
+int apply_penalties(const PenaltyArgs& a);
+// log-probability of a chosen token and the n <= 20 most likely tokens of each row's softmax (T = 1)
+struct LogprobArgs {
+  float* logprob = nullptr;         // [rows]
+  long long* top_ids = nullptr;     // [rows, n]
+  float* top_logprobs = nullptr;    // [rows, n]
+  const void* logits = nullptr;     // fp16 [rows, vocab]
+  const long long* tokens = nullptr;  // [rows]
+  int rows = 0, vocab = 0, n = 0;
+  void* stream = nullptr;
+};
+int logprobs_rows(const LogprobArgs& a);
 
 }  // namespace qs

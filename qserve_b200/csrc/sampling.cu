@@ -23,8 +23,12 @@
 // zeroed).  With no child accepted the bonus token is drawn from p with draw j = 0.  Greedy rows keep p one-hot at the argmax, which makes
 // the result exactly tree_accept_greedy(draft, mask, argmax_rows(logits)).
 //
-// Both kernels read everything a preceding kernel may write (logits, drafts, mask, parameters, offsets) after griddepcontrol.wait, need no
-// host synchronisation and can be captured in a CUDA graph.
+// apply_penalties_kernel: repetition / presence / frequency penalties on the logits before the sampler, one CTA per row over its history
+// only (sorted keys, one writer per distinct token).  logprobs_rows_kernel: the log-probability of a chosen token and the top-n tokens of the
+// T = 1 softmax, on the sample_rows cluster structure (fixed-point sums, radix select of the n-th largest key).
+//
+// All kernels read everything a preceding kernel may write (logits, drafts, mask, history, parameters, offsets) after griddepcontrol.wait,
+// need no host synchronisation and can be captured in a CUDA graph.
 #include "common.cuh"
 #include "launch.cuh"
 
@@ -512,6 +516,277 @@ __global__ void __launch_bounds__(kThreads, 1) tree_accept_sampling_kernel(
   if (rank == 0 && threadIdx.x == 0) offsets[b] = off + 1;
 }
 
+// ------------------------------------------------------------------------------------------------
+// repetition / presence / frequency penalties
+// ------------------------------------------------------------------------------------------------
+constexpr int kPenThreads = 1024;
+constexpr int kMaxHistory = 32768;  // 128 KB of sort keys per row
+constexpr uint32_t kNoKey = 0xffffffffu;
+
+// first index in [lo, hi) of the ascending keys with keys[i] >= v
+__device__ __forceinline__ int lower_bound(const uint32_t* keys, int lo, int hi, uint32_t v) {
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (keys[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// One CTA per row.  The history becomes keys (token << 1) | is_output in shared memory (padding, out-of-range ids and the tail past the
+// row's length: kNoKey), sorted ascending (bitonic over the next power of two of the row's length).  The first key of each run of one token
+// applies the penalties to that token's logit: the run's output keys are its upper part, found by binary search.  Every distinct token is
+// written by exactly one thread, and only when its fp16 bits change.
+__global__ void __launch_bounds__(kPenThreads, 1) apply_penalties_kernel(__half* __restrict__ logits, const long long* __restrict__ history,
+                                                                       const int* __restrict__ prompt_lens, const int* __restrict__ seq_lens,
+                                                                       const float* __restrict__ repetition, const float* __restrict__ presence,
+                                                                       const float* __restrict__ frequency, int V, int H) {
+  extern __shared__ uint32_t keys[];
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // logits, history, lengths and parameters may come from the preceding kernels
+  const int row = blockIdx.x;
+  const float rep = repetition[row], pres = presence[row], freq = frequency[row];
+  if (rep == 1.f && pres == 0.f && freq == 0.f) return;  // neutral row: nothing is written
+  const int hl = min(max(seq_lens[row], 0), H);
+  const int pl = min(max(prompt_lens[row], 0), hl);
+  int n = 1;
+  while (n < hl) n <<= 1;
+  const long long* hrow = history + static_cast<size_t>(row) * H;
+  for (int i = threadIdx.x; i < n; i += kPenThreads) {
+    uint32_t k = kNoKey;
+    if (i < hl) {
+      const long long t = hrow[i];
+      if (t >= 0 && t < V) k = (static_cast<uint32_t>(t) << 1) | (i >= pl ? 1u : 0u);
+    }
+    keys[i] = k;
+  }
+  __syncthreads();
+  for (int k = 2; k <= n; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = threadIdx.x; i < n; i += kPenThreads) {
+        const int p = i ^ j;
+        if (p > i) {
+          const uint32_t a = keys[i], b = keys[p];
+          if ((a > b) == ((i & k) == 0)) {
+            keys[i] = b;
+            keys[p] = a;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  __half* lrow = logits + static_cast<size_t>(row) * V;
+  for (int i = threadIdx.x; i < n; i += kPenThreads) {
+    const uint32_t k = keys[i];
+    if (k == kNoKey || (i > 0 && (keys[i - 1] >> 1) == (k >> 1))) continue;
+    const uint32_t t = k >> 1;
+    const int c_out = lower_bound(keys, i, n, (t + 1) << 1) - lower_bound(keys, i, n, (t << 1) | 1u);
+    const __half old = lrow[t];
+    float x = __half2float(old);
+    if (x != x) continue;  // NaN logits are not written
+    if (rep != 1.f) x = x > 0.f ? __fdiv_rn(x, rep) : __fmul_rn(x, rep);
+    if (c_out > 0) {
+      x = __fsub_rn(x, __fmul_rn(freq, static_cast<float>(c_out)));
+      x = __fsub_rn(x, pres);
+    }
+    const __half nw = __float2half_rn(x);
+    if (__half_as_ushort(nw) != __half_as_ushort(old)) lrow[t] = nw;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// log-probabilities of a chosen token and the top-n tokens
+// ------------------------------------------------------------------------------------------------
+constexpr int kMaxTop = 20;
+
+struct TopSmem {
+  int n_above, n_eq;
+  uint32_t above_key[kMaxTop];  // this CTA's keys > tau (fewer than n in the whole cluster)
+  int above_idx[kMaxTop];
+  int eq_idx[kMaxTop];          // this CTA's first keys == tau, in index order
+  uint32_t top_key[kMaxTop];    // rank 0: the merged, ordered list
+  int top_idx[kMaxTop];
+  uint32_t wmax[kWarps];        // this CTA's per-warp maximum keys (0: no non-NaN logit)
+  uint32_t allw[kCluster * kWarps];
+  uint32_t tau0;
+};
+
+__device__ __forceinline__ bool not_nan_bits(uint32_t b) { return (b & 0x7fffu) <= 0x7c00u; }
+// the order key of the top-n list: -0 ties with +0
+__device__ __forceinline__ uint32_t top_key(uint32_t b) { return okey(b == 0x8000u ? 0u : b); }
+
+// One cluster of 8 CTAs per row (the sample_rows structure).  The softmax is the sampler's at T = 1: NaN and -inf weigh 0, w = exp(x - max)
+// with w = 1 at the maximum, S = sum w in 64-bit fixed point; a logit's log-probability is (x - max) - log S in fp64 (-log S at the
+// maximum).  Top-n: tau = the n-th largest non-NaN key by the two-level radix select over the keys above a lower bound (the n-th largest
+// per-warp maximum); the keys > tau (fewer than n) and the first keys == tau in index order are merged by rank 0.
+__global__ void __launch_bounds__(kThreads, 1) logprobs_rows_kernel(float* __restrict__ logprob, long long* __restrict__ top_ids,
+                                                                  float* __restrict__ top_logprobs, const __half* __restrict__ logits,
+                                                                  const long long* __restrict__ tokens, int n, int V) {
+  extern __shared__ uint4 dyn[];
+  __shared__ Smem s;
+  __shared__ TopSmem ts;
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // logits and tokens may come from the preceding kernels
+  const int row = blockIdx.x / kCluster, rank = blockIdx.x % kCluster;
+  int v0, v1;
+  slice_of(V, rank, v0, v1);
+  const int n_loc = (v1 - v0) * 8, g0 = v0 * 8;
+  __half* xs = reinterpret_cast<__half*>(dyn);
+  const __half* lrow = logits + static_cast<size_t>(row) * V;
+  load_slice(xs, lrow, v0, v1);
+  const uint16_t* xb = reinterpret_cast<const uint16_t*>(xs);
+  int phase = 0;
+  u64 all[kCluster];
+
+  // max key and count of the weighted logits, count of the non-NaN ones
+  u64 mk = 0, cv = 0, cn = 0;
+  for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+    const uint32_t b = xb[i];
+    if (valid_bits(b)) {
+      mk = max(mk, static_cast<u64>(okey(b)));
+      ++cv;
+    }
+    cn += not_nan_bits(b) ? 1 : 0;
+  }
+  mk = block_reduce(mk, s.red, OpMax());
+  cv = block_reduce(cv, s.red, OpAdd());
+  cn = block_reduce(cn, s.red, OpAdd());
+  gather(s, phase, (mk << 48) | (cv << 24) | cn, all);  // counts < 2^24 (V <= 196608)
+  mk = cv = cn = 0;
+#pragma unroll
+  for (int q = 0; q < kCluster; ++q) {
+    mk = max(mk, all[q] >> 48);
+    cv += (all[q] >> 24) & 0xffffffu;
+    cn += all[q] & 0xffffffu;
+  }
+  const bool none = cv == 0;  // no weight: NaN log-probabilities, no top tokens
+  float mz = 0.f;
+  double log_s = 0.0;
+  if (!none) {
+    mz = __half2float(__ushort_as_half(static_cast<unsigned short>(key_bits(static_cast<uint32_t>(mk)))));
+    u64 m = 0;
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t b = xb[i];
+      if (valid_bits(b)) m += fix(weight(b, 1.f, mz));
+    }
+    m = block_reduce(m, s.red, OpAdd());
+    gather(s, phase, m, all);
+    u64 S = 0;
+#pragma unroll
+    for (int q = 0; q < kCluster; ++q) S += all[q];
+    log_s = log(static_cast<double>(S) * 9.094947017729282e-13);  // S 2^-40 >= 1
+  }
+  const float kNan = __int_as_float(0x7fc00000);
+  auto lp_of = [&](float x) -> float {
+    if (none || x != x) return kNan;
+    if (x == mz) return static_cast<float>(-log_s);
+    return static_cast<float>(static_cast<double>(x) - static_cast<double>(mz) - log_s);
+  };
+
+  const int ne = none ? 0 : static_cast<int>(min(static_cast<u64>(n), cn));  // listed tokens; the slots past ne get -1 / -inf
+  if (ne > 0) {
+    // tau0 = the ne-th largest of the cluster's 64 per-warp maximum keys: ne warps hold a key >= tau0 each, so the ne-th largest key is
+    // >= tau0 and the histograms count only the keys >= tau0 (a handful for most rows, instead of the whole row on a few bins)
+    uint32_t wm = 0;
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t b = xb[i];
+      if (not_nan_bits(b)) wm = max(wm, top_key(b));
+    }
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) wm = max(wm, __shfl_xor_sync(0xffffffffu, wm, m));
+    if ((threadIdx.x & 31) == 0) ts.wmax[threadIdx.x >> 5] = wm;
+    cluster_sync();
+    if (threadIdx.x < kCluster * kWarps) ts.allw[threadIdx.x] = peer(ts.wmax, threadIdx.x / kWarps)[threadIdx.x % kWarps];
+    __syncthreads();
+    if (threadIdx.x < kCluster * kWarps) {
+      const int t = threadIdx.x;
+      const uint32_t v = ts.allw[t];
+      int below = 0;  // the warp maxima ordered before this one (larger, or equal with a smaller position)
+      for (int j = 0; j < kCluster * kWarps; ++j) below += (ts.allw[j] > v || (ts.allw[j] == v && j < t)) ? 1 : 0;
+      if (below == ne - 1) ts.tau0 = v;
+    }
+    __syncthreads();
+    const uint32_t tau0 = ts.tau0;
+    u64 above;
+    zero_hist(s);
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t b = xb[i];
+      if (not_nan_bits(b) && top_key(b) >= tau0) atomicAdd(&s.hist[top_key(b) >> 8], 1ull);
+    }
+    const int hi = hist_select<true>(s, static_cast<u64>(ne), 0, 0.0, above);
+    zero_hist(s);
+    for (int i = threadIdx.x; i < n_loc; i += kThreads) {
+      const uint32_t b = xb[i];
+      if (not_nan_bits(b) && top_key(b) >= tau0 && static_cast<int>(top_key(b) >> 8) == hi) atomicAdd(&s.hist[top_key(b) & 255u], 1ull);
+    }
+    const int lo = hist_select<true>(s, static_cast<u64>(ne) - above, 0, 0.0, above);
+    const uint32_t tau = static_cast<uint32_t>(hi << 8 | lo);
+    if (threadIdx.x == 0) ts.n_above = 0;
+    __syncthreads();
+    const int per = (n_loc + kThreads - 1) / kThreads;
+    const int i0 = min(static_cast<int>(threadIdx.x) * per, n_loc), i1 = min(i0 + per, n_loc);
+    u64 ce = 0;
+    for (int i = i0; i < i1; ++i) {
+      const uint32_t b = xb[i];
+      if (!not_nan_bits(b)) continue;
+      const uint32_t k = top_key(b);
+      if (k > tau) {
+        const int slot = atomicAdd(&ts.n_above, 1);
+        ts.above_key[slot] = k;
+        ts.above_idx[slot] = g0 + i;
+      } else if (k == tau) {
+        ++ce;
+      }
+    }
+    const u64 ex = block_excl_scan(ce, s.red);
+    if (ce > 0 && ex < static_cast<u64>(ne)) {
+      int j = static_cast<int>(ex);
+      for (int i = i0; i < i1 && j < ne; ++i) {
+        const uint32_t b = xb[i];
+        if (not_nan_bits(b) && top_key(b) == tau) ts.eq_idx[j++] = g0 + i;
+      }
+    }
+    if (threadIdx.x == kThreads - 1) ts.n_eq = static_cast<int>(min(ex + ce, static_cast<u64>(ne)));
+    cluster_sync();  // every CTA's lists are complete
+    if (rank == 0 && threadIdx.x == 0) {
+      int m = 0;
+      for (int r = 0; r < kCluster; ++r) {  // the keys > tau, insertion-sorted by (key descending, index ascending)
+        const TopSmem* p = peer(&ts, r);
+        for (int a = 0; a < p->n_above; ++a) {
+          const uint32_t k = p->above_key[a];
+          const int idx = p->above_idx[a];
+          int j = m++;
+          while (j > 0 && (ts.top_key[j - 1] < k || (ts.top_key[j - 1] == k && ts.top_idx[j - 1] > idx))) {
+            ts.top_key[j] = ts.top_key[j - 1];
+            ts.top_idx[j] = ts.top_idx[j - 1];
+            --j;
+          }
+          ts.top_key[j] = k;
+          ts.top_idx[j] = idx;
+        }
+      }
+      for (int r = 0; r < kCluster && m < ne; ++r) {  // then the ties at tau, lowest indices first
+        const TopSmem* p = peer(&ts, r);
+        for (int a = 0; a < p->n_eq && m < ne; ++a) {
+          ts.top_key[m] = tau;
+          ts.top_idx[m++] = p->eq_idx[a];
+        }
+      }
+    }
+  }
+  if (rank == 0 && threadIdx.x == 0) {
+    const long long t = tokens[row];
+    logprob[row] = (t >= 0 && t < V) ? lp_of(__half2float(lrow[t])) : kNan;
+    for (int j = 0; j < n; ++j) {
+      const bool listed = j < ne;
+      top_ids[static_cast<size_t>(row) * n + j] = listed ? ts.top_idx[j] : -1;
+      top_logprobs[static_cast<size_t>(row) * n + j] =
+          listed ? lp_of(__half2float(__ushort_as_half(static_cast<unsigned short>(key_bits(ts.top_key[j]))))) : (none ? kNan : -INFINITY);
+    }
+  }
+  cluster_sync();  // the peers' lists stay alive until rank 0 has read them
+}
+
 int slice_cap_of(int V) { return ((V / 8 + kCluster - 1) / kCluster) * 8; }
 
 }  // namespace
@@ -546,6 +821,36 @@ int tree_accept_sampling(const TreeAcceptSamplingArgs& a) {
   return launch(tree_accept_sampling_kernel, dim3(static_cast<unsigned>(a.batch) * kCluster), dim3(kThreads), smem, kCluster, a.stream,
                 "tree_accept_sampling", a.draft, a.tree_mask, static_cast<const __half*>(a.logits), a.draft_probs, a.temperature, a.top_k, a.top_p,
                 static_cast<u64>(a.seed), a.offsets, a.accept_len, a.path, a.bonus, a.num_nodes, a.vocab, cap);
+}
+
+int apply_penalties(const PenaltyArgs& a) {
+  QS_REQUIRE(a.rows >= 0 && a.vocab >= 8 && a.vocab % 8 == 0 && a.vocab <= kMaxVocab, "apply_penalties: rows=%d vocab=%d (a multiple of 8, 8 .. %d)",
+             a.rows, a.vocab, kMaxVocab);
+  QS_REQUIRE(a.history_len >= 0 && a.history_len <= kMaxHistory, "apply_penalties: history_len=%d (0 .. %d)", a.history_len, kMaxHistory);
+  if (a.rows == 0 || a.history_len == 0) return QS_OK;
+  QS_REQUIRE(a.logits && a.history && a.prompt_lens && a.seq_lens && a.repetition && a.presence && a.frequency, "apply_penalties: null pointer");
+  int n = 1;
+  while (n < a.history_len) n <<= 1;
+  const size_t smem = static_cast<size_t>(n) * sizeof(uint32_t);
+  const int rc = raise_smem_limit(apply_penalties_kernel, smem, "apply_penalties");
+  if (rc) return rc;
+  return launch(apply_penalties_kernel, dim3(static_cast<unsigned>(a.rows)), dim3(kPenThreads), smem, 0, a.stream, "apply_penalties",
+                static_cast<__half*>(a.logits), a.history, a.prompt_lens, a.seq_lens, a.repetition, a.presence, a.frequency, a.vocab,
+                a.history_len);
+}
+
+int logprobs_rows(const LogprobArgs& a) {
+  QS_REQUIRE(a.rows >= 0 && a.vocab >= 8 && a.vocab % 8 == 0 && a.vocab <= kMaxVocab, "logprobs_rows: rows=%d vocab=%d (a multiple of 8, 8 .. %d)",
+             a.rows, a.vocab, kMaxVocab);
+  QS_REQUIRE(a.n >= 0 && a.n <= kMaxTop, "logprobs_rows: n=%d (0 .. %d)", a.n, kMaxTop);
+  QS_REQUIRE(a.rows <= 0x7fffffff / kCluster, "logprobs_rows: too many rows");
+  if (a.rows == 0) return QS_OK;
+  QS_REQUIRE(a.logprob && a.logits && a.tokens && (a.n == 0 || (a.top_ids && a.top_logprobs)), "logprobs_rows: null pointer");
+  const size_t smem = static_cast<size_t>(slice_cap_of(a.vocab)) * 2;
+  const int rc = raise_smem_limit(logprobs_rows_kernel, smem, "logprobs_rows");
+  if (rc) return rc;
+  return launch(logprobs_rows_kernel, dim3(static_cast<unsigned>(a.rows) * kCluster), dim3(kThreads), smem, kCluster, a.stream, "logprobs_rows",
+                a.logprob, a.top_ids, a.top_logprobs, static_cast<const __half*>(a.logits), a.tokens, a.n, a.vocab);
 }
 
 }  // namespace qs

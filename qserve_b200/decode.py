@@ -95,13 +95,20 @@ class DecodeRunner:
     def __init__(self, model: str = "llama-3-8b", precision: str = "w4a8kv4", batch: int = 64, ctx: int = 1024,
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
-                 verify_len: int = 0):
+                 verify_len: int = 0, max_new_tokens: int = 0):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
         ctx + verify_len tokens and verify buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers and its
-        random draws exactly as they are without it."""
+        random draws exactly as they are without it.
+
+        max_new_tokens > 0 adds penalties and log-probabilities to the decode step (forward(..., penalties=True, logprobs=n)): the token
+        history s_history int64 [batch, ctx + max_new_tokens] (the caller writes the prompts into [:, :ctx]; the step appends its token),
+        s_prompt_lens / s_seq_lens (= ctx), the per-row s_repetition / s_presence / s_frequency (neutral: 1, 0, 0) and the log-probability
+        outputs s_logprob [batch], s_top_ids / s_top_logprobs [batch, n].  All made with torch.full / torch.zeros: max_new_tokens = 0 and
+        max_new_tokens > 0 give the same weights, pages and greedy / sampled steps."""
         assert precision in PRECISIONS, precision
         assert 0 <= verify_len <= 16, "verify_len: at most 16 draft tokens per sequence"
         assert verify_len == 0 or (tp_size == 1 and fused), "the verify step is single-GPU and uses the fused path"
+        assert max_new_tokens == 0 or 0 < ctx + max_new_tokens <= _ext.MAX_PENALTY_HISTORY, "the token history holds at most 32768 tokens per row"
         self.verify_len = verify_len
         self.ops = ops = ops or DEFAULT_OPS
         self.tp_exact = tp_exact
@@ -201,6 +208,10 @@ class DecodeRunner:
         self.s_top_k = torch.full((batch,), 1, dtype=torch.int32, device=dev)
         self.s_top_p = torch.full((batch,), 1.0, dtype=torch.float32, device=dev)
         self.s_offsets = torch.full((batch,), 0, dtype=torch.int64, device=dev)
+        self.max_new_tokens = max_new_tokens
+        self.graphs = {}  # (sample, penalties, logprobs) -> CUDA graph (capture); self.graph is the latest
+        if max_new_tokens:
+            self._alloc_penalty_buffers()
 
     # ---------------------------------------------------------------------------------------------------------
     def _norm_quant(self, x, gamma):
@@ -226,13 +237,52 @@ class DecodeRunner:
         if self.tp_size > 1 and not self.no_comm:
             torch.distributed.all_reduce(t, group=self.pg)
 
-    def forward(self, tokens: torch.Tensor, sample: bool = False) -> torch.Tensor:
+    def forward(self, tokens: torch.Tensor, sample: bool = False, penalties: bool = False, logprobs: int = 0) -> torch.Tensor:
         """One decode step for `batch` sequences; returns the greedy next tokens [batch] (device).  sample=True ends the step in sample_rows
-        with the per-row s_temperature / s_top_k / s_top_p, seed s_seed and counters s_offsets (advanced by one) instead of argmax_rows."""
-        if not sample:
-            return self._forward_fused(tokens) if self.fused else self._forward_reference(tokens)
+        with the per-row s_temperature / s_top_k / s_top_p, seed s_seed and counters s_offsets (advanced by one) instead of argmax_rows.
+
+        penalties / logprobs (need max_new_tokens > 0): logits -> apply_penalties (s_history, s_prompt_lens, s_seq_lens, s_repetition,
+        s_presence, s_frequency) if penalties -> sample_rows / argmax_rows -> logprobs_rows of the penalised logits with n = logprobs
+        (s_logprob, s_top_ids, s_top_logprobs: the distribution before the temperature / top-k / top-p warpers) if logprobs > 0 -> the token
+        is appended to s_history at s_seq_lens (index clamped to the last column) and s_seq_lens advances by one.  A caller must not run
+        more than max_new_tokens such steps (eager or replayed) without resetting s_seq_lens and s_history."""
+        if not (penalties or logprobs):
+            if not sample:
+                return self._forward_fused(tokens) if self.fused else self._forward_reference(tokens)
+            logits = self._forward_fused(tokens, True) if self.fused else self._forward_reference(tokens, True)
+            return _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets)
+        assert self.max_new_tokens, "construct the runner with max_new_tokens > 0 for penalties / logprobs"
         logits = self._forward_fused(tokens, True) if self.fused else self._forward_reference(tokens, True)
-        return _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets)
+        if penalties:
+            _ext.apply_penalties(logits, self.s_history, self.s_prompt_lens, self.s_seq_lens, self.s_repetition, self.s_presence, self.s_frequency)
+        if sample:
+            tok = _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets)
+        else:
+            tok = _ext.argmax_rows(logits)
+        if logprobs:
+            _ext.logprobs_rows(logits, tok, int(logprobs), self.s_logprob, *self.top_logprobs_view(int(logprobs)))
+        col = self.s_seq_lens.clamp(max=self.s_history.size(1) - 1).long().unsqueeze(1)
+        self.s_history.scatter_(1, col, tok.unsqueeze(1))
+        self.s_seq_lens.add_(1)
+        return tok
+
+    def _alloc_penalty_buffers(self) -> None:
+        B, dev = self.batch, self.dev
+        self.s_history = torch.full((B, self.ctx + self.max_new_tokens), -1, dtype=torch.int64, device=dev)
+        self.s_prompt_lens = torch.full((B,), self.ctx, dtype=torch.int32, device=dev)
+        self.s_seq_lens = torch.full((B,), self.ctx, dtype=torch.int32, device=dev)
+        self.s_repetition = torch.full((B,), 1.0, dtype=torch.float32, device=dev)
+        self.s_presence = torch.zeros(B, dtype=torch.float32, device=dev)
+        self.s_frequency = torch.zeros(B, dtype=torch.float32, device=dev)
+        self.s_logprob = torch.zeros(B, dtype=torch.float32, device=dev)
+        # flat, so that [:B n] viewed as [B, n] is contiguous for any n <= 20
+        self.s_top_ids = torch.zeros(B * _ext.MAX_TOP_LOGPROBS, dtype=torch.int64, device=dev)
+        self.s_top_logprobs = torch.zeros(B * _ext.MAX_TOP_LOGPROBS, dtype=torch.float32, device=dev)
+
+    def top_logprobs_view(self, n: int):
+        """(s_top_ids, s_top_logprobs) as the [batch, n] tensors a step with logprobs = n writes."""
+        B = self.batch
+        return self.s_top_ids[: B * n].view(B, n), self.s_top_logprobs[: B * n].view(B, n)
 
     def _attention(self, li):
         cfg, D = self.cfg, self.cfg.head_dim
@@ -569,24 +619,28 @@ class DecodeRunner:
         self.context_lens.copy_(full.context_lens)
 
     # ---------------------------------------------------------------------------------------------------------
-    def capture(self, warmup: int = 2, sample: bool = False) -> None:
+    def capture(self, warmup: int = 2, sample: bool = False, penalties: bool = False, logprobs: int = 0) -> None:
         """Warm up eagerly (allocates workspaces, sets kernel attributes) and capture the whole step in a CUDA graph.  sample=True: the step
-        ends in sample_rows (see forward); each warm-up call and each replay advances s_offsets by one."""
+        ends in sample_rows (see forward); each warm-up call and each replay advances s_offsets by one.  penalties / logprobs: see forward;
+        each warm-up call and each replay appends one token to s_history.  The graph is kept in graphs[(sample, penalties, logprobs)] and
+        becomes self.graph."""
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(s), torch.no_grad():
             for _ in range(warmup):
-                self.tokens_out.copy_(self.forward(self.tokens_in, sample))
+                self.tokens_out.copy_(self.forward(self.tokens_in, sample, penalties, logprobs))
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         g = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(g):
-            self.tokens_out.copy_(self.forward(self.tokens_in, sample))
+            self.tokens_out.copy_(self.forward(self.tokens_in, sample, penalties, logprobs))
         self.graph = g
+        self.graphs[(bool(sample), bool(penalties), int(logprobs))] = g
 
-    def step(self) -> None:
-        """Replay the captured step: tokens_in -> tokens_out (both device resident)."""
-        self.graph.replay()
+    def step(self, key: Optional[tuple] = None) -> None:
+        """Replay the captured step: tokens_in -> tokens_out (both device resident).  key = (sample, penalties, logprobs) selects one of
+        graphs; None replays the latest capture."""
+        (self.graph if key is None else self.graphs[key]).replay()
 
     def weight_bytes_per_step(self) -> int:
         return sum(l.weight_bytes() for ly in self.layers for l in (ly["qkv"], ly["o"], ly["gate_up"], ly["down"]))
