@@ -343,6 +343,34 @@ QS_API int qs_apply_penalties(void* logits, const int64_t* history, const int32_
 QS_API int qs_logprobs_rows(float* logprob, int64_t* top_ids, float* top_logprobs, const void* logits, const int64_t* tokens, int rows, int vocab,
                             int n, void* stream);
 
+/* Prompt-lookup speculative decoding: the drafter and the commit that close the loop around the tree verify and acceptance above.  Both read
+ * every input after the PDL dependency wait (the previous step's commit writes the history and the lengths), need no host synchronisation,
+ * are CUDA-graph capturable and bitwise deterministic.  Row state: history int64 [batch, history_len] holds the prompt and the generated
+ * tokens, seq_lens int32 [batch] = L, the last token h[L - 1] (the ROOT) is the latest emitted token and is not yet in the KV cache, so the
+ * cache holds L - 1 tokens.
+ *
+ * qs_ngram_propose: a draft tree of num_nodes = n <= 16 nodes (root included) per row from the row's own history (Saxena 2023 prompt
+ *   lookup).  L is clamped to [0, history_len <= 32768].  For every end position j in [0, L - 2], m(j) is the largest g <= min(n_max, j + 1)
+ *   with h[j - g + 1 .. j] == h[L - g .. L - 1] and every id of both windows >= 0 (the windows may overlap).  Candidates are the j with
+ *   m(j) >= n_min, ranked by (m descending, j descending); the first `branches` are taken.  The continuation of candidate j is
+ *   h[j + 1 .. min(j + n - 1, L - 1)].  Node 0 is the root (token h[L - 1], or -1 if L = 0; mask 0).  The continuations are inserted in rank
+ *   order into a trie below the root: an existing child with the same token is followed, otherwise node `count` is created (creation order is
+ *   topological) with mask = mask[parent] | (1 << parent), until n nodes exist.  Uncreated nodes are padding: token -1, mask 1.  Outputs
+ *   tokens int64 [batch, n] and tree_mask int32 [batch, n], the ancestor words of qs_tree_decode_attention.  1 <= n_min <= n_max <= 8,
+ *   1 <= branches <= 8.
+ * qs_spec_commit: advances every unfinished row (finished[b] == 0; finished rows are not touched) by what its step accepted: draft_tokens
+ *   int64 [batch, n], path int32 [batch, n], accept_len int32 [batch] and bonus int64 [batch] as qs_tree_accept_greedy / _sampling return
+ *   them (acc = accept_len clamped to [1, n], path entries to [0, n - 1]).  The appended tokens draft[path[1 .. acc - 1]], bonus are cut after
+ *   the first eos[b] (eos < 0: none), then to budget[b] - (L - prompt_lens[b]) (at least 0) tokens, written at history[L ..] (columns >=
+ *   history_len dropped) and L += count.  Then start_pos = L - 1, context_lens = L and roots = the row's last token (the last appended one,
+ *   else h[L - 1]); context_lens and roots may be NULL.  The row becomes finished if it appended eos or L - prompt_lens >= budget.  A plain
+ *   decode step is the call with n = 1, path = 0, accept_len = 1 and bonus = the sampled token.                                          */
+QS_API int qs_ngram_propose(const int64_t* history, const int32_t* seq_lens, int64_t* tokens, int32_t* tree_mask, int batch, int history_len,
+                            int num_nodes, int n_min, int n_max, int branches, void* stream);
+QS_API int qs_spec_commit(const int64_t* draft_tokens, const int32_t* path, const int32_t* accept_len, const int64_t* bonus, int64_t* history,
+                          int32_t* seq_lens, const int32_t* prompt_lens, const int32_t* budget, const int64_t* eos, int32_t* finished,
+                          int32_t* start_pos, int32_t* context_lens, int64_t* roots, int batch, int num_nodes, int history_len, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -817,6 +817,80 @@ def logprobs_rows(logits, tokens, n: int, logprob: Optional[torch.Tensor] = None
     return logprob, top_ids, top_logprobs
 
 
+MAX_DRAFT_NGRAM = 8
+MAX_DRAFT_BRANCHES = 8
+
+
+def _rows_tensor(t, name: str, dt, shape, dev) -> None:
+    _cuda(t, name)
+    _require(t.dtype == dt and t.is_contiguous() and tuple(t.shape) == tuple(shape) and t.device == dev, f"{name} must be contiguous {dt} {tuple(shape)}")
+
+
+def ngram_propose(history, seq_lens, num_nodes: int, n_min: int = 1, n_max: int = 4, branches: int = 1, tokens: Optional[torch.Tensor] = None,
+                  tree_mask: Optional[torch.Tensor] = None):
+    """Prompt-lookup draft trees (n-gram drafting) from each row's own token history, one CTA per row and no host synchronisation.
+    history int64 [B, H] (H <= 32768), seq_lens int32 [B] = L (clamped to [0, H] on the device); the last token h[L - 1] is the root.  For
+    every end position j <= L - 2, m(j) is the longest g <= min(n_max, j + 1) with h[j - g + 1 .. j] == h[L - g .. L - 1] (ids < 0 never
+    match); the j with m(j) >= n_min, ranked by (m, j) descending, give up to `branches` continuations h[j + 1 .. min(j + n - 1, L - 1)],
+    inserted in rank order into a trie below the root until num_nodes = n nodes exist.  Returns (tokens int64 [B, n], tree_mask int32 [B, n])
+    ready for verify_forward / tree_accept_*: node 0 is the root (mask 0), padding nodes have token -1 and mask 1.  1 <= n <= 16,
+    1 <= n_min <= n_max <= 8, 1 <= branches <= 8.  The optional out tensors are written in place (CUDA-graph capture).  See
+    include/qserve_b200.h."""
+    n, n_min, n_max, branches = int(num_nodes), int(n_min), int(n_max), int(branches)
+    _require(1 <= n <= 16, f"num_nodes={n}: a draft tree has 1 .. 16 nodes")
+    _require(1 <= n_min <= n_max <= MAX_DRAFT_NGRAM, f"n_min={n_min}, n_max={n_max}: need 1 <= n_min <= n_max <= {MAX_DRAFT_NGRAM}")
+    _require(1 <= branches <= MAX_DRAFT_BRANCHES, f"branches={branches}: 1 .. {MAX_DRAFT_BRANCHES}")
+    _cuda(history, "history")
+    _require(history.dtype == torch.int64 and history.dim() == 2 and history.is_contiguous(), "history must be contiguous int64 [B, H]")
+    B, H = history.shape
+    _require(1 <= H <= MAX_PENALTY_HISTORY, f"history of {H} tokens per row: 1 .. {MAX_PENALTY_HISTORY}")
+    dev = history.device
+    _rows_tensor(seq_lens, "seq_lens", torch.int32, (B,), dev)
+    tokens = torch.empty((B, n), dtype=torch.int64, device=dev) if tokens is None else tokens
+    tree_mask = torch.empty((B, n), dtype=torch.int32, device=dev) if tree_mask is None else tree_mask
+    _rows_tensor(tokens, "tokens", torch.int64, (B, n), dev)
+    _rows_tensor(tree_mask, "tree_mask", torch.int32, (B, n), dev)
+    if B:
+        _call(history, lib.qs_ngram_propose, history.data_ptr(), seq_lens.data_ptr(), tokens.data_ptr(), tree_mask.data_ptr(), B, H, n, n_min, n_max,
+              branches)
+    return tokens, tree_mask
+
+
+def spec_commit(draft_tokens, path, accept_len, bonus, history, seq_lens, prompt_lens, budget, eos, finished, start_pos,
+                context_lens: Optional[torch.Tensor] = None, roots: Optional[torch.Tensor] = None) -> None:
+    """Advance every unfinished row by what its speculative step accepted, in place and without host synchronisation: the tokens
+    draft_tokens[b, path[b, 1 .. acc - 1]] and bonus[b] (acc = accept_len[b]; draft_tokens int64 [B, n], path int32 [B, n], accept_len int32 [B]
+    and bonus int64 [B] as tree_accept_greedy / tree_accept_sampling return them) are cut after the first eos[b] (int64 [B], -1: none), then
+    to budget[b] - (L - prompt_lens[b]) tokens (int32 [B]), and appended to history int64 [B, H] at L = seq_lens[b] (columns >= H dropped);
+    seq_lens advances by the count.  start_pos (int32 [B]) = L - 1, the optional context_lens (int32 [B]) = L and roots (int64 [B]) = the last
+    token: what the next verify step (start_pos) or decode step (context_lens, tokens = roots) reads.  finished int32 [B] is set when a row
+    appends eos or reaches its budget; finished rows are left untouched.  A plain decode step commits with n = 1, path = 0, accept_len = 1 and
+    bonus = its token.  See include/qserve_b200.h."""
+    _cuda(draft_tokens, "draft_tokens")
+    _require(draft_tokens.dtype == torch.int64 and draft_tokens.dim() == 2 and draft_tokens.is_contiguous(), "draft_tokens must be contiguous int64 [B, n]")
+    B, n = draft_tokens.shape
+    _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
+    dev = draft_tokens.device
+    _cuda(history, "history")
+    _require(history.dtype == torch.int64 and history.dim() == 2 and history.is_contiguous() and history.size(0) == B and history.device == dev,
+             f"history must be contiguous int64 [{B}, H] on the device of the drafts")
+    H = history.size(1)
+    _require(1 <= H <= MAX_PENALTY_HISTORY, f"history of {H} tokens per row: 1 .. {MAX_PENALTY_HISTORY}")
+    _rows_tensor(path, "path", torch.int32, (B, n), dev)
+    for t, nm, dt in ((accept_len, "accept_len", torch.int32), (bonus, "bonus", torch.int64), (seq_lens, "seq_lens", torch.int32),
+                      (prompt_lens, "prompt_lens", torch.int32), (budget, "budget", torch.int32), (eos, "eos", torch.int64),
+                      (finished, "finished", torch.int32), (start_pos, "start_pos", torch.int32)):
+        _rows_tensor(t, nm, dt, (B,), dev)
+    if context_lens is not None:
+        _rows_tensor(context_lens, "context_lens", torch.int32, (B,), dev)
+    if roots is not None:
+        _rows_tensor(roots, "roots", torch.int64, (B,), dev)
+    if B:
+        _call(history, lib.qs_spec_commit, draft_tokens.data_ptr(), path.data_ptr(), accept_len.data_ptr(), bonus.data_ptr(), history.data_ptr(),
+              seq_lens.data_ptr(), prompt_lens.data_ptr(), budget.data_ptr(), eos.data_ptr(), finished.data_ptr(), start_pos.data_ptr(),
+              context_lens.data_ptr() if context_lens is not None else None, roots.data_ptr() if roots is not None else None, B, n, H)
+
+
 class PeerContext:
     """Peer-mapped buffers of a tensor-parallel group for the fused all-reduce (qs_add_rms_norm_general_peer): built once from
     torch.distributed._symmetric_memory (device memory + NVLink peer mappings are torch's plumbing; the kernel is ours).

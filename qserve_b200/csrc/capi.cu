@@ -321,7 +321,27 @@ int qs_logprobs_rows(float* logprob, int64_t* top_ids, float* top_logprobs, cons
   return logprobs_rows(a);
 }
 
-int qs_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
+int qs_ngram_propose(const int64_t* history, const int32_t* seq_lens, int64_t* tokens, int32_t* tree_mask, int batch, int history_len, int num_nodes,
+                     int n_min, int n_max, int branches, void* stream) {
+  NgramProposeArgs a;
+  a.history = reinterpret_cast<const long long*>(history); a.seq_lens = seq_lens; a.tokens = reinterpret_cast<long long*>(tokens);
+  a.tree_mask = tree_mask; a.batch = batch; a.history_len = history_len; a.num_nodes = num_nodes; a.n_min = n_min; a.n_max = n_max;
+  a.branches = branches; a.stream = stream;
+  return ngram_propose(a);
+}
+
+int qs_spec_commit(const int64_t* draft_tokens, const int32_t* path, const int32_t* accept_len, const int64_t* bonus, int64_t* history, int32_t* seq_lens,
+                   const int32_t* prompt_lens, const int32_t* budget, const int64_t* eos, int32_t* finished, int32_t* start_pos, int32_t* context_lens,
+                   int64_t* roots, int batch, int num_nodes, int history_len, void* stream) {
+  SpecCommitArgs a;
+  a.draft = reinterpret_cast<const long long*>(draft_tokens); a.path = path; a.accept_len = accept_len; a.bonus = reinterpret_cast<const long long*>(bonus);
+  a.history = reinterpret_cast<long long*>(history); a.seq_lens = seq_lens; a.prompt_lens = prompt_lens; a.budget = budget;
+  a.eos = reinterpret_cast<const long long*>(eos); a.finished = finished; a.start_pos = start_pos; a.context_lens = context_lens;
+  a.roots = reinterpret_cast<long long*>(roots); a.batch = batch; a.num_nodes = num_nodes; a.history_len = history_len; a.stream = stream;
+  return spec_commit(a);
+}
+
+int qs_prefill_attention(const void* q,const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
                          int64_t out_stride, const int32_t* cu_seqlens, int batch, int num_tokens, int max_seqlen, int num_heads, int num_kv_heads,
                          int head_dim, float softmax_scale, void* stream) {
   PrefillAttnArgs a;

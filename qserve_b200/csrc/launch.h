@@ -231,4 +231,33 @@ struct LogprobArgs {
 };
 int logprobs_rows(const LogprobArgs& a);
 
+// speculative.cu: prompt-lookup draft trees from the token history, and the commit that advances every sequence by what it accepted
+struct NgramProposeArgs {
+  const long long* history = nullptr;  // [batch, history_len]
+  const int* seq_lens = nullptr;       // [batch], clamped to [0, history_len] on the device
+  long long* tokens = nullptr;         // [batch, num_nodes] out: root, drafted nodes, padding -1
+  int* tree_mask = nullptr;            // [batch, num_nodes] out: ancestor words, padding 1
+  int batch = 0, history_len = 0, num_nodes = 0, n_min = 1, n_max = 4, branches = 1;
+  void* stream = nullptr;
+};
+int ngram_propose(const NgramProposeArgs& a);
+struct SpecCommitArgs {
+  const long long* draft = nullptr;    // [batch, num_nodes]
+  const int* path = nullptr;           // [batch, num_nodes]
+  const int* accept_len = nullptr;     // [batch]
+  const long long* bonus = nullptr;    // [batch]
+  long long* history = nullptr;        // [batch, history_len], appended in place
+  int* seq_lens = nullptr;             // [batch], advanced in place
+  const int* prompt_lens = nullptr;    // [batch]
+  const int* budget = nullptr;         // [batch] tokens a row may generate
+  const long long* eos = nullptr;      // [batch], -1: none
+  int* finished = nullptr;             // [batch], set in place
+  int* start_pos = nullptr;            // [batch] out: seq_lens - 1
+  int* context_lens = nullptr;         // optional [batch] out: seq_lens
+  long long* roots = nullptr;          // optional [batch] out: the last token of the row
+  int batch = 0, num_nodes = 0, history_len = 0;
+  void* stream = nullptr;
+};
+int spec_commit(const SpecCommitArgs& a);
+
 }  // namespace qs

@@ -95,7 +95,7 @@ class DecodeRunner:
     def __init__(self, model: str = "llama-3-8b", precision: str = "w4a8kv4", batch: int = 64, ctx: int = 1024,
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
-                 verify_len: int = 0, max_new_tokens: int = 0):
+                 verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
         ctx + verify_len tokens and verify buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers and its
         random draws exactly as they are without it.
@@ -104,11 +104,24 @@ class DecodeRunner:
         history s_history int64 [batch, ctx + max_new_tokens] (the caller writes the prompts into [:, :ctx]; the step appends its token),
         s_prompt_lens / s_seq_lens (= ctx), the per-row s_repetition / s_presence / s_frequency (neutral: 1, 0, 0) and the log-probability
         outputs s_logprob [batch], s_top_ids / s_top_logprobs [batch, n].  All made with torch.full / torch.zeros: max_new_tokens = 0 and
-        max_new_tokens > 0 give the same weights, pages and greedy / sampled steps."""
+        max_new_tokens > 0 give the same weights, pages and greedy / sampled steps.
+
+        generate=True (single GPU, fused path, max_new_tokens = T >= 1) adds the generation loop (reset_generation, generate_forward,
+        capture_generate / generate_step): plain decode steps (n = 1) and prompt-lookup speculative steps (2 <= n <= verify_len) that advance
+        every row by what it accepted.  The history is [batch, ctx + 1 + T] (the prompt is ctx cached tokens and the root), the page tables
+        cover ctx + T + max(1, verify_len) tokens (the pages past blocks_per_seq come from zero-filled pools made after every random draw, so
+        the weights and the first blocks_per_seq pages of each row are those of generate=False), and the per-row state is g_budget (tokens a
+        row may generate, default T), g_eos (-1: none) and g_finished."""
         assert precision in PRECISIONS, precision
         assert 0 <= verify_len <= 16, "verify_len: at most 16 draft tokens per sequence"
         assert verify_len == 0 or (tp_size == 1 and fused), "the verify step is single-GPU and uses the fused path"
         assert max_new_tokens == 0 or 0 < ctx + max_new_tokens <= _ext.MAX_PENALTY_HISTORY, "the token history holds at most 32768 tokens per row"
+        self.generate = generate
+        if generate:
+            assert tp_size == 1 and fused, "generation is single-GPU and uses the fused path"
+            assert max_new_tokens >= 1, "generate=True needs max_new_tokens >= 1"
+            assert ctx + 1 + max_new_tokens <= _ext.MAX_PENALTY_HISTORY, "the token history holds at most 32768 tokens per row"
+            assert ctx + max_new_tokens + max(1, verify_len) <= min(8192, MODELS[model].max_pos), "generation runs past the positions the attention supports"
         self.verify_len = verify_len
         self.ops = ops = ops or DEFAULT_OPS
         self.tp_exact = tp_exact
@@ -174,9 +187,24 @@ class DecodeRunner:
             self.kpools.append(pools[0]); self.vpools.append(pools[1])
             # [B, 2, blocks] absolute addresses (model_runner.py:506-530)
             tables.append(torch.stack([pools[0].data_ptr() + blk * self.page_bytes, pools[1].data_ptr() + blk * self.page_bytes], dim=1))
+        self.table_blocks = self.blocks_per_seq
+        self.kpools_gen, self.vpools_gen = [], []
+        if generate:  # pages for the generated tokens: zero-filled (no generator draws), after the pages above in every row's table
+            self.table_blocks = (ctx + max_new_tokens + max(1, verify_len) + 63) // 64
+            extra = self.table_blocks - self.blocks_per_seq
+            if extra:
+                blk = torch.arange(batch * extra, device=dev, dtype=torch.int64).view(batch, extra)
+                for li in range(self.L):
+                    kp = torch.zeros((batch * extra, self.page_bytes), dtype=torch.uint8, device=dev)
+                    vp = torch.zeros_like(kp)
+                    self.kpools_gen.append(kp); self.vpools_gen.append(vp)
+                    more = torch.stack([kp.data_ptr() + blk * self.page_bytes, vp.data_ptr() + blk * self.page_bytes], dim=1)
+                    tables[li] = torch.cat([tables[li], more], dim=2)
         self.block_tables = torch.stack(tables, dim=0).contiguous()  # [L, B, 2, blocks]
         self.context_lens = torch.full((batch,), ctx + 1, dtype=torch.int32, device=dev)
-        self.max_seq_len = ctx + 1
+        # host bounds of the attention launches: in generation the contexts grow up to ctx + 1 + max_new_tokens
+        self.max_seq_len = ctx + 1 + (max_new_tokens if generate else 0)
+        self.max_prefix_len = ctx + (max_new_tokens if generate else 0)
 
         # ---- persistent ActivationBuffer (input_metadata.py:71-109; aliasing kept) ------------------------------
         # (H is in the max for tensor parallelism: at TP = 8 a 72B model's sharded qkv / gate_up rows are narrower than the full hidden row of out_buf)
@@ -212,6 +240,8 @@ class DecodeRunner:
         self.graphs = {}  # (sample, penalties, logprobs) -> CUDA graph (capture); self.graph is the latest
         if max_new_tokens:
             self._alloc_penalty_buffers()
+        if generate:
+            self._alloc_generate_buffers()
 
     # ---------------------------------------------------------------------------------------------------------
     def _norm_quant(self, x, gamma):
@@ -268,7 +298,7 @@ class DecodeRunner:
 
     def _alloc_penalty_buffers(self) -> None:
         B, dev = self.batch, self.dev
-        self.s_history = torch.full((B, self.ctx + self.max_new_tokens), -1, dtype=torch.int64, device=dev)
+        self.s_history = torch.full((B, self.ctx + int(self.generate) + self.max_new_tokens), -1, dtype=torch.int64, device=dev)
         self.s_prompt_lens = torch.full((B,), self.ctx, dtype=torch.int32, device=dev)
         self.s_seq_lens = torch.full((B,), self.ctx, dtype=torch.int32, device=dev)
         self.s_repetition = torch.full((B,), 1.0, dtype=torch.float32, device=dev)
@@ -458,7 +488,7 @@ class DecodeRunner:
                                                    cfg.rope_theta, min(8192, cfg.max_pos), True, self.kv_bits == 4, True, tree_mask=tm)
             q, k, v = qkv.split([self.q_size, self.kv_size, self.kv_size], dim=-1)
             attn = _ext.multi_token_decode_attention(q.reshape(M, self.Hq, D), k.reshape(M, self.Hkv, D), v.reshape(M, self.Hkv, D), cu, n, self.v_start,
-                                                     self.ctx, table, 64, self.size_per_token, self.kv_bits == 4, tree_mask=tm)
+                                                     self.max_prefix_len, table, 64, self.size_per_token, self.kv_bits == 4, tree_mask=tm)
             if self.act_sum:
                 fused_kernels.invoke_quant_fuse_sum(q_attn, attn.view(M, -1), q_sum, q_scale)
             else:
@@ -549,6 +579,95 @@ class DecodeRunner:
     def verify_step(self, n: int, tree: bool = False, sampled: bool = False, draft_probs: bool = False) -> None:
         """Replay the captured verify step for n draft tokens."""
         self.v_graphs[self._verify_key(n, tree, sampled, draft_probs)].replay()
+
+    # ---------------------------------------------------------------------------------------------------------
+    # generation: plain decode steps and prompt-lookup speculative steps that advance every row by what it accepted
+    # ---------------------------------------------------------------------------------------------------------
+    def _alloc_generate_buffers(self) -> None:
+        """Row state and step buffers of the generation loop (torch.full / torch.zeros: no random draws)."""
+        B, dev, n = self.batch, self.dev, max(1, self.verify_len)
+        self.g_budget = torch.full((B,), self.max_new_tokens, dtype=torch.int32, device=dev)
+        self.g_eos = torch.full((B,), -1, dtype=torch.int64, device=dev)
+        self.g_finished = torch.zeros(B, dtype=torch.int32, device=dev)
+        # the verify step's cached length P = L - 1 (the verify buffers' v_start when there are any)
+        self.g_start = self.v_start if self.verify_len else torch.full((B,), self.ctx, dtype=torch.int32, device=dev)
+        self.g_path1 = torch.zeros((B, 1), dtype=torch.int32, device=dev)  # a plain step commits the path [0] ...
+        self.g_accept1 = torch.ones(B, dtype=torch.int32, device=dev)      # ... of length 1, so only its token is appended
+        # drafts of the speculative step, flat so that [:B n] viewed as [B, n] is contiguous for any n
+        self.g_tokens = torch.zeros(B * n, dtype=torch.int64, device=dev)
+        self.g_mask = torch.zeros(B * n, dtype=torch.int32, device=dev)
+        self.g_graphs = {}  # (n, branches, ngram, sampled) -> CUDA graph
+
+    def reset_generation(self, prompt: torch.Tensor) -> None:
+        """Start generating after prompt int64 [batch, ctx + 1]: the ctx tokens the pages hold, then the root (the latest token, not yet
+        cached).  Sets the history and its lengths, the positions of both step kinds and tokens_in, and clears g_finished; g_budget and g_eos
+        stay as the caller set them."""
+        assert self.generate, "construct the runner with generate=True"
+        B, C = self.batch, self.ctx + 1
+        assert tuple(prompt.shape) == (B, C) and prompt.dtype == torch.int64, f"prompt must be int64 [{B}, {C}]"
+        self.s_history.fill_(-1)
+        self.s_history[:, :C].copy_(prompt)
+        self.s_prompt_lens.fill_(C)
+        self.s_seq_lens.fill_(C)
+        self.g_start.fill_(self.ctx)
+        self.context_lens.fill_(C)
+        self.tokens_in.copy_(prompt[:, self.ctx])
+        self.g_finished.zero_()
+
+    def generate_forward(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False) -> None:
+        """One generation step for every row; the tokens go to s_history (lengths s_seq_lens).  n = 1: the decode step at the rows' own
+        lengths, argmax_rows (or sample_rows with the s_* parameters if sampled), spec_commit of that token.  2 <= n <= verify_len:
+        ngram_propose (n nodes, `branches` continuations, match lengths ngram = (n_min, n_max)) -> verify_forward of the draft tree ->
+        accept_and_compact (or accept_sampled_and_compact with one-hot drafts, which keeps sampling lossless) -> spec_commit.  Finished rows
+        (g_finished) are computed but not advanced.  No host synchronisation."""
+        assert self.generate, "construct the runner with generate=True"
+        B = self.batch
+        common = (self.s_history, self.s_seq_lens, self.s_prompt_lens, self.g_budget, self.g_eos, self.g_finished, self.g_start, self.context_lens,
+                  self.tokens_in)
+        if n == 1:
+            logits = self._forward_fused(self.tokens_in, True)
+            if sampled:
+                tok = _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets, out=self.tokens_out)
+            else:
+                tok = _ext.argmax_rows(logits, out=self.tokens_out)
+            # the path [0] of length 1 never reads the drafts: any [B, 1] tensor that is not an output will do
+            _ext.spec_commit(tok.view(B, 1), self.g_path1, self.g_accept1, tok, *common)
+            return
+        assert 2 <= n <= self.verify_len, f"n={n}: 1, or 2 .. verify_len={self.verify_len}"
+        n_min, n_max = ngram
+        toks = self.g_tokens[: B * n].view(B, n)
+        mask = self.g_mask[: B * n].view(B, n)
+        _ext.ngram_propose(self.s_history, self.s_seq_lens, n, n_min, n_max, branches, tokens=toks, tree_mask=mask)
+        emb = toks.clamp(min=0)  # padding nodes (-1) are embedded as token 0; they are never accepted
+        if sampled:
+            logits = self.verify_forward(emb, return_logits=True, tree_mask=mask)
+            acc, path, bonus = self.accept_sampled_and_compact(toks, mask, logits, None)
+        else:
+            target = self.verify_forward(emb, tree_mask=mask)
+            acc, path, bonus = self.accept_and_compact(toks, mask, target)
+        _ext.spec_commit(toks, path, acc, bonus, *common)
+
+    def _generate_key(self, n: int, branches: int, ngram: tuple, sampled: bool):
+        return (int(n), int(branches), tuple(int(x) for x in ngram), bool(sampled))
+
+    def capture_generate(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False, warmup: int = 2) -> None:
+        """Capture generate_forward(n, branches, ngram, sampled) in a CUDA graph.  The warm-up runs the step eagerly, so it advances the rows
+        like a replay does: call reset_generation afterwards."""
+        s = torch.cuda.Stream(device=self.dev)
+        s.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(s), torch.no_grad():
+            for _ in range(warmup):
+                self.generate_forward(n, branches, ngram, sampled)
+        torch.cuda.current_stream(self.dev).wait_stream(s)
+        torch.cuda.synchronize(self.dev)
+        g = torch.cuda.CUDAGraph()
+        with torch.no_grad(), torch.cuda.graph(g):
+            self.generate_forward(n, branches, ngram, sampled)
+        self.g_graphs[self._generate_key(n, branches, ngram, sampled)] = g
+
+    def generate_step(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False) -> None:
+        """Replay the captured generation step."""
+        self.g_graphs[self._generate_key(n, branches, ngram, sampled)].replay()
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
