@@ -20,7 +20,7 @@ GEMM.  Two quantisation modes for the inputs of the row-parallel GEMMs:
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 
@@ -91,14 +91,26 @@ class _Linear:
         return self.N * self.K if self.mode == "w8" else self.N * self.K // 2
 
 
+class _Rows(NamedTuple):
+    """Views of the first M rows of the ActivationBuffer: what one step's layers read and write."""
+    qkv: torch.Tensor       # fp16 [M, q + 2 kv]
+    out: torch.Tensor       # fp16 [M, hidden], aliases qkv
+    gate_up: torch.Tensor   # fp16 [M, 2 I], aliases qkv
+    q_hidden: torch.Tensor  # int8 [M, hidden]
+    q_attn: torch.Tensor    # int8 [M, q], aliases q_hidden
+    q_mlp: torch.Tensor     # int8 [M, I], aliases q_hidden
+    q_scale: torch.Tensor   # fp16 [M]
+    q_sum: torch.Tensor     # fp16 [M]
+
+
 class DecodeRunner:
     def __init__(self, model: str = "llama-3-8b", precision: str = "w4a8kv4", batch: int = 64, ctx: int = 1024,
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
                  verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
-        ctx + verify_len tokens and verify buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers and its
-        random draws exactly as they are without it.
+        ctx + verify_len tokens and the activation buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers
+        and its random draws exactly as they are without it.
 
         max_new_tokens > 0 adds penalties and log-probabilities to the decode step (forward(..., penalties=True, logprobs=n)): the token
         history s_history int64 [batch, ctx + max_new_tokens] (the caller writes the prompts into [:, :ctx]; the step appends its token),
@@ -125,7 +137,6 @@ class DecodeRunner:
         self.verify_len = verify_len
         self.ops = ops = ops or DEFAULT_OPS
         self.tp_exact = tp_exact
-        self.fuse_attn_quant = True  # attention with the per-token quant fused in: one launch per layer fewer
         self.no_comm = no_comm  # debugging: run one rank's shard of a tensor-parallel model without the collectives (sanitizer / profiler runs)
         # tensor parallel, fused path: the all-reduce of the row-parallel GEMM outputs is folded into the following add+norm+quant kernel
         # (peer loads over NVLink symmetric memory) instead of an NCCL call
@@ -206,18 +217,15 @@ class DecodeRunner:
         self.max_seq_len = ctx + 1 + (max_new_tokens if generate else 0)
         self.max_prefix_len = ctx + (max_new_tokens if generate else 0)
 
-        # ---- persistent ActivationBuffer (input_metadata.py:71-109; aliasing kept) ------------------------------
+        # ---- persistent ActivationBuffer (input_metadata.py:71-109; aliasing kept) for the rows of the widest step --------------------
         # (H is in the max for tensor parallelism: at TP = 8 a 72B model's sharded qkv / gate_up rows are narrower than the full hidden row of out_buf)
-        self.act_buffer = torch.empty(M * max(self.q_size + 2 * self.kv_size, 2 * self.Iloc, H), dtype=torch.half, device=dev)
-        self.qkv_buf = self.act_buffer[: M * (self.q_size + 2 * self.kv_size)].view(M, -1)
-        self.out_buf = self.act_buffer[: M * H].view(M, H)
-        self.gate_up_buf = self.act_buffer[: M * 2 * self.Iloc].view(M, -1)
-        self.q_act = torch.empty(M * max(H, self.Iloc), dtype=torch.int8, device=dev)
-        self.q_hidden = self.q_act[: M * H].view(M, H)
-        self.q_attn = self.q_act[: M * self.q_size].view(M, self.q_size)
-        self.q_mlp = self.q_act[: M * self.Iloc].view(M, self.Iloc)
-        self.q_scale = torch.empty(M, dtype=torch.half, device=dev)
-        self.q_sum = torch.empty(M, dtype=torch.half, device=dev)
+        R = M * max(1, verify_len)
+        self.act_buffer = torch.empty(R * max(self.q_size + 2 * self.kv_size, 2 * self.Iloc, H), dtype=torch.half, device=dev)
+        self.q_act = torch.empty(R * max(H, self.Iloc), dtype=torch.int8, device=dev)
+        self.scale_buffer = torch.empty(R, dtype=torch.half, device=dev)
+        self.sum_buffer = torch.empty(R, dtype=torch.half, device=dev)
+        self.rows = self._row_views(M)  # the decode step's
+        self.qkv_buf, self.out_buf, self.gate_up_buf, self.q_hidden, self.q_attn, self.q_mlp, self.q_scale, self.q_sum = self.rows
         self.q_amax = torch.empty(M, dtype=torch.float32, device=dev)  # TP parity mode: per-token amax, max-all-reduced
         self.mlp_act = torch.empty((M, self.Iloc), dtype=torch.half, device=dev)  # reference: fresh torch.empty per call (activation.py:26)
         self.peer = None
@@ -225,7 +233,8 @@ class DecodeRunner:
             self.peer = _ext.PeerContext(M, H, dev, process_group if process_group is not None else torch.distributed.group.WORLD)
         self.tokens_in = torch.zeros(M, dtype=torch.int64, device=dev)
         self.tokens_out = torch.zeros(M, dtype=torch.int64, device=dev)
-        self.graph: Optional[torch.cuda.CUDAGraph] = None
+        self.graph: Optional[torch.cuda.CUDAGraph] = None  # the latest capture()
+        self.graphs = {}  # ("decode" | "verify" | "generate", *arguments) -> CUDA graph
         self.launches_per_step = 0
         if verify_len:
             self._alloc_verify_buffers()
@@ -237,31 +246,37 @@ class DecodeRunner:
         self.s_top_p = torch.full((batch,), 1.0, dtype=torch.float32, device=dev)
         self.s_offsets = torch.full((batch,), 0, dtype=torch.int64, device=dev)
         self.max_new_tokens = max_new_tokens
-        self.graphs = {}  # (sample, penalties, logprobs) -> CUDA graph (capture); self.graph is the latest
         if max_new_tokens:
             self._alloc_penalty_buffers()
         if generate:
             self._alloc_generate_buffers()
 
     # ---------------------------------------------------------------------------------------------------------
-    def _norm_quant(self, x, gamma):
-        if self.act_sum:  # layernorm.py:88
-            self.ops.layernorm_ops.rms_norm_general_fuse_sum(self.q_hidden, x, gamma, self.q_sum, self.q_scale, self.cfg.eps, True)
-        else:             # layernorm.py:72
-            self.ops.layernorm_ops.rms_norm_general(self.q_hidden, x, gamma, self.q_scale, self.cfg.eps, True)
+    def _row_views(self, M: int) -> _Rows:
+        H, W = self.cfg.hidden, self.q_size + 2 * self.kv_size
+        a, q = self.act_buffer, self.q_act
+        return _Rows(a[: M * W].view(M, W), a[: M * H].view(M, H), a[: M * 2 * self.Iloc].view(M, -1), q[: M * H].view(M, H),
+                     q[: M * self.q_size].view(M, self.q_size), q[: M * self.Iloc].view(M, self.Iloc), self.scale_buffer[:M], self.sum_buffer[:M])
 
-    def _quant(self, out_q, x):
-        """Per-token quantisation of the input of a ROW-parallel GEMM (o_proj, down_proj)."""
+    def _norm_quant(self, r: _Rows, x, gamma):
+        """Per-token quantised RMS norm of x into r.q_hidden, r.q_scale and r.q_sum."""
+        if self.act_sum:  # layernorm.py:88
+            self.ops.layernorm_ops.rms_norm_general_fuse_sum(r.q_hidden, x, gamma, r.q_sum, r.q_scale, self.cfg.eps, True)
+        else:             # layernorm.py:72
+            self.ops.layernorm_ops.rms_norm_general(r.q_hidden, x, gamma, r.q_scale, self.cfg.eps, True)
+
+    def _quant(self, r: _Rows, out_q, x):
+        """Per-token quantisation of the input of a ROW-parallel GEMM (o_proj, down_proj) into out_q, r.q_scale and r.q_sum."""
         if self.tp_size > 1 and self.tp_exact:
             # SURVEY.md 8e: same per-token scale on all ranks (global amax), local-K-shard activation sum
             _ext.row_absmax(self.q_amax, x)
             if not self.no_comm:
                 torch.distributed.all_reduce(self.q_amax, op=torch.distributed.ReduceOp.MAX, group=self.pg)
-            _ext.invoke_quant_given_amax(out_q, x, self.q_amax, self.q_sum if self.act_sum else None, self.q_scale)
+            _ext.invoke_quant_given_amax(out_q, x, self.q_amax, r.q_sum if self.act_sum else None, r.q_scale)
         elif self.act_sum:  # llama_w4a8_unpad.py:177-183
-            self.ops.fused_kernels.invoke_quant_fuse_sum(out_q, x, self.q_sum, self.q_scale)
+            self.ops.fused_kernels.invoke_quant_fuse_sum(out_q, x, r.q_sum, r.q_scale)
         else:
-            self.ops.fused_kernels.invoke_quant(out_q, x, self.q_scale)
+            self.ops.fused_kernels.invoke_quant(out_q, x, r.q_scale)
 
     def _allreduce(self, t):
         if self.tp_size > 1 and not self.no_comm:
@@ -276,24 +291,26 @@ class DecodeRunner:
         (s_logprob, s_top_ids, s_top_logprobs: the distribution before the temperature / top-k / top-p warpers) if logprobs > 0 -> the token
         is appended to s_history at s_seq_lens (index clamped to the last column) and s_seq_lens advances by one.  A caller must not run
         more than max_new_tokens such steps (eager or replayed) without resetting s_seq_lens and s_history."""
-        if not (penalties or logprobs):
-            if not sample:
-                return self._forward_fused(tokens) if self.fused else self._forward_reference(tokens)
-            logits = self._forward_fused(tokens, True) if self.fused else self._forward_reference(tokens, True)
-            return _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets)
-        assert self.max_new_tokens, "construct the runner with max_new_tokens > 0 for penalties / logprobs"
+        assert self.max_new_tokens or not (penalties or logprobs), "construct the runner with max_new_tokens > 0 for penalties / logprobs"
         logits = self._forward_fused(tokens, True) if self.fused else self._forward_reference(tokens, True)
+        return self._next_tokens(logits, sample, penalties, logprobs)
+
+    def _next_tokens(self, logits, sample: bool, penalties: bool = False, logprobs: int = 0, out: Optional[torch.Tensor] = None):
+        """logits -> the step's tokens as forward describes them, written into out if given."""
         if penalties:
             _ext.apply_penalties(logits, self.s_history, self.s_prompt_lens, self.s_seq_lens, self.s_repetition, self.s_presence, self.s_frequency)
         if sample:
-            tok = _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets)
+            tok = _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets, out=out)
+        elif self.fused or penalties or logprobs:
+            tok = _ext.argmax_rows(logits, out=out)  # one launch instead of torch's two-pass reduction
         else:
-            tok = _ext.argmax_rows(logits)
+            tok = torch.argmax(logits, dim=-1)  # the reference's greedy step
         if logprobs:
             _ext.logprobs_rows(logits, tok, int(logprobs), self.s_logprob, *self.top_logprobs_view(int(logprobs)))
-        col = self.s_seq_lens.clamp(max=self.s_history.size(1) - 1).long().unsqueeze(1)
-        self.s_history.scatter_(1, col, tok.unsqueeze(1))
-        self.s_seq_lens.add_(1)
+        if penalties or logprobs:
+            col = self.s_seq_lens.clamp(max=self.s_history.size(1) - 1).long().unsqueeze(1)
+            self.s_history.scatter_(1, col, tok.unsqueeze(1))
+            self.s_seq_lens.add_(1)
         return tok
 
     def _alloc_penalty_buffers(self) -> None:
@@ -314,108 +331,117 @@ class DecodeRunner:
         B = self.batch
         return self.s_top_ids[: B * n].view(B, n), self.s_top_logprobs[: B * n].view(B, n)
 
+    def _heads(self, qkv):
+        """q [M, Hq, D], k and v [M, Hkv, D]: views of the qkv GEMM output (:245-252)."""
+        D = self.cfg.head_dim
+        q, k, v = qkv.split([self.q_size, self.kv_size, self.kv_size], dim=-1)
+        return q.reshape(q.size(0), self.Hq, D), k.reshape(k.size(0), self.Hkv, D), v.reshape(v.size(0), self.Hkv, D)
+
     def _attention(self, li):
-        cfg, D = self.cfg, self.cfg.head_dim
-        q, k, v = self.qkv_buf.split([self.q_size, self.kv_size, self.kv_size], dim=-1)  # :245-252
-        q = q.reshape(q.size(0), self.Hq, D)
-        k = k.reshape(k.size(0), self.Hkv, D)
-        v = v.reshape(v.size(0), self.Hkv, D)
+        cfg = self.cfg
+        q, k, v = self._heads(self.qkv_buf)
         attn = self.ops.fused_attention.single_query_attention(
             q, k, v, self.block_tables[li], self.context_lens, None, min(8192, cfg.max_pos), 64, self.size_per_token,
-            self.max_seq_len, D, cfg.rope_theta, True, self.kv_bits == 4, True)  # :265-281
+            self.max_seq_len, cfg.head_dim, cfg.rope_theta, True, self.kv_bits == 4, True)  # :265-281
         return attn.reshape(q.size(0), -1)
 
-    def _attention_quant(self, li, qsum) -> None:
-        cfg, D = self.cfg, self.cfg.head_dim
-        q, k, v = self.qkv_buf.split([self.q_size, self.kv_size, self.kv_size], dim=-1)
-        q = q.reshape(q.size(0), self.Hq, D)
-        k = k.reshape(k.size(0), self.Hkv, D)
-        v = v.reshape(v.size(0), self.Hkv, D)
+    def _attention_quant(self, li, r: _Rows) -> None:
+        """The decode step's attention, quantised into r.q_attn: one launch, or with tp_exact on TP > 1 the attention and then _quant."""
+        if self.tp_size > 1 and self.tp_exact:
+            self._quant(r, r.q_attn, self._attention(li))
+            return
+        cfg = self.cfg
+        q, k, v = self._heads(r.qkv)
         _ext.single_query_attention_quant(q, k, v, self.block_tables[li], self.context_lens, min(8192, cfg.max_pos), 64, self.size_per_token,
-                                                 self.max_seq_len, D, cfg.rope_theta, self.kv_bits == 4, True, self.q_attn, self.q_scale, qsum)
+                                          self.max_seq_len, cfg.head_dim, cfg.rope_theta, self.kv_bits == 4, True, r.q_attn, r.q_scale,
+                                          r.q_sum if self.act_sum else None)
+
+    def _logits(self, hidden):
+        """Final norm (:408) and the fp16 lm_head (cuBLAS, :474-476)."""
+        out = torch.empty_like(hidden)
+        self.ops.layernorm_ops.rms_norm(out, hidden, self.norm_w, self.cfg.eps, False)
+        return torch.nn.functional.linear(out, self.lm_head)
 
     def _forward_reference(self, tokens: torch.Tensor, return_logits: bool = False) -> torch.Tensor:
         """Exactly the reference's op sequence (LlamaDecoderLayer.forward, llama_w4a8_unpad.py:330-361)."""
-        cfg = self.cfg
+        r = self.rows
         n = 0
         hidden = self.embed[tokens]  # LlamaModel.forward (:401-404)
         for li, ly in enumerate(self.layers):
             residual = hidden
-            self._norm_quant(hidden, ly["ln1"])
+            self._norm_quant(r, hidden, ly["ln1"])
             ly["qkv"](self.q_hidden, self.q_scale, self.q_sum, self.qkv_buf)
             attn = self._attention(li)
-            self._quant(self.q_attn, attn)
+            self._quant(r, self.q_attn, attn)
             ly["o"](self.q_attn, self.q_scale, self.q_sum, self.out_buf)
             self._allreduce(self.out_buf)
             hidden = residual + self.out_buf  # :348
             residual = hidden
-            self._norm_quant(hidden, ly["ln2"])
+            self._norm_quant(r, hidden, ly["ln2"])
             ly["gate_up"](self.q_hidden, self.q_scale, self.q_sum, self.gate_up_buf)
             self.ops.activation_ops.silu_and_mul(self.mlp_act, self.gate_up_buf)  # activation.py:24-29
-            self._quant(self.q_mlp, self.mlp_act)
+            self._quant(r, self.q_mlp, self.mlp_act)
             ly["down"](self.q_mlp, self.q_scale, self.q_sum, self.out_buf)
             self._allreduce(self.out_buf)
             hidden = residual + self.out_buf  # :360
             n += 10
-        out = torch.empty_like(hidden)
-        self.ops.layernorm_ops.rms_norm(out, hidden, self.norm_w, cfg.eps, False)  # final norm (:408)
-        logits = torch.nn.functional.linear(out, self.lm_head)           # fp16 lm_head (:474-476)
+        logits = self._logits(hidden)
         self.launches_per_step = n + 1
         self.last_logits = logits  # what the step computed before sampling (bench.py --dump-outputs)
         return logits if return_logits else torch.argmax(logits, dim=-1)
 
-    def _forward_fused(self, tokens: torch.Tensor, return_logits: bool = False) -> torch.Tensor:
-        """Same arithmetic, three launches fewer per layer: the two torch residual adds are folded into the following norm
-        (`add_rms_norm_general`) and silu_and_mul into the following per-token quant (`silu_and_mul_quant`)."""
+    def _fused_layers(self, hidden: torch.Tensor, r: _Rows, attention):
+        """The decoder layers over the M rows of r, from the embedded tokens hidden [M, H]: the reference's arithmetic, three launches fewer
+        per layer (the two torch residual adds are folded into the following norm, `add_rms_norm_general`, and silu_and_mul into the
+        following per-token quant, `silu_and_mul_quant`).  attention(li, r) reads r.qkv and writes r.q_attn, r.q_scale and r.q_sum.
+        Returns the final hidden state [M, H] and the number of launches."""
         cfg = self.cfg
-        qsum = self.q_sum if self.act_sum else None
-        n = 0
-        hidden = self.embed[tokens]
+        exact = self.tp_size > 1 and self.tp_exact
+        qsum = r.q_sum if self.act_sum else None
         nxt = torch.empty_like(hidden)
-        self._norm_quant(hidden, self.layers[0]["ln1"])
-        n += 1
+        self._norm_quant(r, hidden, self.layers[0]["ln1"])
+        n = 1
         for li, ly in enumerate(self.layers):
-            exact = self.tp_size > 1 and self.tp_exact
-            ly["qkv"](self.q_hidden, self.q_scale, self.q_sum, self.qkv_buf)
-            if exact or not self.fuse_attn_quant:
-                self._quant(self.q_attn, self._attention(li))
-            else:
-                self._attention_quant(li, qsum)
+            ly["qkv"](r.q_hidden, r.q_scale, r.q_sum, r.qkv)
+            attention(li, r)
             if self.tp_peer:
-                ly["o"](self.q_attn, self.q_scale, self.q_sum, self.peer.partial[0])
-                _ext.add_rms_norm_general_peer(self.q_hidden, nxt, hidden, self.peer, 0, ly["ln2"], qsum, self.q_scale, cfg.eps)
+                ly["o"](r.q_attn, r.q_scale, r.q_sum, self.peer.partial[0])
+                _ext.add_rms_norm_general_peer(r.q_hidden, nxt, hidden, self.peer, 0, ly["ln2"], qsum, r.q_scale, cfg.eps)
             else:
-                ly["o"](self.q_attn, self.q_scale, self.q_sum, self.out_buf)
-                self._allreduce(self.out_buf)
-                _ext.add_rms_norm_general(self.q_hidden, nxt, hidden, self.out_buf, ly["ln2"], qsum, self.q_scale, cfg.eps)
+                ly["o"](r.q_attn, r.q_scale, r.q_sum, r.out)
+                self._allreduce(r.out)
+                _ext.add_rms_norm_general(r.q_hidden, nxt, hidden, r.out, ly["ln2"], qsum, r.q_scale, cfg.eps)
             hidden, nxt = nxt, hidden
-            ly["gate_up"](self.q_hidden, self.q_scale, self.q_sum, self.gate_up_buf)
+            ly["gate_up"](r.q_hidden, r.q_scale, r.q_sum, r.gate_up)
             if exact:
-                activation_ops.silu_and_mul(self.mlp_act, self.gate_up_buf)
-                self._quant(self.q_mlp, self.mlp_act)
+                activation_ops.silu_and_mul(self.mlp_act, r.gate_up)
+                self._quant(r, r.q_mlp, self.mlp_act)
             else:
-                _ext.silu_and_mul_quant(self.q_mlp, self.gate_up_buf, qsum, self.q_scale)
+                _ext.silu_and_mul_quant(r.q_mlp, r.gate_up, qsum, r.q_scale)
             if self.tp_peer:
-                ly["down"](self.q_mlp, self.q_scale, self.q_sum, self.peer.partial[1])
+                ly["down"](r.q_mlp, r.q_scale, r.q_sum, self.peer.partial[1])
             else:
-                ly["down"](self.q_mlp, self.q_scale, self.q_sum, self.out_buf)
-                self._allreduce(self.out_buf)
+                ly["down"](r.q_mlp, r.q_scale, r.q_sum, r.out)
+                self._allreduce(r.out)
             n += 11 if exact else 7
             if self.tp_peer:
                 # the last layer has no following norm: the same kernel delivers hidden + sum(partials) (its quantised output is not used)
                 gam = self.layers[li + 1]["ln1"] if li + 1 < len(self.layers) else ly["ln1"]
-                _ext.add_rms_norm_general_peer(self.q_hidden, nxt, hidden, self.peer, 1, gam, qsum, self.q_scale, cfg.eps)
+                _ext.add_rms_norm_general_peer(r.q_hidden, nxt, hidden, self.peer, 1, gam, qsum, r.q_scale, cfg.eps)
                 hidden, nxt = nxt, hidden
                 n += 1
             elif li + 1 < len(self.layers):
-                _ext.add_rms_norm_general(self.q_hidden, nxt, hidden, self.out_buf, self.layers[li + 1]["ln1"], qsum, self.q_scale, cfg.eps)
+                _ext.add_rms_norm_general(r.q_hidden, nxt, hidden, r.out, self.layers[li + 1]["ln1"], qsum, r.q_scale, cfg.eps)
                 hidden, nxt = nxt, hidden
                 n += 1
             else:
-                hidden = hidden + self.out_buf
-        out = torch.empty_like(hidden)
-        layernorm_ops.rms_norm(out, hidden, self.norm_w, cfg.eps, False)
-        logits = torch.nn.functional.linear(out, self.lm_head)
+                hidden = hidden + r.out
+        return hidden, n
+
+    def _forward_fused(self, tokens: torch.Tensor, return_logits: bool = False) -> torch.Tensor:
+        """The decode step on the fused layers: the arithmetic of _forward_reference, three launches fewer per layer."""
+        hidden, n = self._fused_layers(self.embed[tokens], self.rows, self._attention_quant)
+        logits = self._logits(hidden)
         self.launches_per_step = n + 2
         self.last_logits = logits
         return logits if return_logits else _ext.argmax_rows(logits)  # one launch instead of torch's two-pass reduction
@@ -424,16 +450,8 @@ class DecodeRunner:
     # speculative-decoding verify: n draft tokens per sequence at positions ctx .. ctx + n - 1 in one step
     # ---------------------------------------------------------------------------------------------------------
     def _alloc_verify_buffers(self) -> None:
-        """Activation buffers for batch * verify_len rows, separate from the decode step's (torch.empty: no random draws)."""
-        dev, H, M = self.dev, self.cfg.hidden, self.batch * self.verify_len
-        self.v_qkv = torch.empty((M, self.q_size + 2 * self.kv_size), dtype=torch.half, device=dev)
-        self.v_out = torch.empty((M, H), dtype=torch.half, device=dev)
-        self.v_gate_up = torch.empty((M, 2 * self.Iloc), dtype=torch.half, device=dev)
-        self.v_q_hidden = torch.empty((M, H), dtype=torch.int8, device=dev)
-        self.v_q_attn = torch.empty((M, self.q_size), dtype=torch.int8, device=dev)
-        self.v_q_mlp = torch.empty((M, self.Iloc), dtype=torch.int8, device=dev)
-        self.v_q_scale = torch.empty(M, dtype=torch.half, device=dev)
-        self.v_q_sum = torch.empty(M, dtype=torch.half, device=dev)
+        """State of the verify step (torch.full / torch.zeros: no random draws)."""
+        dev = self.dev
         self.v_start = torch.full((self.batch,), self.ctx, dtype=torch.int32, device=dev)  # tokens cached before the drafts
         self.v_meta = {}  # n -> (draft lengths [B], cu_seqlens [B + 1], padding offsets [B n]), built on first use (before any capture)
         self.v_tokens_in = torch.zeros((self.batch, self.verify_len), dtype=torch.int64, device=dev)
@@ -443,7 +461,6 @@ class DecodeRunner:
         self.v_accept_len = torch.zeros(self.batch, dtype=torch.int32, device=dev)
         self.v_path = torch.zeros(self.batch * self.verify_len, dtype=torch.int32, device=dev)  # [:B n] viewed as [B, n] for n nodes
         self.v_bonus = torch.zeros(self.batch, dtype=torch.int64, device=dev)
-        self.v_graphs = {}  # (n, tree) -> CUDA graph; (n, True, "sampled", draft_probs) for the sampled tree step
         self.v_draft_probs = None  # fp32 [B * verify_len * vocab], allocated by capture_verify(..., draft_probs=True)
 
     def _verify_meta(self, n: int):
@@ -465,48 +482,23 @@ class DecodeRunner:
         assert self.verify_len, "construct the runner with verify_len > 0"
         B, n = tokens.shape
         assert B == self.batch and 1 <= n <= self.verify_len
-        cfg, D, M = self.cfg, self.cfg.head_dim, B * n
+        cfg, M = self.cfg, B * n
         lens, cu, pad = self._verify_meta(n)
         tm = None
         if tree_mask is not None:
             assert tuple(tree_mask.shape) == (B, n) and tree_mask.dtype == torch.int32
             tm = tree_mask.contiguous().view(-1)
-        qkv, out_buf, gate_up = self.v_qkv[:M], self.v_out[:M], self.v_gate_up[:M]
-        q_hidden, q_attn, q_mlp = self.v_q_hidden[:M], self.v_q_attn[:M], self.v_q_mlp[:M]
-        q_scale, q_sum = self.v_q_scale[:M], self.v_q_sum[:M]
-        qsum = q_sum if self.act_sum else None
-        hidden = self.embed[tokens.reshape(-1)]
-        nxt = torch.empty_like(hidden)
-        if self.act_sum:
-            layernorm_ops.rms_norm_general_fuse_sum(q_hidden, hidden, self.layers[0]["ln1"], q_sum, q_scale, cfg.eps, True)
-        else:
-            layernorm_ops.rms_norm_general(q_hidden, hidden, self.layers[0]["ln1"], q_scale, cfg.eps, True)
-        for li, ly in enumerate(self.layers):
-            ly["qkv"](q_hidden, q_scale, q_sum, qkv)
+
+        def attention(li, r):
             table = self.block_tables[li]
-            _ext.apply_bias_rope_update_kv_cache_at(qkv, lens, pad, self.v_start, table, self.Hq, self.Hkv, n, 64, self.size_per_token, D,
-                                                   cfg.rope_theta, min(8192, cfg.max_pos), True, self.kv_bits == 4, True, tree_mask=tm)
-            q, k, v = qkv.split([self.q_size, self.kv_size, self.kv_size], dim=-1)
-            attn = _ext.multi_token_decode_attention(q.reshape(M, self.Hq, D), k.reshape(M, self.Hkv, D), v.reshape(M, self.Hkv, D), cu, n, self.v_start,
-                                                     self.max_prefix_len, table, 64, self.size_per_token, self.kv_bits == 4, tree_mask=tm)
-            if self.act_sum:
-                fused_kernels.invoke_quant_fuse_sum(q_attn, attn.view(M, -1), q_sum, q_scale)
-            else:
-                fused_kernels.invoke_quant(q_attn, attn.view(M, -1), q_scale)
-            ly["o"](q_attn, q_scale, q_sum, out_buf)
-            _ext.add_rms_norm_general(q_hidden, nxt, hidden, out_buf, ly["ln2"], qsum, q_scale, cfg.eps)
-            hidden, nxt = nxt, hidden
-            ly["gate_up"](q_hidden, q_scale, q_sum, gate_up)
-            _ext.silu_and_mul_quant(q_mlp, gate_up, qsum, q_scale)
-            ly["down"](q_mlp, q_scale, q_sum, out_buf)
-            if li + 1 < len(self.layers):
-                _ext.add_rms_norm_general(q_hidden, nxt, hidden, out_buf, self.layers[li + 1]["ln1"], qsum, q_scale, cfg.eps)
-                hidden, nxt = nxt, hidden
-            else:
-                hidden = hidden + out_buf
-        out = torch.empty_like(hidden)
-        layernorm_ops.rms_norm(out, hidden, self.norm_w, cfg.eps, False)
-        logits = torch.nn.functional.linear(out, self.lm_head)
+            _ext.apply_bias_rope_update_kv_cache_at(r.qkv, lens, pad, self.v_start, table, self.Hq, self.Hkv, n, 64, self.size_per_token,
+                                                   cfg.head_dim, cfg.rope_theta, min(8192, cfg.max_pos), True, self.kv_bits == 4, True, tree_mask=tm)
+            attn = _ext.multi_token_decode_attention(*self._heads(r.qkv), cu, n, self.v_start, self.max_prefix_len, table, 64, self.size_per_token,
+                                                     self.kv_bits == 4, tree_mask=tm)
+            self._quant(r, r.q_attn, attn.view(M, -1))
+
+        hidden, _ = self._fused_layers(self.embed[tokens.reshape(-1)], self._row_views(M), attention)
+        logits = self._logits(hidden)
         self.last_verify_logits = logits.view(B, n, -1)
         return self.last_verify_logits if return_logits else _ext.argmax_rows(logits).view(B, n)
 
@@ -553,7 +545,7 @@ class DecodeRunner:
         self.accept_and_compact(tin, mask, tout)
 
     def _verify_key(self, n: int, tree: bool, sampled: bool, draft_probs: bool):
-        return (n, True, "sampled", bool(draft_probs)) if sampled else (n, tree)
+        return ("verify", int(n), bool(tree or sampled), bool(sampled), bool(sampled and draft_probs))
 
     def capture_verify(self, n: int, warmup: int = 2, tree: bool = False, sampled: bool = False, draft_probs: bool = False) -> None:
         """Capture the verify step for n draft tokens in a CUDA graph: v_tokens_in[:, :n] -> v_tokens_out[:, :n].  tree=True: the graph
@@ -564,21 +556,11 @@ class DecodeRunner:
         assert not sampled or tree, "sampled acceptance runs on the tree step (a chain is a tree with mask (1 << i) - 1)"
         if sampled and draft_probs and self.v_draft_probs is None:
             self.v_draft_probs = torch.zeros(self.batch * self.verify_len * self.cfg.vocab, dtype=torch.float32, device=self.dev)
-        s = torch.cuda.Stream(device=self.dev)
-        s.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(s), torch.no_grad():
-            for _ in range(warmup):
-                self._verify_graph_body(n, tree, sampled, draft_probs)
-        torch.cuda.current_stream(self.dev).wait_stream(s)
-        torch.cuda.synchronize(self.dev)
-        g = torch.cuda.CUDAGraph()
-        with torch.no_grad(), torch.cuda.graph(g):
-            self._verify_graph_body(n, tree, sampled, draft_probs)
-        self.v_graphs[self._verify_key(n, tree, sampled, draft_probs)] = g
+        self._capture(self._verify_key(n, tree, sampled, draft_probs), lambda: self._verify_graph_body(n, tree, sampled, draft_probs), warmup)
 
     def verify_step(self, n: int, tree: bool = False, sampled: bool = False, draft_probs: bool = False) -> None:
         """Replay the captured verify step for n draft tokens."""
-        self.v_graphs[self._verify_key(n, tree, sampled, draft_probs)].replay()
+        self.graphs[self._verify_key(n, tree, sampled, draft_probs)].replay()
 
     # ---------------------------------------------------------------------------------------------------------
     # generation: plain decode steps and prompt-lookup speculative steps that advance every row by what it accepted
@@ -589,14 +571,13 @@ class DecodeRunner:
         self.g_budget = torch.full((B,), self.max_new_tokens, dtype=torch.int32, device=dev)
         self.g_eos = torch.full((B,), -1, dtype=torch.int64, device=dev)
         self.g_finished = torch.zeros(B, dtype=torch.int32, device=dev)
-        # the verify step's cached length P = L - 1 (the verify buffers' v_start when there are any)
+        # the verify step's cached length P = L - 1 (the verify step's v_start when there is one)
         self.g_start = self.v_start if self.verify_len else torch.full((B,), self.ctx, dtype=torch.int32, device=dev)
         self.g_path1 = torch.zeros((B, 1), dtype=torch.int32, device=dev)  # a plain step commits the path [0] ...
         self.g_accept1 = torch.ones(B, dtype=torch.int32, device=dev)      # ... of length 1, so only its token is appended
         # drafts of the speculative step, flat so that [:B n] viewed as [B, n] is contiguous for any n
         self.g_tokens = torch.zeros(B * n, dtype=torch.int64, device=dev)
         self.g_mask = torch.zeros(B * n, dtype=torch.int32, device=dev)
-        self.g_graphs = {}  # (n, branches, ngram, sampled) -> CUDA graph
 
     def reset_generation(self, prompt: torch.Tensor) -> None:
         """Start generating after prompt int64 [batch, ctx + 1]: the ctx tokens the pages hold, then the root (the latest token, not yet
@@ -625,11 +606,7 @@ class DecodeRunner:
         common = (self.s_history, self.s_seq_lens, self.s_prompt_lens, self.g_budget, self.g_eos, self.g_finished, self.g_start, self.context_lens,
                   self.tokens_in)
         if n == 1:
-            logits = self._forward_fused(self.tokens_in, True)
-            if sampled:
-                tok = _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets, out=self.tokens_out)
-            else:
-                tok = _ext.argmax_rows(logits, out=self.tokens_out)
+            tok = self._next_tokens(self._forward_fused(self.tokens_in, True), sampled, out=self.tokens_out)
             # the path [0] of length 1 never reads the drafts: any [B, 1] tensor that is not an output will do
             _ext.spec_commit(tok.view(B, 1), self.g_path1, self.g_accept1, tok, *common)
             return
@@ -648,26 +625,16 @@ class DecodeRunner:
         _ext.spec_commit(toks, path, acc, bonus, *common)
 
     def _generate_key(self, n: int, branches: int, ngram: tuple, sampled: bool):
-        return (int(n), int(branches), tuple(int(x) for x in ngram), bool(sampled))
+        return ("generate", int(n), int(branches), tuple(int(x) for x in ngram), bool(sampled))
 
     def capture_generate(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False, warmup: int = 2) -> None:
         """Capture generate_forward(n, branches, ngram, sampled) in a CUDA graph.  The warm-up runs the step eagerly, so it advances the rows
         like a replay does: call reset_generation afterwards."""
-        s = torch.cuda.Stream(device=self.dev)
-        s.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(s), torch.no_grad():
-            for _ in range(warmup):
-                self.generate_forward(n, branches, ngram, sampled)
-        torch.cuda.current_stream(self.dev).wait_stream(s)
-        torch.cuda.synchronize(self.dev)
-        g = torch.cuda.CUDAGraph()
-        with torch.no_grad(), torch.cuda.graph(g):
-            self.generate_forward(n, branches, ngram, sampled)
-        self.g_graphs[self._generate_key(n, branches, ngram, sampled)] = g
+        self._capture(self._generate_key(n, branches, ngram, sampled), lambda: self.generate_forward(n, branches, ngram, sampled), warmup)
 
     def generate_step(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False) -> None:
         """Replay the captured generation step."""
-        self.g_graphs[self._generate_key(n, branches, ngram, sampled)].replay()
+        self.graphs[self._generate_key(n, branches, ngram, sampled)].replay()
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
@@ -738,28 +705,34 @@ class DecodeRunner:
         self.context_lens.copy_(full.context_lens)
 
     # ---------------------------------------------------------------------------------------------------------
-    def capture(self, warmup: int = 2, sample: bool = False, penalties: bool = False, logprobs: int = 0) -> None:
-        """Warm up eagerly (allocates workspaces, sets kernel attributes) and capture the whole step in a CUDA graph.  sample=True: the step
-        ends in sample_rows (see forward); each warm-up call and each replay advances s_offsets by one.  penalties / logprobs: see forward;
-        each warm-up call and each replay appends one token to s_history.  The graph is kept in graphs[(sample, penalties, logprobs)] and
-        becomes self.graph."""
+    def _capture(self, key: tuple, body, warmup: int) -> torch.cuda.CUDAGraph:
+        """Run body() `warmup` times eagerly on a side stream (allocates workspaces, sets kernel attributes), then capture it in a CUDA
+        graph kept in graphs[key]."""
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(s), torch.no_grad():
             for _ in range(warmup):
-                self.tokens_out.copy_(self.forward(self.tokens_in, sample, penalties, logprobs))
+                body()
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         g = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(g):
-            self.tokens_out.copy_(self.forward(self.tokens_in, sample, penalties, logprobs))
-        self.graph = g
-        self.graphs[(bool(sample), bool(penalties), int(logprobs))] = g
+            body()
+        self.graphs[key] = g
+        return g
+
+    def capture(self, warmup: int = 2, sample: bool = False, penalties: bool = False, logprobs: int = 0) -> None:
+        """Warm up eagerly (allocates workspaces, sets kernel attributes) and capture the whole step in a CUDA graph.  sample=True: the step
+        ends in sample_rows (see forward); each warm-up call and each replay advances s_offsets by one.  penalties / logprobs: see forward;
+        each warm-up call and each replay appends one token to s_history.  The graph is kept under the key (sample, penalties, logprobs) of
+        step and becomes self.graph."""
+        self.graph = self._capture(("decode", bool(sample), bool(penalties), int(logprobs)),
+                                   lambda: self.tokens_out.copy_(self.forward(self.tokens_in, sample, penalties, logprobs)), warmup)
 
     def step(self, key: Optional[tuple] = None) -> None:
         """Replay the captured step: tokens_in -> tokens_out (both device resident).  key = (sample, penalties, logprobs) selects one of
-        graphs; None replays the latest capture."""
-        (self.graph if key is None else self.graphs[key]).replay()
+        the captures; None replays the latest."""
+        (self.graph if key is None else self.graphs[("decode", *key)]).replay()
 
     def weight_bytes_per_step(self) -> int:
         return sum(l.weight_bytes() for ly in self.layers for l in (ly["qkv"], ly["o"], ly["gate_up"], ly["down"]))

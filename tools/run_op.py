@@ -43,9 +43,9 @@ def call(i):
         fa.single_query_attention(q, k, v, run.block_tables[i % run.L], run.context_lens, None, 8192, 64, run.size_per_token, run.max_seq_len, D,
                                   run.cfg.rope_theta, True, run.kv_bits == 4, True)
     elif a.op == "norm":
-        run._norm_quant(hidden, ly["ln1"])
+        run._norm_quant(run.rows, hidden, ly["ln1"])
     elif a.op == "quant":
-        run._quant(run.q_mlp, run.mlp_act)
+        run._quant(run.rows, run.q_mlp, run.mlp_act)
     elif a.op == "silu":
         from qserve_backend import activation_ops
         activation_ops.silu_and_mul(run.mlp_act, run.gate_up_buf)
