@@ -43,33 +43,63 @@ def _cuda(t: torch.Tensor, name: str) -> None:
     _require(t.is_cuda, f"{name} must be on CUDA")  # CHECK_DEVICE, fused_attention.cpp:22
 
 
+def _tensor(t: torch.Tensor, name: str, dtype: torch.dtype, shape: Optional[tuple] = None, device: Optional[torch.device] = None) -> torch.Tensor:
+    """Require t to be a contiguous CUDA tensor of dtype, of exactly `shape` if given (a None entry leaves that dimension free) and on
+    `device` if given; returns t."""
+    _cuda(t, name)
+    if t.dtype != dtype or not t.is_contiguous():
+        raise RuntimeError(f"{name} must be a contiguous {dtype} tensor, got {t.dtype}")
+    if shape is not None and (t.dim() != len(shape) or any(s is not None and s != d for s, d in zip(shape, t.shape))):
+        raise RuntimeError(f"{name} must have shape {tuple('*' if s is None else s for s in shape)}, got {tuple(t.shape)}")
+    if device is not None and t.device != device:
+        raise RuntimeError(f"{name} is on {t.device}, the other tensors on {device}")
+    return t
+
+
+def _out(t: Optional[torch.Tensor], name: str, dtype: torch.dtype, shape: tuple, device: torch.device) -> torch.Tensor:
+    """An output: a new tensor if t is None, else t checked by _tensor (written in place, e.g. inside a CUDA graph capture)."""
+    return torch.empty(shape, dtype=dtype, device=device) if t is None else _tensor(t, name, dtype, shape, device)
+
+
+def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
+    """The device address of an optional tensor argument (None: NULL)."""
+    return None if t is None else t.data_ptr()
+
+
+def _half_scalar(x) -> float:
+    """A scalar scale rounded to fp16, as the reference's at::Half overloads receive it."""
+    return float(torch.tensor(float(x), dtype=_HALF))
+
+
 _workspaces: dict = {}
-_retired: list = []  # outgrown workspaces, kept alive for graphs captured with them
+# A workspace that was handed out is never freed: a captured CUDA graph may still hold its address, and the self-cleaning counters inside
+# must not alias reused memory on replay.  Outgrown workspaces are kept alive here.
+_retired: list = []
 
 
-def gemm_workspace(device: torch.device) -> torch.Tensor:
-    """Zero-initialised once per device; afterwards owned by the library (self-cleaning split-K counters)."""
-    key = ("gemm", device.index)
+def _workspace(kind: str, device: torch.device, nbytes: int) -> torch.Tensor:
+    """The zero-initialised workspace `kind` of `device`, replaced by a larger one when it holds fewer than nbytes bytes; once handed out
+    it is owned by the library (self-cleaning counters)."""
+    key = (kind, device.index)
     ws = _workspaces.get(key)
-    if ws is None:
-        ws = torch.zeros(lib.qs_gemm_workspace_bytes(), dtype=torch.uint8, device=device)
-        _workspaces[key] = ws
-    return ws
-
-
-def attention_workspace(device: torch.device, batch: int, num_heads: int, head_dim: int) -> torch.Tensor:
-    key = ("attn", device.index)
-    need = lib.qs_attention_workspace_bytes(batch, num_heads, head_dim)
-    ws = _workspaces.get(key)
-    if ws is None or ws.numel() < need:
-        # a workspace that was handed out is never freed: a captured CUDA graph may still hold its address (the self-cleaning
-        # counters inside must not alias reused memory on replay)
+    if ws is None or ws.numel() < nbytes:
         if ws is not None:
             _retired.append(ws)
         with torch.cuda.device(device):
-            ws = torch.zeros(need, dtype=torch.uint8, device=device)
+            ws = torch.zeros(nbytes, dtype=torch.uint8, device=device)
         _workspaces[key] = ws
     return ws
+
+
+_GEMM_WORKSPACE_BYTES = lib.qs_gemm_workspace_bytes()
+
+
+def gemm_workspace(device: torch.device) -> torch.Tensor:
+    return _workspace("gemm", device, _GEMM_WORKSPACE_BYTES)
+
+
+def attention_workspace(device: torch.device, batch: int, num_heads: int, head_dim: int) -> torch.Tensor:
+    return _workspace("attn", device, lib.qs_attention_workspace_bytes(batch, num_heads, head_dim))
 
 
 def set_pdl(enabled: bool) -> bool:
@@ -83,10 +113,7 @@ def set_pdl(enabled: bool) -> bool:
 
 
 def _gemm_common(in_feats, kernel, out_feats, k_div: int):
-    _cuda(in_feats, "in_feats"); _cuda(kernel, "kernel"); _cuda(out_feats, "out_feats")
-    _require(in_feats.dtype == torch.int8 and kernel.dtype == torch.int8, "in_feats and kernel must be int8")
-    _require(out_feats.dtype == _HALF, "out_feats must be float16")
-    _require(in_feats.is_contiguous() and kernel.is_contiguous() and out_feats.is_contiguous(), "GEMM operands must be contiguous")
+    _tensor(in_feats, "in_feats", torch.int8); _tensor(kernel, "kernel", torch.int8); _tensor(out_feats, "out_feats", _HALF)
     M, K = in_feats.size(0), in_feats.size(1)  # gemm_cuda.cu:604-605
     N = out_feats.size(-1)                     # gemm_cuda.cu:613
     _require(out_feats.size(-2) == M, "out_feats rows must match in_feats rows")
@@ -104,8 +131,7 @@ def w4a8_per_chn_gemm_forward_cuda(in_feats, kernel, wscales, ascales, w_szs, a_
         return
     ws = gemm_workspace(in_feats.device)
     _call(in_feats, lib.qs_w4a8_gemm_per_chn, in_feats.data_ptr(), kernel.data_ptr(), wscales.data_ptr(), ascales.data_ptr(), w_szs.data_ptr(),
-                                   a_ssums.data_ptr(), out_feats.data_ptr(), _acc_out.data_ptr() if _acc_out is not None else None,
-                                   M, N, K, ws.data_ptr(), ws.numel())
+                                   a_ssums.data_ptr(), out_feats.data_ptr(), _ptr(_acc_out), M, N, K, ws.data_ptr(), ws.numel())
 
 
 def w4a8_per_group_gemm_forward_cuda(in_feats, kernel, zeros, scales_i8, wscales, ascales, out_feats, _acc_out=None) -> None:
@@ -120,8 +146,7 @@ def w4a8_per_group_gemm_forward_cuda(in_feats, kernel, zeros, scales_i8, wscales
         return
     ws = gemm_workspace(in_feats.device)
     _call(in_feats, lib.qs_w4a8_gemm_per_group, in_feats.data_ptr(), kernel.data_ptr(), zeros.data_ptr(), scales_i8.data_ptr(), wscales.data_ptr(),
-                                     ascales.data_ptr(), out_feats.data_ptr(), _acc_out.data_ptr() if _acc_out is not None else None,
-                                     M, N, K, ws.data_ptr(), ws.numel())
+                                     ascales.data_ptr(), out_feats.data_ptr(), _ptr(_acc_out), M, N, K, ws.data_ptr(), ws.numel())
 
 
 def w8a8_gemm_forward_cuda(in_feats, kernel, wscales, ascales, out_feats, _acc_out=None) -> None:
@@ -132,7 +157,7 @@ def w8a8_gemm_forward_cuda(in_feats, kernel, wscales, ascales, out_feats, _acc_o
         return
     ws = gemm_workspace(in_feats.device)
     _call(in_feats, lib.qs_w8a8_gemm, in_feats.data_ptr(), kernel.data_ptr(), wscales.data_ptr(), ascales.data_ptr(), out_feats.data_ptr(),
-                           _acc_out.data_ptr() if _acc_out is not None else None, M, N, K, ws.data_ptr(), ws.numel())
+                           _ptr(_acc_out), M, N, K, ws.data_ptr(), ws.numel())
 
 
 # --------------------------------------------------------------------------------------------------
@@ -148,32 +173,27 @@ def single_query_attention(q, k, v, kv_pointers, length_per_sample_: Optional[to
 
     Returns a NEW tensor shaped like q (the reference returns torch::empty_like(q), :205).  Mutates the KV pages.
     """
-    for t, n in ((q, "q"), (k, "k"), (v, "v"), (kv_pointers, "kv_pointers")):
+    for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _cuda(t, n)
+    _tensor(kv_pointers, "kv_pointers", torch.int64)  # :182
     _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "single_query_attention: only float16 is supported (fused_attention.cpp:24-30)")
     batch = kv_pointers.size(0)
     nheads, nheads_kv, headdim = q.size(1), k.size(1), k.size(-1)
     _require(k.stride(2) == 1 and k.stride(1) == headdim, "k must have stride(2) == 1 and stride(1) == head_dim")  # :179
     _require(v.stride(2) == 1 and v.stride(1) == headdim, "v must have stride(2) == 1 and stride(1) == head_dim")  # :180
     _require(q.stride(2) == 1 and q.stride(1) == headdim, "q must have stride(2) == 1 and stride(1) == head_dim")
-    _require(kv_pointers.is_contiguous() and kv_pointers.dtype == torch.int64, "kv_pointers must be contiguous int64")  # :182
-    lens_ptr = None
     if length_per_sample_ is not None:
-        _cuda(length_per_sample_, "length_per_sample")
-        _require(tuple(length_per_sample_.shape) == (batch,), "length_per_sample must have shape (batch_size)")
-        _require(length_per_sample_.is_contiguous(), "length_per_sample must be contiguous")
-        _require(length_per_sample_.dtype == torch.int32, "length_per_sample must be int32")  # :189
-        lens_ptr = length_per_sample_.data_ptr()
+        _tensor(length_per_sample_, "length_per_sample", torch.int32, (batch,))  # :184-189
     if alibi_slopes_ is not None:  # accepted, validated and ignored, exactly like the reference (:192-199, :91)
         _cuda(alibi_slopes_, "alibi_slopes")
         _require(tuple(alibi_slopes_.shape) == (nheads,) and alibi_slopes_.dtype == torch.float32, "alibi_slopes must be float32 [nheads]")
     out = torch.empty((q.size(0), nheads, headdim), dtype=q.dtype, device=q.device)
     ws = attention_workspace(q.device, batch, nheads, headdim)
     _call(q, lib.qs_single_query_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), kv_pointers.data_ptr(),
-                                        lens_ptr, out.data_ptr(), batch, nheads, nheads_kv, headdim, kv_pointers.size(-1), int(memory_max_seqlen),
-                                        int(tokens_per_block), int(size_per_token), int(timestep), int(rotary_embedding_dim), float(rotary_base),
-                                        int(bool(neox_rotary_style)), int(bool(int4_kv_cache)), int(bool(kv_cache_with_zeros)), ws.data_ptr(),
-                                        ws.numel())
+                                        _ptr(length_per_sample_), out.data_ptr(), batch, nheads, nheads_kv, headdim, kv_pointers.size(-1),
+                                        int(memory_max_seqlen), int(tokens_per_block), int(size_per_token), int(timestep), int(rotary_embedding_dim),
+                                        float(rotary_base), int(bool(neox_rotary_style)), int(bool(int4_kv_cache)), int(bool(kv_cache_with_zeros)),
+                                        ws.data_ptr(), ws.numel())
     return out
 
 
@@ -183,8 +203,7 @@ def apply_bias_rope_update_kv_cache(qkv, seq_lens, padding_offset, kv_pointers: 
                                     int4_kv_cache: bool, kv_cache_with_zeros: bool) -> None:
     """qserve_backend.fused_attention.apply_bias_rope_update_kv_cache (update_kv_cache.cu:20-108): in-place RoPE on the
     packed qkv [T,(Hq+2Hkv)*D] and per-token-per-head asymmetric quantisation of K/V into the pages."""
-    _cuda(qkv, "qkv")
-    _require(qkv.dtype == _HALF and qkv.is_contiguous(), "qkv must be contiguous float16")
+    _tensor(qkv, "qkv", _HALF)
     _require(seq_lens.dtype == torch.int32 and padding_offset.dtype == torch.int32, "seq_lens and padding_offset must be int32")
     head_dim = int(rotary_embedding_dim)  # size_per_head = rotary_embedding_dim (update_kv_cache.cu:54)
     _require(qkv.size(-1) == (head_num + 2 * kv_head_num) * head_dim, "qkv width does not match (head_num + 2*kv_head_num) * head_dim")
@@ -208,6 +227,16 @@ def compute_padding_offsets(cu_seqlens, max_seqlen: int, tot_num_tokens: int) ->
     return out
 
 
+def _qkv_heads(q, k, v):
+    """The layout of the prompt attentions' q [T,Hq,128] and k / v [T,Hkv,128]: fp16, heads as contiguous rows of 128 halfs (strided views of
+    the qkv buffer are fine), one token count.  Returns (T, Hq, Hkv).  The device checks are the caller's."""
+    for t, name in ((q, "q"), (k, "k"), (v, "v")):
+        _require(t.dtype == _HALF and t.dim() == 3 and t.size(2) == 128, f"{name} must be float16 [T, H, 128]")
+        _require(t.stride(2) == 1 and t.stride(1) == 128, f"{name}: heads must be contiguous rows of 128 halfs")
+    _require(k.shape == v.shape and q.size(0) == k.size(0), "q, k, v must cover the same tokens; k and v the same heads")
+    return q.size(0), q.size(1), k.size(1)
+
+
 def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q: int, max_seqlen_k: int, dropout_p: float = 0.0,
                            softmax_scale: Optional[float] = None, causal: bool = False, **unsupported) -> torch.Tensor:
     """Drop-in for the ONE way the reference calls flash_attn.flash_attn_varlen_func (llama_w4a8_unpad.py:232-242): causal self-attention over a
@@ -216,16 +245,11 @@ def flash_attn_varlen_func(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q: in
     _cuda(q, "q")
     _require(not unsupported or all(val in (None, False, 0, 0.0, (-1, -1)) for val in unsupported.values()), f"unsupported arguments {sorted(unsupported)}")
     _require(causal and float(dropout_p) == 0.0, "only causal=True, dropout_p=0.0 is implemented")
-    _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
-    _require(q.dim() == 3 and k.dim() == 3 and v.dim() == 3 and q.size(2) == 128 and k.size(2) == 128 and v.size(2) == 128, "q, k, v must be [T, H, 128]")
-    _require(k.shape == v.shape and q.size(0) == k.size(0), "q, k, v must cover the same tokens; k and v the same heads")
+    T, hq, hkv = _qkv_heads(q, k, v)
     _require(cu_seqlens_q.dtype == torch.int32 and cu_seqlens_q.is_contiguous(), "cu_seqlens must be contiguous int32")
     _require(cu_seqlens_k is cu_seqlens_q or (cu_seqlens_k.shape == cu_seqlens_q.shape and cu_seqlens_k.data_ptr() == cu_seqlens_q.data_ptr())
              or bool(torch.equal(cu_seqlens_k, cu_seqlens_q)), "queries and keys must share cu_seqlens (prompt self-attention)")
     _require(int(max_seqlen_q) == int(max_seqlen_k), "max_seqlen_q and max_seqlen_k must agree")
-    for t, name in ((q, "q"), (k, "k"), (v, "v")):
-        _require(t.stride(2) == 1 and t.stride(1) == 128, f"{name}: heads must be contiguous rows of 128 halfs")
-    T, hq, hkv = q.size(0), q.size(1), k.size(1)
     out = torch.empty((T, hq, 128), dtype=_HALF, device=q.device)
     if T == 0:
         return out
@@ -293,9 +317,8 @@ def invoke_dequant_add_residual_rms_norm_quant(out, input, residual, gamma, scal
         _call(input, lib.qs_dequant_add_residual_rms_norm_quant, out.data_ptr(), input.data_ptr(), residual.data_ptr(), gamma.data_ptr(), scale.data_ptr(), 0.0,
                                                          float(epsilon), tokens, hidden)
     else:
-        s = float(torch.tensor(float(scale), dtype=_HALF))  # at::Half argument
-        _call(input, lib.qs_dequant_add_residual_rms_norm_quant, out.data_ptr(), input.data_ptr(), residual.data_ptr(), gamma.data_ptr(), None, s,
-                                                         float(epsilon), tokens, hidden)
+        _call(input, lib.qs_dequant_add_residual_rms_norm_quant, out.data_ptr(), input.data_ptr(), residual.data_ptr(), gamma.data_ptr(), None,
+                                                         _half_scalar(scale), float(epsilon), tokens, hidden)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -313,8 +336,7 @@ def invoke_quant(out, input, scale) -> None:
     if isinstance(scale, torch.Tensor):
         _call(input, lib.qs_invoke_quant, out.data_ptr(), input.data_ptr(), scale.data_ptr(), tokens, hidden)
     else:
-        s = float(torch.tensor(float(scale), dtype=_HALF))
-        _call(input, lib.qs_invoke_quant_scalar, out.data_ptr(), input.data_ptr(), s, tokens, hidden)
+        _call(input, lib.qs_invoke_quant_scalar, out.data_ptr(), input.data_ptr(), _half_scalar(scale), tokens, hidden)
 
 
 def invoke_quant_fuse_sum(out, input, input_sum, scale) -> None:
@@ -327,8 +349,7 @@ def invoke_quant_fuse_sum(out, input, input_sum, scale) -> None:
     if isinstance(scale, torch.Tensor):
         _call(input, lib.qs_invoke_quant_fuse_sum, out.data_ptr(), input.data_ptr(), input_sum.data_ptr(), scale.data_ptr(), tokens, hidden)
     else:  # scalar overload: static scale, the sum argument is unused by the reference kernel (fused_kernels.cu:131-136)
-        s = float(torch.tensor(float(scale), dtype=_HALF))
-        _call(input, lib.qs_invoke_quant_scalar, out.data_ptr(), input.data_ptr(), s, tokens, hidden)
+        _call(input, lib.qs_invoke_quant_scalar, out.data_ptr(), input.data_ptr(), _half_scalar(scale), tokens, hidden)
 
 
 def invoke_dequant_add_residual(out, input, residual, scale) -> None:
@@ -340,8 +361,7 @@ def invoke_dequant_add_residual(out, input, residual, scale) -> None:
     if isinstance(scale, torch.Tensor):
         _call(input, lib.qs_invoke_dequant_add_residual, out.data_ptr(), input.data_ptr(), residual.data_ptr(), scale.data_ptr(), 0.0, tokens, hidden)
     else:
-        s = float(torch.tensor(float(scale), dtype=_HALF))
-        _call(input, lib.qs_invoke_dequant_add_residual, out.data_ptr(), input.data_ptr(), residual.data_ptr(), None, s, tokens, hidden)
+        _call(input, lib.qs_invoke_dequant_add_residual, out.data_ptr(), input.data_ptr(), residual.data_ptr(), None, _half_scalar(scale), tokens, hidden)
 
 
 def invoke_dequant(out, input, scale) -> None:
@@ -350,8 +370,7 @@ def invoke_dequant(out, input, scale) -> None:
     if _noop(input):
         return
     tokens, hidden = _rows(input)
-    s = float(torch.tensor(float(scale), dtype=_HALF))
-    _call(input, lib.qs_invoke_dequant, out.data_ptr(), input.data_ptr(), s, tokens, hidden, input.stride(-2), out.stride(-2))
+    _call(input, lib.qs_invoke_dequant, out.data_ptr(), input.data_ptr(), _half_scalar(scale), tokens, hidden, input.stride(-2), out.stride(-2))
 
 
 # --------------------------------------------------------------------------------------------------
@@ -409,7 +428,7 @@ def add_rms_norm_general(out, hidden_out, x, delta, weight, input_sum: Optional[
         return
     tokens, hidden = _rows(x)
     _call(x, lib.qs_add_rms_norm_general, out.data_ptr(), hidden_out.data_ptr(), x.data_ptr(), delta.data_ptr(), weight.data_ptr(),
-                                      input_sum.data_ptr() if input_sum is not None else None, scaling.data_ptr(), float(epsilon), tokens, hidden)
+                                      _ptr(input_sum), scaling.data_ptr(), float(epsilon), tokens, hidden)
 
 
 def silu_and_mul_quant(out, input, input_sum: Optional[torch.Tensor], scale) -> None:
@@ -419,8 +438,7 @@ def silu_and_mul_quant(out, input, input_sum: Optional[torch.Tensor], scale) -> 
         return
     d = input.size(-1) // 2
     tokens = input.numel() // input.size(-1)
-    _call(input, lib.qs_silu_and_mul_quant, out.data_ptr(), input.data_ptr(), input_sum.data_ptr() if input_sum is not None else None, scale.data_ptr(),
-                                    tokens, d)
+    _call(input, lib.qs_silu_and_mul_quant, out.data_ptr(), input.data_ptr(), _ptr(input_sum), scale.data_ptr(), tokens, d)
 
 
 def single_query_attention_quant(q, k, v, kv_pointers, length_per_sample, memory_max_seqlen: int, tokens_per_block: int, size_per_token: int,
@@ -428,20 +446,28 @@ def single_query_attention_quant(q, k, v, kv_pointers, length_per_sample, memory
                                  out_q, out_scale, out_sum: Optional[torch.Tensor]) -> None:
     """single_query_attention + invoke_quant[_fuse_sum] in one launch: out_q int8 [B, Hq*D], out_scale / out_sum fp16 [B].
     Bit-identical to the two reference ops run back to back (llama_w4a8_unpad.py:265-283)."""
+    for t, n in ((q, "q"), (k, "k"), (v, "v")):
+        _cuda(t, n)
+    dev = q.device
+    _tensor(kv_pointers, "kv_pointers", torch.int64, device=dev)
     batch = kv_pointers.size(0)
     if batch == 0:
         return
     nheads, nheads_kv, headdim = q.size(1), k.size(1), k.size(-1)
-    _require(q.dtype == _HALF and q.stride(2) == 1 and q.stride(1) == headdim, "q must be float16 with stride(1) == head_dim")
-    _require(k.stride(1) == headdim and v.stride(1) == headdim and kv_pointers.is_contiguous(), "k, v, kv_pointers layout")
-    _require(out_q.dtype == torch.int8 and out_q.is_contiguous() and out_q.numel() == batch * nheads * headdim, "out_q must be int8 [B, Hq*D]")
-    ws = attention_workspace(q.device, batch, nheads, headdim)
+    _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
+    _require(q.stride(2) == 1 and q.stride(1) == headdim and k.stride(1) == headdim and v.stride(1) == headdim, "q, k, v: stride(1) must be head_dim")
+    _tensor(length_per_sample, "length_per_sample", torch.int32, (batch,), dev)
+    _tensor(out_q, "out_q", torch.int8, device=dev)
+    _require(out_q.numel() == batch * nheads * headdim, "out_q must be int8 [B, Hq*D]")
+    _tensor(out_scale, "out_scale", _HALF, (batch,), dev)
+    if out_sum is not None:
+        _tensor(out_sum, "out_sum", _HALF, (batch,), dev)
+    ws = attention_workspace(dev, batch, nheads, headdim)
     _call(q, lib.qs_single_query_attention_quant, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), kv_pointers.data_ptr(),
-                                              length_per_sample.data_ptr(), out_q.data_ptr(), out_scale.data_ptr(),
-                                              out_sum.data_ptr() if out_sum is not None else None, batch, nheads, nheads_kv, headdim,
-                                              kv_pointers.size(-1), int(memory_max_seqlen), int(tokens_per_block), int(size_per_token), int(timestep),
-                                              int(rotary_embedding_dim), float(rotary_base), int(bool(int4_kv_cache)), int(bool(kv_cache_with_zeros)),
-                                              ws.data_ptr(), ws.numel())
+                                              length_per_sample.data_ptr(), out_q.data_ptr(), out_scale.data_ptr(), _ptr(out_sum), batch, nheads,
+                                              nheads_kv, headdim, kv_pointers.size(-1), int(memory_max_seqlen), int(tokens_per_block), int(size_per_token),
+                                              int(timestep), int(rotary_embedding_dim), float(rotary_base), int(bool(int4_kv_cache)),
+                                              int(bool(kv_cache_with_zeros)), ws.data_ptr(), ws.numel())
 
 
 def apply_bias_rope_update_kv_cache_at(qkv, seq_lens, padding_offset, start_pos, kv_pointers: Optional[torch.Tensor], head_num: int,
@@ -454,32 +480,46 @@ def apply_bias_rope_update_kv_cache_at(qkv, seq_lens, padding_offset, start_pos,
 
     tree_mask (int32 [T], one ancestor word per row, see tree_decode_attention in multi_token_decode_attention): the rows are draft-tree
     nodes (seq_len <= 16); node i is rotated at position start_pos[b] + depth(i) and stored in slot start_pos[b] + i.  None: the call above."""
-    for t, n in ((qkv, "qkv"), (seq_lens, "seq_lens"), (padding_offset, "padding_offset"), (start_pos, "start_pos")):
+    _tensor(qkv, "qkv", _HALF)
+    for t, n in ((seq_lens, "seq_lens"), (padding_offset, "padding_offset")):
         _cuda(t, n)
-    _require(qkv.dtype == _HALF and qkv.is_contiguous(), "qkv must be contiguous float16")
-    _require(seq_lens.dtype == torch.int32 and padding_offset.dtype == torch.int32, "seq_lens and padding_offset must be int32")
-    _require(start_pos.dtype == torch.int32 and start_pos.is_contiguous() and tuple(start_pos.shape) == (seq_lens.size(0),),
-             "start_pos must be contiguous int32 [batch]")
+        _require(t.dtype == torch.int32, f"{n} must be int32")
+    _tensor(start_pos, "start_pos", torch.int32, (seq_lens.size(0),))
     head_dim = int(rotary_embedding_dim)
     _require(head_dim == 128, "apply_bias_rope_update_kv_cache_at: head_dim must be 128")
     _require(qkv.size(-1) == (head_num + 2 * kv_head_num) * head_dim, "qkv width does not match (head_num + 2*kv_head_num) * head_dim")
-    kvp, max_blocks = None, 0
     if kv_pointers is not None:
-        _cuda(kv_pointers, "kv_pointers")
-        _require(kv_pointers.is_contiguous() and kv_pointers.dtype == torch.int64, "kv_pointers must be contiguous int64")
-        kvp, max_blocks = kv_pointers.data_ptr(), kv_pointers.size(-1)
+        _tensor(kv_pointers, "kv_pointers", torch.int64)
+    fn, mask = lib.qs_apply_bias_rope_update_kv_cache_at, ()
     if tree_mask is not None:
-        _tree_mask_check(tree_mask, qkv.size(0), qkv.device)
+        _tensor(tree_mask, "tree_mask", torch.int32, device=qkv.device)
+        _require(tree_mask.numel() == qkv.size(0), "tree_mask must hold one word per draft row")
         _require(1 <= int(seq_len) <= 16, "apply_bias_rope_update_kv_cache_at: a draft tree has at most 16 nodes per sequence (seq_len)")
-        _call(qkv, lib.qs_apply_bias_rope_update_kv_cache_tree, qkv.data_ptr(), seq_lens.data_ptr(), padding_offset.data_ptr(), start_pos.data_ptr(),
-              tree_mask.data_ptr(), kvp, seq_lens.size(0), qkv.size(0), max_blocks, int(head_num), int(kv_head_num), head_dim, int(seq_len),
-              int(tokens_per_block), int(size_per_token), int(rotary_embedding_dim), float(rotary_embedding_base), int(rotary_embedding_max_positions),
-              int(bool(neox_rotary_style)), int(bool(int4_kv_cache)), int(bool(kv_cache_with_zeros)))
-        return
-    _call(qkv, lib.qs_apply_bias_rope_update_kv_cache_at, qkv.data_ptr(), seq_lens.data_ptr(), padding_offset.data_ptr(), start_pos.data_ptr(), kvp,
-          seq_lens.size(0), qkv.size(0), max_blocks, int(head_num), int(kv_head_num), head_dim, int(seq_len), int(tokens_per_block),
+        fn, mask = lib.qs_apply_bias_rope_update_kv_cache_tree, (tree_mask.data_ptr(),)
+    _call(qkv, fn, qkv.data_ptr(), seq_lens.data_ptr(), padding_offset.data_ptr(), start_pos.data_ptr(), *mask, _ptr(kv_pointers), seq_lens.size(0),
+          qkv.size(0), 0 if kv_pointers is None else kv_pointers.size(-1), int(head_num), int(kv_head_num), head_dim, int(seq_len), int(tokens_per_block),
           int(size_per_token), int(rotary_embedding_dim), float(rotary_embedding_base), int(rotary_embedding_max_positions),
           int(bool(neox_rotary_style)), int(bool(int4_kv_cache)), int(bool(kv_cache_with_zeros)))
+
+
+def _paged_prompt(q, k, v, cu_seqlens, max_seqlen, prefix_lens, max_prefix_len, kv_pointers, tokens_per_block, size_per_token, int4_kv_cache):
+    """The checks prefix_prefill_attention and multi_token_decode_attention share: q / k / v as _qkv_heads, every tensor on q's CUDA device,
+    cu_seqlens int32 [B+1], prefix_lens int32 [B], kv_pointers int64 [B, 2, max_blocks] of 64-token pages covering max_prefix_len + max_seqlen
+    tokens, and size_per_token of the KV heads and the cache type.  Returns (B, T, Hq, Hkv).  The callers bound max_seqlen."""
+    _cuda(q, "q")
+    dev = q.device
+    for t, n in ((k, "k"), (v, "v")):
+        _require(t.device == dev, f"{n} is on {t.device}, q on {dev}")
+    T, hq, hkv = _qkv_heads(q, k, v)
+    batch = _tensor(cu_seqlens, "cu_seqlens", torch.int32, (None,), dev).size(0) - 1
+    _tensor(prefix_lens, "prefix_lens", torch.int32, (batch,), dev)
+    _tensor(kv_pointers, "kv_pointers", torch.int64, (batch, 2, None), dev)
+    _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
+    _require(hq % hkv == 0, "num_heads must be a multiple of num_kv_heads")
+    _require(int(size_per_token) == hkv * 128 * (4 if int4_kv_cache else 8) // 8, "size_per_token does not match the kv heads and the cache type")
+    _require(int(max_prefix_len) >= 0, "negative max_prefix_len")
+    _require(int(max_prefix_len) + int(max_seqlen) <= kv_pointers.size(-1) * 64, "the page table is too short for max_prefix_len + max_seqlen")
+    return batch, T, hq, hkv
 
 
 def prefix_prefill_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, max_prefix_len: int, kv_pointers, tokens_per_block: int,
@@ -490,24 +530,9 @@ def prefix_prefill_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, 
     prefix keys dequantised from the ZINT4 / ZINT8 pages and to chunk keys 0..i in fp16.  max_prefix_len bounds prefix_lens (it is not checked
     on the device).  Returns fp16 [T,Hq,128].  Every chunk key is used un-quantised: this is prompt attention, not n decode steps (for those,
     e.g. speculative-decoding verification, use multi_token_decode_attention, which reads the earlier chunk tokens back from the pages)."""
-    for t, n in ((q, "q"), (k, "k"), (v, "v"), (cu_seqlens, "cu_seqlens"), (prefix_lens, "prefix_lens"), (kv_pointers, "kv_pointers")):
-        _cuda(t, n)
-    _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
-    _require(q.dim() == 3 and k.dim() == 3 and v.dim() == 3 and q.size(2) == 128 and k.size(2) == 128 and v.size(2) == 128, "q, k, v must be [T, H, 128]")
-    _require(k.shape == v.shape and q.size(0) == k.size(0), "q, k, v must cover the same tokens; k and v the same heads")
-    for t, name in ((q, "q"), (k, "k"), (v, "v")):
-        _require(t.stride(2) == 1 and t.stride(1) == 128, f"{name}: heads must be contiguous rows of 128 halfs")
-    _require(cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous() and cu_seqlens.dim() == 1, "cu_seqlens must be contiguous int32")
-    batch = cu_seqlens.size(0) - 1
-    _require(prefix_lens.dtype == torch.int32 and prefix_lens.is_contiguous() and tuple(prefix_lens.shape) == (batch,), "prefix_lens must be contiguous int32 [batch]")
-    _require(kv_pointers.dtype == torch.int64 and kv_pointers.is_contiguous() and kv_pointers.dim() == 3 and kv_pointers.size(0) == batch
-             and kv_pointers.size(1) == 2, "kv_pointers must be contiguous int64 [batch, 2, max_blocks]")
-    _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
-    T, hq, hkv = q.size(0), q.size(1), k.size(1)
-    _require(hq % hkv == 0, "num_heads must be a multiple of num_kv_heads")
-    _require(int(size_per_token) == hkv * 128 * (4 if int4_kv_cache else 8) // 8, "size_per_token does not match the kv heads and the cache type")
-    _require(int(max_prefix_len) >= 0 and int(max_seqlen) >= 0, "negative max_prefix_len / max_seqlen")
-    _require(int(max_prefix_len) + int(max_seqlen) <= kv_pointers.size(-1) * 64, "the page table is too short for max_prefix_len + max_seqlen")
+    _require(int(max_seqlen) >= 0, "negative max_seqlen")
+    batch, T, hq, hkv = _paged_prompt(q, k, v, cu_seqlens, max_seqlen, prefix_lens, max_prefix_len, kv_pointers, tokens_per_block, size_per_token,
+                                      int4_kv_cache)
     out = torch.empty((T, hq, 128), dtype=_HALF, device=q.device)
     if T == 0 or batch == 0:
         return out
@@ -520,25 +545,8 @@ def prefix_prefill_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, 
 
 def multi_token_workspace(device: torch.device, batch: int, num_tokens: int, max_seqlen: int, max_prefix_len: int, num_heads: int,
                           num_kv_heads: int, int4_kv_cache: bool) -> torch.Tensor:
-    """Zero-initialised workspace of multi_token_decode_attention, grown on demand and never freed once handed out (as attention_workspace)."""
-    key = ("mtok", device.index)
-    need = max(1, lib.qs_multi_token_attention_workspace_bytes(batch, num_tokens, max_seqlen, max_prefix_len, num_heads, num_kv_heads,
-                                                                           int(bool(int4_kv_cache))))
-    ws = _workspaces.get(key)
-    if ws is None or ws.numel() < need:
-        if ws is not None:
-            _retired.append(ws)
-        with torch.cuda.device(device):
-            ws = torch.zeros(need, dtype=torch.uint8, device=device)
-        _workspaces[key] = ws
-    return ws
-
-
-def _tree_mask_check(tree_mask: torch.Tensor, rows: int, device: torch.device) -> None:
-    _cuda(tree_mask, "tree_mask")
-    _require(tree_mask.device == device, "tree_mask must be on the device of the other tensors")
-    _require(tree_mask.dtype == torch.int32 and tree_mask.is_contiguous() and tree_mask.numel() == rows,
-             "tree_mask must be contiguous int32 with one word per draft row")
+    return _workspace("mtok", device, max(1, lib.qs_multi_token_attention_workspace_bytes(batch, num_tokens, max_seqlen, max_prefix_len, num_heads,
+                                                                                         num_kv_heads, int(bool(int4_kv_cache)))))
 
 
 def multi_token_decode_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_lens, max_prefix_len: int, kv_pointers, tokens_per_block: int,
@@ -560,40 +568,22 @@ def multi_token_decode_attention(q, k, v, cu_seqlens, max_seqlen: int, prefix_le
     its ancestors and to its own key / value, i.e. it gets the decode step at position prefix_lens[b] + depth(i) after sequential decoding
     along its root path.  The mask contents are not validated (that would need a host synchronisation); whatever they hold, the kernels never
     read a slot >= prefix_lens[b] + i for node i.  A chain mask gives this function's result without a mask bit for bit.  None: no mask."""
-    for t, n in ((q, "q"), (k, "k"), (v, "v"), (cu_seqlens, "cu_seqlens"), (prefix_lens, "prefix_lens"), (kv_pointers, "kv_pointers")):
-        _cuda(t, n)
-    _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
-    _require(q.dim() == 3 and k.dim() == 3 and v.dim() == 3 and q.size(2) == 128 and k.size(2) == 128 and v.size(2) == 128, "q, k, v must be [T, H, 128]")
-    _require(k.shape == v.shape and q.size(0) == k.size(0), "q, k, v must cover the same tokens; k and v the same heads")
-    for t, name in ((q, "q"), (k, "k"), (v, "v")):
-        _require(t.stride(2) == 1 and t.stride(1) == 128, f"{name}: heads must be contiguous rows of 128 halfs")
-    _require(cu_seqlens.dtype == torch.int32 and cu_seqlens.is_contiguous() and cu_seqlens.dim() == 1, "cu_seqlens must be contiguous int32")
-    batch = cu_seqlens.size(0) - 1
-    _require(prefix_lens.dtype == torch.int32 and prefix_lens.is_contiguous() and tuple(prefix_lens.shape) == (batch,), "prefix_lens must be contiguous int32 [batch]")
-    _require(kv_pointers.dtype == torch.int64 and kv_pointers.is_contiguous() and kv_pointers.dim() == 3 and kv_pointers.size(0) == batch
-             and kv_pointers.size(1) == 2, "kv_pointers must be contiguous int64 [batch, 2, max_blocks]")
-    _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
-    T, hq, hkv = q.size(0), q.size(1), k.size(1)
-    _require(hq % hkv == 0, "num_heads must be a multiple of num_kv_heads")
-    _require(int(size_per_token) == hkv * 128 * (4 if int4_kv_cache else 8) // 8, "size_per_token does not match the kv heads and the cache type")
     _require(1 <= int(max_seqlen) <= 16, "max_seqlen must be 1 .. 16 draft tokens")
-    _require(int(max_prefix_len) >= 0, "negative max_prefix_len")
-    _require(int(max_prefix_len) + int(max_seqlen) <= kv_pointers.size(-1) * 64, "the page table is too short for max_prefix_len + max_seqlen")
+    batch, T, hq, hkv = _paged_prompt(q, k, v, cu_seqlens, max_seqlen, prefix_lens, max_prefix_len, kv_pointers, tokens_per_block, size_per_token,
+                                      int4_kv_cache)
     out = torch.empty((T, hq, 128), dtype=_HALF, device=q.device)
     if T == 0 or batch == 0:
         return out
+    fn, mask = lib.qs_multi_token_decode_attention, ()
+    if tree_mask is not None:
+        _tensor(tree_mask, "tree_mask", torch.int32, device=q.device)
+        _require(tree_mask.numel() == T, "tree_mask must hold one word per draft row")
+        fn, mask = lib.qs_tree_decode_attention, (tree_mask.data_ptr(),)
     ws = multi_token_workspace(q.device, batch, T, int(max_seqlen), int(max_prefix_len), hq, hkv, int4_kv_cache)
     scale = float(softmax_scale) if softmax_scale is not None else 0.0
-    if tree_mask is not None:
-        _tree_mask_check(tree_mask, T, q.device)
-        _call(q, lib.qs_tree_decode_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), out.data_ptr(),
-              out.stride(0), cu_seqlens.data_ptr(), prefix_lens.data_ptr(), tree_mask.data_ptr(), kv_pointers.data_ptr(), batch, T, int(max_seqlen),
-              int(max_prefix_len), kv_pointers.size(-1), hq, hkv, 128, int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), scale,
-              ws.data_ptr(), ws.numel())
-        return out
-    _call(q, lib.qs_multi_token_decode_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), out.data_ptr(),
-          out.stride(0), cu_seqlens.data_ptr(), prefix_lens.data_ptr(), kv_pointers.data_ptr(), batch, T, int(max_seqlen), int(max_prefix_len),
-          kv_pointers.size(-1), hq, hkv, 128, int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), scale, ws.data_ptr(), ws.numel())
+    _call(q, fn, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0), out.data_ptr(), out.stride(0), cu_seqlens.data_ptr(),
+          prefix_lens.data_ptr(), *mask, kv_pointers.data_ptr(), batch, T, int(max_seqlen), int(max_prefix_len), kv_pointers.size(-1), hq, hkv, 128,
+          int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), scale, ws.data_ptr(), ws.numel())
     return out
 
 
@@ -605,20 +595,14 @@ def tree_accept_greedy(draft_tokens, tree_mask, target_tokens, accept_len: Optio
     walk moves to the lowest-index child c of the current node with draft[c] == target[current] until no child matches.  Returns
     (accept_len int32 [B] >= 1, path int32 [B, n] with path[:, 0] = 0 and -1 past accept_len, bonus int64 [B] = target[last accepted node]);
     the optional out tensors are written in place (CUDA-graph capture)."""
-    for t, n in ((draft_tokens, "draft_tokens"), (tree_mask, "tree_mask"), (target_tokens, "target_tokens")):
-        _cuda(t, n)
-        _require(t.dim() == 2 and t.is_contiguous() and t.device == draft_tokens.device, f"{n} must be a contiguous [B, n] tensor on one device")
-    _require(draft_tokens.dtype == torch.int64 and target_tokens.dtype == torch.int64 and tree_mask.dtype == torch.int32,
-             "draft_tokens / target_tokens must be int64, tree_mask int32")
-    B, n = draft_tokens.shape
-    _require(tuple(tree_mask.shape) == (B, n) and tuple(target_tokens.shape) == (B, n), "draft_tokens, tree_mask and target_tokens must have one shape")
-    _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
+    B, n = _tensor(draft_tokens, "draft_tokens", torch.int64, (None, None)).shape
     dev = draft_tokens.device
-    accept_len = torch.empty(B, dtype=torch.int32, device=dev) if accept_len is None else accept_len
-    path = torch.empty((B, n), dtype=torch.int32, device=dev) if path is None else path
-    bonus = torch.empty(B, dtype=torch.int64, device=dev) if bonus is None else bonus
-    for t, n_, dt, shape in ((accept_len, "accept_len", torch.int32, (B,)), (path, "path", torch.int32, (B, n)), (bonus, "bonus", torch.int64, (B,))):
-        _require(t.device == dev and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, f"{n_} must be contiguous {dt} {shape}")
+    _tensor(tree_mask, "tree_mask", torch.int32, (B, n), dev)
+    _tensor(target_tokens, "target_tokens", torch.int64, (B, n), dev)
+    _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
+    accept_len = _out(accept_len, "accept_len", torch.int32, (B,), dev)
+    path = _out(path, "path", torch.int32, (B, n), dev)
+    bonus = _out(bonus, "bonus", torch.int64, (B,), dev)
     if B:
         _call(draft_tokens, lib.qs_tree_accept_greedy, draft_tokens.data_ptr(), tree_mask.data_ptr(), target_tokens.data_ptr(), accept_len.data_ptr(),
               path.data_ptr(), bonus.data_ptr(), B, n)
@@ -633,17 +617,14 @@ def kv_cache_compact(kv_pointers, start_pos, path, accept_len, num_kv_heads: int
     decoding of the accepted tokens writes; the engine then advances the context by accept_len.  kv_pointers int64 [L, B, 2, max_blocks] or
     [B, 2, max_blocks]; start_pos int32 [B]; path int32 [B, n] and accept_len int32 [B] as tree_accept_greedy returns them (n <= 16).
     The page table must cover start_pos[b] + n slots (not checked on the device: slots outside the table are left alone)."""
-    for t, n in ((kv_pointers, "kv_pointers"), (start_pos, "start_pos"), (path, "path"), (accept_len, "accept_len")):
-        _cuda(t, n)
-        _require(t.is_contiguous() and t.device == kv_pointers.device, f"{n} must be contiguous and on the device of kv_pointers")
-    _require(kv_pointers.dtype == torch.int64 and kv_pointers.dim() in (3, 4) and kv_pointers.size(-2) == 2,
-             "kv_pointers must be int64 [L, B, 2, max_blocks] or [B, 2, max_blocks]")
+    _tensor(kv_pointers, "kv_pointers", torch.int64)
+    _require(kv_pointers.dim() in (3, 4) and kv_pointers.size(-2) == 2, "kv_pointers must be int64 [L, B, 2, max_blocks] or [B, 2, max_blocks]")
     L = kv_pointers.size(0) if kv_pointers.dim() == 4 else 1
     B = kv_pointers.size(-3)
-    _require(start_pos.dtype == torch.int32 and tuple(start_pos.shape) == (B,), "start_pos must be int32 [B]")
-    _require(path.dtype == torch.int32 and path.dim() == 2 and path.size(0) == B, "path must be int32 [B, n]")
-    _require(accept_len.dtype == torch.int32 and tuple(accept_len.shape) == (B,), "accept_len must be int32 [B]")
-    n = path.size(1)
+    dev = kv_pointers.device
+    _tensor(start_pos, "start_pos", torch.int32, (B,), dev)
+    n = _tensor(path, "path", torch.int32, (B, None), dev).size(1)
+    _tensor(accept_len, "accept_len", torch.int32, (B,), dev)
     _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
     _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
     _require(int(num_kv_heads) >= 1 and int(size_per_token) == int(num_kv_heads) * 128 * (4 if int4_kv_cache else 8) // 8,
@@ -659,9 +640,7 @@ def _row_vec(v, n: int, dev, dt, name: str, ok, what: str) -> torch.Tensor:
     """A per-row parameter as a device tensor: a scalar broadcasts (and is checked on the host); a tensor is used as given (its values are
     trusted: checking them would synchronise with the device)."""
     if isinstance(v, torch.Tensor):
-        _cuda(v, name)
-        _require(v.dtype == dt and v.is_contiguous() and tuple(v.shape) == (n,) and v.device == dev, f"{name} must be contiguous {dt} [{n}]")
-        return v
+        return _tensor(v, name, dt, (n,), dev)
     _require(ok(v), f"{name}={v}: {what}")
     return torch.full((n,), v, dtype=dt, device=dev)
 
@@ -673,10 +652,14 @@ def _row_params(n: int, dev, temperature, top_k, top_p, offsets):
     T = vec(temperature, torch.float32, "temperature", lambda v: float(v) >= 0, "must be >= 0")
     K = vec(top_k, torch.int32, "top_k", lambda v: int(v) == -1 or int(v) >= 1, "must be -1 (off) or >= 1")
     P = vec(top_p, torch.float32, "top_p", lambda v: 0 < float(v) <= 1, "must lie in (0, 1]")
-    _cuda(offsets, "offsets")
-    _require(offsets.dtype == torch.int64 and offsets.is_contiguous() and tuple(offsets.shape) == (n,) and offsets.device == dev,
-             f"offsets must be a contiguous int64 [{n}] tensor")
+    _tensor(offsets, "offsets", torch.int64, (n,), dev)
     return T, K, P
+
+
+def _logit_rows(logits) -> tuple:
+    rows, V = _tensor(logits, "logits", _HALF, (None, None)).shape
+    _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
+    return rows, V
 
 
 def _seed(seed) -> int:
@@ -693,15 +676,10 @@ def sample_rows(logits, temperature, top_k, top_p, seed: int, offsets, out: Opti
     token is the inverse CDF of the kept softmax at the Philox draw u (see include/qserve_b200.h).  Differences from the reference: the
     reference divides by T and runs softmax().cumsum() over the row in fp16 and draws with torch's RNG, so the distribution agrees up to its
     fp16 rounding but the same seed does not give the same tokens.  V % 8 == 0, V <= 196608.  Returns out int64 [rows]."""
-    _cuda(logits, "logits")
-    _require(logits.dtype == _HALF and logits.dim() == 2 and logits.is_contiguous(), "logits must be contiguous float16 [rows, vocab]")
-    rows, V = logits.shape
+    rows, V = _logit_rows(logits)
     dev = logits.device
-    _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
     T, K, P = _row_params(rows, dev, temperature, top_k, top_p, offsets)
-    if out is None:
-        out = torch.empty(rows, dtype=torch.int64, device=dev)
-    _require(out.dtype == torch.int64 and out.is_contiguous() and tuple(out.shape) == (rows,) and out.device == dev, "out must be contiguous int64 [rows]")
+    out = _out(out, "out", torch.int64, (rows,), dev)
     if rows:
         _call(logits, lib.qs_sample_rows, out.data_ptr(), logits.data_ptr(), T.data_ptr(), K.data_ptr(), P.data_ptr(), _seed(seed), offsets.data_ptr(),
               rows, V)
@@ -720,46 +698,26 @@ def tree_accept_sampling(draft_tokens, tree_mask, logits, temperature, top_k, to
     0); with no child accepted the bonus is drawn from p with draw j = 0.  Greedy rows (T < 1e-5 or top_p < 1e-8) give exactly
     tree_accept_greedy(draft, mask, argmax_rows(logits)).  Returns (accept_len int32 [B], path int32 [B, n], bonus int64 [B]), ready for
     kv_cache_compact; the optional out tensors are written in place (CUDA-graph capture)."""
-    for t, nm in ((draft_tokens, "draft_tokens"), (tree_mask, "tree_mask")):
-        _cuda(t, nm)
-        _require(t.dim() == 2 and t.is_contiguous() and t.device == draft_tokens.device, f"{nm} must be a contiguous [B, n] tensor on one device")
-    _require(draft_tokens.dtype == torch.int64 and tree_mask.dtype == torch.int32, "draft_tokens must be int64, tree_mask int32")
-    B, n = draft_tokens.shape
+    B, n = _tensor(draft_tokens, "draft_tokens", torch.int64, (None, None)).shape
     dev = draft_tokens.device
-    _require(tuple(tree_mask.shape) == (B, n), "draft_tokens and tree_mask must have one shape")
+    _tensor(tree_mask, "tree_mask", torch.int32, (B, n), dev)
     _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
-    _cuda(logits, "logits")
-    _require(logits.dtype == _HALF and logits.dim() == 3 and logits.is_contiguous() and tuple(logits.shape[:2]) == (B, n) and logits.device == dev,
-             "logits must be contiguous float16 [B, n, vocab] on the device of the drafts")
-    V = logits.size(2)
+    V = _tensor(logits, "logits", _HALF, (B, n, None), dev).size(2)
     _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
     if draft_probs is not None:
-        _cuda(draft_probs, "draft_probs")
-        _require(draft_probs.dtype == torch.float32 and draft_probs.is_contiguous() and tuple(draft_probs.shape) == (B, n, V) and draft_probs.device == dev,
-                 "draft_probs must be contiguous float32 [B, n, vocab]")
+        _tensor(draft_probs, "draft_probs", torch.float32, (B, n, V), dev)
     T, K, P = _row_params(B, dev, temperature, top_k, top_p, offsets)
-    accept_len = torch.empty(B, dtype=torch.int32, device=dev) if accept_len is None else accept_len
-    path = torch.empty((B, n), dtype=torch.int32, device=dev) if path is None else path
-    bonus = torch.empty(B, dtype=torch.int64, device=dev) if bonus is None else bonus
-    for t, n_, dt, shape in ((accept_len, "accept_len", torch.int32, (B,)), (path, "path", torch.int32, (B, n)), (bonus, "bonus", torch.int64, (B,))):
-        _require(t.device == dev and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, f"{n_} must be contiguous {dt} {shape}")
+    accept_len = _out(accept_len, "accept_len", torch.int32, (B,), dev)
+    path = _out(path, "path", torch.int32, (B, n), dev)
+    bonus = _out(bonus, "bonus", torch.int64, (B,), dev)
     if B:
-        _call(draft_tokens, lib.qs_tree_accept_sampling, draft_tokens.data_ptr(), tree_mask.data_ptr(), logits.data_ptr(),
-              draft_probs.data_ptr() if draft_probs is not None else None, T.data_ptr(), K.data_ptr(), P.data_ptr(), _seed(seed), offsets.data_ptr(),
-              accept_len.data_ptr(), path.data_ptr(), bonus.data_ptr(), B, n, V)
+        _call(draft_tokens, lib.qs_tree_accept_sampling, draft_tokens.data_ptr(), tree_mask.data_ptr(), logits.data_ptr(), _ptr(draft_probs), T.data_ptr(),
+              K.data_ptr(), P.data_ptr(), _seed(seed), offsets.data_ptr(), accept_len.data_ptr(), path.data_ptr(), bonus.data_ptr(), B, n, V)
     return accept_len, path, bonus
 
 
 MAX_PENALTY_HISTORY = 32768  # history tokens per row apply_penalties supports
 MAX_TOP_LOGPROBS = 20
-
-
-def _logit_rows(logits) -> tuple:
-    _cuda(logits, "logits")
-    _require(logits.dtype == _HALF and logits.dim() == 2 and logits.is_contiguous(), "logits must be contiguous float16 [rows, vocab]")
-    rows, V = logits.shape
-    _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
-    return rows, V
 
 
 def apply_penalties(logits, history, prompt_lens, seq_lens, repetition, presence, frequency) -> torch.Tensor:
@@ -773,14 +731,10 @@ def apply_penalties(logits, history, prompt_lens, seq_lens, repetition, presence
     the call is bitwise deterministic.  See include/qserve_b200.h."""
     rows, V = _logit_rows(logits)
     dev = logits.device
-    _cuda(history, "history")
-    _require(history.dtype == torch.int64 and history.dim() == 2 and history.is_contiguous() and history.size(0) == rows and history.device == dev,
-             f"history must be contiguous int64 [{rows}, H] on the device of the logits")
-    H = history.size(1)
+    H = _tensor(history, "history", torch.int64, (rows, None), dev).size(1)
     _require(H <= MAX_PENALTY_HISTORY, f"history of {H} tokens per row: at most {MAX_PENALTY_HISTORY}")
-    for t, nm in ((prompt_lens, "prompt_lens"), (seq_lens, "seq_lens")):
-        _cuda(t, nm)
-        _require(t.dtype == torch.int32 and t.is_contiguous() and tuple(t.shape) == (rows,) and t.device == dev, f"{nm} must be contiguous int32 [{rows}]")
+    _tensor(prompt_lens, "prompt_lens", torch.int32, (rows,), dev)
+    _tensor(seq_lens, "seq_lens", torch.int32, (rows,), dev)
     R = _row_vec(repetition, rows, dev, torch.float32, "repetition", lambda v: 0 < float(v) <= 2, "must lie in (0, 2]")
     P = _row_vec(presence, rows, dev, torch.float32, "presence", lambda v: -2 <= float(v) <= 2, "must lie in [-2, 2]")
     F = _row_vec(frequency, rows, dev, torch.float32, "frequency", lambda v: -2 <= float(v) <= 2, "must lie in [-2, 2]")
@@ -802,28 +756,18 @@ def logprobs_rows(logits, tokens, n: int, logprob: Optional[torch.Tensor] = None
     dev = logits.device
     n = int(n)
     _require(0 <= n <= MAX_TOP_LOGPROBS, f"n={n}: 0 .. {MAX_TOP_LOGPROBS} top log-probabilities")
-    _cuda(tokens, "tokens")
-    _require(tokens.dtype == torch.int64 and tokens.is_contiguous() and tuple(tokens.shape) == (rows,) and tokens.device == dev,
-             f"tokens must be contiguous int64 [{rows}]")
-    logprob = torch.empty(rows, dtype=torch.float32, device=dev) if logprob is None else logprob
-    top_ids = torch.empty((rows, n), dtype=torch.int64, device=dev) if top_ids is None else top_ids
-    top_logprobs = torch.empty((rows, n), dtype=torch.float32, device=dev) if top_logprobs is None else top_logprobs
-    for t, nm, dt, shape in ((logprob, "logprob", torch.float32, (rows,)), (top_ids, "top_ids", torch.int64, (rows, n)),
-                             (top_logprobs, "top_logprobs", torch.float32, (rows, n))):
-        _require(t.device == dev and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, f"{nm} must be contiguous {dt} {shape}")
+    _tensor(tokens, "tokens", torch.int64, (rows,), dev)
+    logprob = _out(logprob, "logprob", torch.float32, (rows,), dev)
+    top_ids = _out(top_ids, "top_ids", torch.int64, (rows, n), dev)
+    top_logprobs = _out(top_logprobs, "top_logprobs", torch.float32, (rows, n), dev)
     if rows:
-        _call(logits, lib.qs_logprobs_rows, logprob.data_ptr(), top_ids.data_ptr() if n else None, top_logprobs.data_ptr() if n else None,
+        _call(logits, lib.qs_logprobs_rows, logprob.data_ptr(), _ptr(top_ids if n else None), _ptr(top_logprobs if n else None),
               logits.data_ptr(), tokens.data_ptr(), rows, V, n)
     return logprob, top_ids, top_logprobs
 
 
 MAX_DRAFT_NGRAM = 8
 MAX_DRAFT_BRANCHES = 8
-
-
-def _rows_tensor(t, name: str, dt, shape, dev) -> None:
-    _cuda(t, name)
-    _require(t.dtype == dt and t.is_contiguous() and tuple(t.shape) == tuple(shape) and t.device == dev, f"{name} must be contiguous {dt} {tuple(shape)}")
 
 
 def ngram_propose(history, seq_lens, num_nodes: int, n_min: int = 1, n_max: int = 4, branches: int = 1, tokens: Optional[torch.Tensor] = None,
@@ -840,16 +784,12 @@ def ngram_propose(history, seq_lens, num_nodes: int, n_min: int = 1, n_max: int 
     _require(1 <= n <= 16, f"num_nodes={n}: a draft tree has 1 .. 16 nodes")
     _require(1 <= n_min <= n_max <= MAX_DRAFT_NGRAM, f"n_min={n_min}, n_max={n_max}: need 1 <= n_min <= n_max <= {MAX_DRAFT_NGRAM}")
     _require(1 <= branches <= MAX_DRAFT_BRANCHES, f"branches={branches}: 1 .. {MAX_DRAFT_BRANCHES}")
-    _cuda(history, "history")
-    _require(history.dtype == torch.int64 and history.dim() == 2 and history.is_contiguous(), "history must be contiguous int64 [B, H]")
-    B, H = history.shape
+    B, H = _tensor(history, "history", torch.int64, (None, None)).shape
     _require(1 <= H <= MAX_PENALTY_HISTORY, f"history of {H} tokens per row: 1 .. {MAX_PENALTY_HISTORY}")
     dev = history.device
-    _rows_tensor(seq_lens, "seq_lens", torch.int32, (B,), dev)
-    tokens = torch.empty((B, n), dtype=torch.int64, device=dev) if tokens is None else tokens
-    tree_mask = torch.empty((B, n), dtype=torch.int32, device=dev) if tree_mask is None else tree_mask
-    _rows_tensor(tokens, "tokens", torch.int64, (B, n), dev)
-    _rows_tensor(tree_mask, "tree_mask", torch.int32, (B, n), dev)
+    _tensor(seq_lens, "seq_lens", torch.int32, (B,), dev)
+    tokens = _out(tokens, "tokens", torch.int64, (B, n), dev)
+    tree_mask = _out(tree_mask, "tree_mask", torch.int32, (B, n), dev)
     if B:
         _call(history, lib.qs_ngram_propose, history.data_ptr(), seq_lens.data_ptr(), tokens.data_ptr(), tree_mask.data_ptr(), B, H, n, n_min, n_max,
               branches)
@@ -866,29 +806,23 @@ def spec_commit(draft_tokens, path, accept_len, bonus, history, seq_lens, prompt
     token: what the next verify step (start_pos) or decode step (context_lens, tokens = roots) reads.  finished int32 [B] is set when a row
     appends eos or reaches its budget; finished rows are left untouched.  A plain decode step commits with n = 1, path = 0, accept_len = 1 and
     bonus = its token.  See include/qserve_b200.h."""
-    _cuda(draft_tokens, "draft_tokens")
-    _require(draft_tokens.dtype == torch.int64 and draft_tokens.dim() == 2 and draft_tokens.is_contiguous(), "draft_tokens must be contiguous int64 [B, n]")
-    B, n = draft_tokens.shape
+    B, n = _tensor(draft_tokens, "draft_tokens", torch.int64, (None, None)).shape
     _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
     dev = draft_tokens.device
-    _cuda(history, "history")
-    _require(history.dtype == torch.int64 and history.dim() == 2 and history.is_contiguous() and history.size(0) == B and history.device == dev,
-             f"history must be contiguous int64 [{B}, H] on the device of the drafts")
-    H = history.size(1)
+    H = _tensor(history, "history", torch.int64, (B, None), dev).size(1)
     _require(1 <= H <= MAX_PENALTY_HISTORY, f"history of {H} tokens per row: 1 .. {MAX_PENALTY_HISTORY}")
-    _rows_tensor(path, "path", torch.int32, (B, n), dev)
+    _tensor(path, "path", torch.int32, (B, n), dev)
     for t, nm, dt in ((accept_len, "accept_len", torch.int32), (bonus, "bonus", torch.int64), (seq_lens, "seq_lens", torch.int32),
                       (prompt_lens, "prompt_lens", torch.int32), (budget, "budget", torch.int32), (eos, "eos", torch.int64),
                       (finished, "finished", torch.int32), (start_pos, "start_pos", torch.int32)):
-        _rows_tensor(t, nm, dt, (B,), dev)
-    if context_lens is not None:
-        _rows_tensor(context_lens, "context_lens", torch.int32, (B,), dev)
-    if roots is not None:
-        _rows_tensor(roots, "roots", torch.int64, (B,), dev)
+        _tensor(t, nm, dt, (B,), dev)
+    for t, nm, dt in ((context_lens, "context_lens", torch.int32), (roots, "roots", torch.int64)):
+        if t is not None:
+            _tensor(t, nm, dt, (B,), dev)
     if B:
         _call(history, lib.qs_spec_commit, draft_tokens.data_ptr(), path.data_ptr(), accept_len.data_ptr(), bonus.data_ptr(), history.data_ptr(),
               seq_lens.data_ptr(), prompt_lens.data_ptr(), budget.data_ptr(), eos.data_ptr(), finished.data_ptr(), start_pos.data_ptr(),
-              context_lens.data_ptr() if context_lens is not None else None, roots.data_ptr() if roots is not None else None, B, n, H)
+              _ptr(context_lens), _ptr(roots), B, n, H)
 
 
 class PeerContext:
@@ -928,7 +862,7 @@ def add_rms_norm_general_peer(out, hidden_out, x, ctx: "PeerContext", phase: int
     tokens, hidden = _rows(x)
     _require(tokens == ctx.tokens and hidden == ctx.hidden, "add_rms_norm_general_peer: shape does not match the PeerContext")
     _call(x, lib.qs_add_rms_norm_general_peer, out.data_ptr(), hidden_out.data_ptr(), x.data_ptr(), ctx._delta[phase], ctx._flags, ctx.state.data_ptr(),
-          ctx.world, ctx.rank, int(phase), weight.data_ptr(), input_sum.data_ptr() if input_sum is not None else None, scaling.data_ptr(), float(epsilon),
+          ctx.world, ctx.rank, int(phase), weight.data_ptr(), _ptr(input_sum), scaling.data_ptr(), float(epsilon),
           tokens, hidden)
 
 
@@ -949,14 +883,13 @@ def invoke_quant_given_amax(out, input, amax: torch.Tensor, input_sum: Optional[
     if _noop(input):
         return
     tokens, hidden = _rows(input)
-    _call(input, lib.qs_invoke_quant_given_amax, out.data_ptr(), input.data_ptr(), amax.data_ptr(), input_sum.data_ptr() if input_sum is not None else None,
+    _call(input, lib.qs_invoke_quant_given_amax, out.data_ptr(), input.data_ptr(), amax.data_ptr(), _ptr(input_sum),
           scale.data_ptr(), tokens, hidden)
 
 
 def argmax_rows(logits: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """torch.argmax(logits, dim=-1) for fp16 logits [rows, vocab] in one launch (greedy sampling of the decode runner)."""
-    _cuda(logits, "logits")
-    _require(logits.dtype == _HALF and logits.dim() == 2 and logits.is_contiguous(), "logits must be contiguous float16 [rows, vocab]")
+    _tensor(logits, "logits", _HALF, (None, None))
     if out is None:
         out = torch.empty(logits.size(0), dtype=torch.int64, device=logits.device)
     if logits.size(0) == 0:

@@ -63,6 +63,43 @@ int raise_smem_limit(const void* kern, size_t bytes, const char* what) {
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// The GemmArgs fields the three GEMM entries share, and the process-wide tuning controls.
+static GemmArgs gemm_args(const int8_t* in_feats, const int8_t* kernel, const void* wscales, const void* ascales, void* out_feats, int32_t* acc_out, int M,
+                          int N, int K, void* workspace, size_t workspace_bytes, void* stream) {
+  GemmArgs a;
+  a.act = in_feats; a.weight = kernel; a.wscales = wscales; a.ascales = ascales; a.out = out_feats; a.acc_out = acc_out; a.M = M; a.N = N; a.K = K;
+  a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.force_split = g_force_split; a.force_nt = g_force_nt; a.prof = g_gemm_prof; a.stream = stream;
+  return a;
+}
+
+// The three qs_apply_bias_rope_update_kv_cache* entries; start_pos and tree_mask are null where an entry has none.
+static int rope_append(void* qkv, const int32_t* seq_lens, const int32_t* padding_offset, const int32_t* start_pos, const int32_t* tree_mask,
+                       const int64_t* kv_pointers, int batch, int num_tokens, int max_blocks, int head_num, int kv_head_num, int head_dim, int seq_len,
+                       int tokens_per_block, int size_per_token, int rotary_dim, float rotary_base, int max_positions, int int4_kv, int kv_zeros,
+                       void* stream) {
+  PrefillAppendArgs a;
+  a.qkv = qkv; a.seq_lens = seq_lens; a.padding_offset = padding_offset; a.start_pos = start_pos; a.tree_mask = tree_mask;
+  a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers); a.batch = batch; a.num_tokens = num_tokens; a.max_blocks = max_blocks;
+  a.num_heads = head_num; a.num_kv_heads = kv_head_num; a.head_dim = head_dim; a.seq_len = seq_len; a.tokens_per_block = tokens_per_block;
+  a.size_per_token = size_per_token; a.rotary_dim = rotary_dim; a.rotary_base = rotary_base; a.max_positions = max_positions; a.int4_kv = int4_kv;
+  a.kv_zeros = kv_zeros; a.stream = stream;
+  return prefill_rope_append(a);
+}
+
+// qs_multi_token_decode_attention (tree_mask null) and qs_tree_decode_attention.
+static int multi_token(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out, int64_t out_stride,
+                       const int32_t* cu_seqlens, const int32_t* prefix_lens, const int32_t* tree_mask, const int64_t* kv_pointers, int batch, int num_tokens,
+                       int max_seqlen, int max_prefix_len, int max_blocks, int num_heads, int num_kv_heads, int head_dim, int tokens_per_block,
+                       int size_per_token, int int4_kv, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
+  MultiTokenAttnArgs a;
+  a.q = q; a.k = k; a.v = v; a.out = out; a.q_stride = q_stride; a.k_stride = k_stride; a.v_stride = v_stride; a.out_stride = out_stride;
+  a.cu_seqlens = cu_seqlens; a.prefix_lens = prefix_lens; a.tree_mask = tree_mask; a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
+  a.batch = batch; a.num_tokens = num_tokens; a.max_seqlen = max_seqlen; a.max_prefix_len = max_prefix_len; a.max_blocks = max_blocks; a.num_heads = num_heads;
+  a.num_kv_heads = num_kv_heads; a.head_dim = head_dim; a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token; a.int4_kv = int4_kv;
+  a.softmax_scale = softmax_scale; a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = stream;
+  return multi_token_attention(a);
+}
+
 }  // namespace qs
 
 using namespace qs;
@@ -103,10 +140,8 @@ int qs_w4a8_gemm_per_chn(const int8_t* in_feats, const int8_t* kernel, const voi
                          const void* a_ssums, void* out_feats, int32_t* acc_out, int M, int N, int K, void* workspace, size_t workspace_bytes,
                          void* stream) {
   QS_REQUIRE(in_feats && kernel && wscales && ascales && w_szs && a_ssums && out_feats, "qgemm_w4a8_per_chn: null tensor");
-  GemmArgs a;
-  a.act = in_feats; a.weight = kernel; a.wscales = wscales; a.ascales = ascales; a.w_szs = w_szs; a.a_ssums = a_ssums;
-  a.out = out_feats; a.acc_out = acc_out; a.M = M; a.N = N; a.K = K;
-  a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.force_split = g_force_split; a.force_nt = g_force_nt; a.prof = g_gemm_prof; a.stream = stream;
+  GemmArgs a = gemm_args(in_feats, kernel, wscales, ascales, out_feats, acc_out, M, N, K, workspace, workspace_bytes, stream);
+  a.w_szs = w_szs; a.a_ssums = a_ssums;
   return gemm_w4a8_per_chn(a);
 }
 
@@ -115,21 +150,15 @@ int qs_w4a8_gemm_per_group(const int8_t* in_feats, const int8_t* kernel, const i
                            size_t workspace_bytes, void* stream) {
   QS_REQUIRE(in_feats && kernel && zeros && scales_i8 && wscales && ascales && out_feats, "qgemm_w4a8_per_group: null tensor");
   QS_REQUIRE(aligned16(zeros) && aligned16(scales_i8), "qgemm_w4a8_per_group: level-2 scale/zero tensors must be 16-byte aligned");
-  GemmArgs a;
-  a.act = in_feats; a.weight = kernel; a.s2_zeros = zeros; a.s2_scales = scales_i8; a.wscales = wscales; a.ascales = ascales;
-  a.out = out_feats; a.acc_out = acc_out; a.M = M; a.N = N; a.K = K;
-  a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.force_split = g_force_split; a.force_nt = g_force_nt; a.prof = g_gemm_prof; a.stream = stream;
+  GemmArgs a = gemm_args(in_feats, kernel, wscales, ascales, out_feats, acc_out, M, N, K, workspace, workspace_bytes, stream);
+  a.s2_zeros = zeros; a.s2_scales = scales_i8;
   return gemm_w4a8_per_group(a);
 }
 
 int qs_w8a8_gemm(const int8_t* in_feats, const int8_t* kernel, const void* wscales, const void* ascales, void* out_feats, int32_t* acc_out,
                  int M, int N, int K, void* workspace, size_t workspace_bytes, void* stream) {
   QS_REQUIRE(in_feats && kernel && wscales && ascales && out_feats, "qgemm_w8a8: null tensor");
-  GemmArgs a;
-  a.act = in_feats; a.weight = kernel; a.wscales = wscales; a.ascales = ascales;
-  a.out = out_feats; a.acc_out = acc_out; a.M = M; a.N = N; a.K = K;
-  a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.force_split = g_force_split; a.force_nt = g_force_nt; a.prof = g_gemm_prof; a.stream = stream;
-  return gemm_w8a8(a);
+  return gemm_w8a8(gemm_args(in_feats, kernel, wscales, ascales, out_feats, acc_out, M, N, K, workspace, workspace_bytes, stream));
 }
 
 size_t qs_attention_workspace_bytes(int batch, int num_heads, int head_dim) { return attention_workspace_bytes(batch, num_heads, head_dim, 32); }
@@ -175,13 +204,9 @@ int qs_apply_bias_rope_update_kv_cache(void* qkv, const int32_t* seq_lens, const
                                        void* stream) {
   (void)neox_rotary_style;
   QS_REQUIRE(qkv && seq_lens, "apply_bias_rope_update_kv_cache: null tensor");
-  PrefillAppendArgs a;
-  a.qkv = qkv; a.seq_lens = seq_lens; a.padding_offset = padding_offset; a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
-  a.batch = batch; a.num_tokens = num_tokens; a.max_blocks = max_blocks_per_seq; a.num_heads = head_num; a.num_kv_heads = kv_head_num;
-  a.head_dim = head_dim; a.seq_len = seq_len; a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token;
-  a.rotary_dim = rotary_embedding_dim; a.rotary_base = rotary_embedding_base; a.max_positions = rotary_embedding_max_positions;
-  a.int4_kv = int4_kv_cache; a.kv_zeros = kv_cache_with_zeros; a.stream = stream;
-  return prefill_rope_append(a);
+  return rope_append(qkv, seq_lens, padding_offset, nullptr, nullptr, kv_pointers, batch, num_tokens, max_blocks_per_seq, head_num, kv_head_num, head_dim,
+                     seq_len, tokens_per_block, size_per_token, rotary_embedding_dim, rotary_embedding_base, rotary_embedding_max_positions, int4_kv_cache,
+                     kv_cache_with_zeros, stream);
 }
 
 int qs_apply_bias_rope_update_kv_cache_at(void* qkv, const int32_t* seq_lens, const int32_t* padding_offset, const int32_t* start_pos,
@@ -191,14 +216,9 @@ int qs_apply_bias_rope_update_kv_cache_at(void* qkv, const int32_t* seq_lens, co
                                           int kv_cache_with_zeros, void* stream) {
   (void)neox_rotary_style;
   QS_REQUIRE(qkv && seq_lens && start_pos, "apply_bias_rope_update_kv_cache_at: null tensor");
-  PrefillAppendArgs a;
-  a.qkv = qkv; a.seq_lens = seq_lens; a.padding_offset = padding_offset; a.start_pos = start_pos;
-  a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
-  a.batch = batch; a.num_tokens = num_tokens; a.max_blocks = max_blocks_per_seq; a.num_heads = head_num; a.num_kv_heads = kv_head_num;
-  a.head_dim = head_dim; a.seq_len = seq_len; a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token;
-  a.rotary_dim = rotary_embedding_dim; a.rotary_base = rotary_embedding_base; a.max_positions = rotary_embedding_max_positions;
-  a.int4_kv = int4_kv_cache; a.kv_zeros = kv_cache_with_zeros; a.stream = stream;
-  return prefill_rope_append(a);
+  return rope_append(qkv, seq_lens, padding_offset, start_pos, nullptr, kv_pointers, batch, num_tokens, max_blocks_per_seq, head_num, kv_head_num, head_dim,
+                     seq_len, tokens_per_block, size_per_token, rotary_embedding_dim, rotary_embedding_base, rotary_embedding_max_positions, int4_kv_cache,
+                     kv_cache_with_zeros, stream);
 }
 
 int qs_apply_bias_rope_update_kv_cache_tree(void* qkv, const int32_t* seq_lens, const int32_t* padding_offset, const int32_t* start_pos,
@@ -208,14 +228,9 @@ int qs_apply_bias_rope_update_kv_cache_tree(void* qkv, const int32_t* seq_lens, 
                                             int neox_rotary_style, int int4_kv_cache, int kv_cache_with_zeros, void* stream) {
   (void)neox_rotary_style;
   QS_REQUIRE(qkv && seq_lens && start_pos && tree_mask, "apply_bias_rope_update_kv_cache_tree: null tensor");
-  PrefillAppendArgs a;
-  a.qkv = qkv; a.seq_lens = seq_lens; a.padding_offset = padding_offset; a.start_pos = start_pos; a.tree_mask = tree_mask;
-  a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
-  a.batch = batch; a.num_tokens = num_tokens; a.max_blocks = max_blocks_per_seq; a.num_heads = head_num; a.num_kv_heads = kv_head_num;
-  a.head_dim = head_dim; a.seq_len = seq_len; a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token;
-  a.rotary_dim = rotary_embedding_dim; a.rotary_base = rotary_embedding_base; a.max_positions = rotary_embedding_max_positions;
-  a.int4_kv = int4_kv_cache; a.kv_zeros = kv_cache_with_zeros; a.stream = stream;
-  return prefill_rope_append(a);
+  return rope_append(qkv, seq_lens, padding_offset, start_pos, tree_mask, kv_pointers, batch, num_tokens, max_blocks_per_seq, head_num, kv_head_num, head_dim,
+                     seq_len, tokens_per_block, size_per_token, rotary_embedding_dim, rotary_embedding_base, rotary_embedding_max_positions, int4_kv_cache,
+                     kv_cache_with_zeros, stream);
 }
 
 int qs_prefix_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
@@ -236,14 +251,9 @@ int qs_multi_token_decode_attention(const void* q, const void* k, const void* v,
                                     int num_tokens, int max_seqlen, int max_prefix_len, int max_blocks_per_seq, int num_heads, int num_kv_heads,
                                     int head_dim, int tokens_per_block, int size_per_token, int int4_kv_cache, float softmax_scale, void* workspace,
                                     size_t workspace_bytes, void* stream) {
-  MultiTokenAttnArgs a;
-  a.q = q; a.k = k; a.v = v; a.out = out; a.q_stride = q_stride; a.k_stride = k_stride; a.v_stride = v_stride; a.out_stride = out_stride;
-  a.cu_seqlens = cu_seqlens; a.prefix_lens = prefix_lens; a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
-  a.batch = batch; a.num_tokens = num_tokens; a.max_seqlen = max_seqlen; a.max_prefix_len = max_prefix_len; a.max_blocks = max_blocks_per_seq;
-  a.num_heads = num_heads; a.num_kv_heads = num_kv_heads; a.head_dim = head_dim; a.tokens_per_block = tokens_per_block;
-  a.size_per_token = size_per_token; a.int4_kv = int4_kv_cache; a.softmax_scale = softmax_scale;
-  a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = stream;
-  return multi_token_attention(a);
+  return multi_token(q, k, v, q_stride, k_stride, v_stride, out, out_stride, cu_seqlens, prefix_lens, nullptr, kv_pointers, batch, num_tokens, max_seqlen,
+                     max_prefix_len, max_blocks_per_seq, num_heads, num_kv_heads, head_dim, tokens_per_block, size_per_token, int4_kv_cache, softmax_scale,
+                     workspace, workspace_bytes, stream);
 }
 size_t qs_multi_token_attention_workspace_bytes(int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads,
                                                 int int4_kv_cache) {
@@ -256,14 +266,9 @@ int qs_tree_decode_attention(const void* q, const void* k, const void* v, int64_
                              int num_heads, int num_kv_heads, int head_dim, int tokens_per_block, int size_per_token, int int4_kv_cache,
                              float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
   QS_REQUIRE(tree_mask, "tree_decode_attention: null tree_mask");
-  MultiTokenAttnArgs a;
-  a.q = q; a.k = k; a.v = v; a.out = out; a.q_stride = q_stride; a.k_stride = k_stride; a.v_stride = v_stride; a.out_stride = out_stride;
-  a.cu_seqlens = cu_seqlens; a.prefix_lens = prefix_lens; a.tree_mask = tree_mask; a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers);
-  a.batch = batch; a.num_tokens = num_tokens; a.max_seqlen = max_seqlen; a.max_prefix_len = max_prefix_len; a.max_blocks = max_blocks_per_seq;
-  a.num_heads = num_heads; a.num_kv_heads = num_kv_heads; a.head_dim = head_dim; a.tokens_per_block = tokens_per_block;
-  a.size_per_token = size_per_token; a.int4_kv = int4_kv_cache; a.softmax_scale = softmax_scale;
-  a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = stream;
-  return multi_token_attention(a);
+  return multi_token(q, k, v, q_stride, k_stride, v_stride, out, out_stride, cu_seqlens, prefix_lens, tree_mask, kv_pointers, batch, num_tokens, max_seqlen,
+                     max_prefix_len, max_blocks_per_seq, num_heads, num_kv_heads, head_dim, tokens_per_block, size_per_token, int4_kv_cache, softmax_scale,
+                     workspace, workspace_bytes, stream);
 }
 
 int qs_tree_accept_greedy(const int64_t* draft_tokens, const int32_t* tree_mask, const int64_t* target_tokens, int32_t* accept_len, int32_t* path,

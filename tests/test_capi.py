@@ -1,5 +1,5 @@
-"""CPU tests: the C-ABI library loads and exports every symbol include/qserve_b200.h declares; the drop-in
-package exposes the reference's module and function names; ops fail loudly without a GPU (no fallback)."""
+"""CPU tests: the C-ABI library loads and exports every symbol include/qserve_b200.h declares, with the ctypes types of its prototype; the
+drop-in package exposes the reference's module and function names; ops fail loudly without a GPU (no fallback)."""
 import ctypes
 import inspect
 import os
@@ -9,22 +9,40 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+_CTYPES = {"int": ctypes.c_int, "int32_t": ctypes.c_int, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64, "unsigned": ctypes.c_uint,
+           "size_t": ctypes.c_size_t, "float": ctypes.c_float}
+
+
+def _ctype(c_type: str, ret: bool = False):
+    """The ctypes type a C type of the header is bound with: every pointer is c_void_p, except a `const char*` result (c_char_p)."""
+    c_type = " ".join(c_type.replace("*", " * ").split())
+    if "*" in c_type:
+        return ctypes.c_char_p if ret and c_type == "const char *" else ctypes.c_void_p
+    return _CTYPES[c_type]
 
 
 def _declared():
-    text = open(os.path.join(ROOT, "include", "qserve_b200.h")).read()
-    return sorted(set(re.findall(r"QS_API[^;(]*?\b(qs_[a-z0-9_]+)\s*\(", text)))
+    """name -> (restype, argtypes) of every qs_* prototype in include/qserve_b200.h, in ctypes terms."""
+    text = re.sub(r"/\*.*?\*/", " ", open(os.path.join(ROOT, "include", "qserve_b200.h")).read(), flags=re.S)
+    protos = {}
+    for ret, name, params in re.findall(r"QS_API\s+([^;(]*?)\s*\b(qs_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", text):
+        params = [] if params.strip() == "void" else [re.fullmatch(r"(.*?)\s*\w+", p.strip()).group(1) for p in params.split(",")]
+        protos[name] = (_ctype(ret, ret=True), [_ctype(p) for p in params])
+    return protos
 
 
 def test_library_exports_every_declared_symbol():
     from qserve_b200 import _lib
 
-    names = _declared()
+    protos = _declared()
+    names = sorted(protos)
     assert len(names) >= 25
     raw = ctypes.CDLL(_lib.LIB_PATH)
     for n in names:
         assert hasattr(raw, n), f"{n} declared in include/qserve_b200.h but not exported"
     assert sorted(_lib.SIGNATURES) == names, "python binding and header disagree"
+    wrong = {n: (_lib.SIGNATURES[n], protos[n]) for n in names if _lib.SIGNATURES[n] != protos[n]}
+    assert not wrong, f"ctypes (restype, argtypes) differ from include/qserve_b200.h (binding, header): {wrong}"
     assert raw.qs_abi_version() == _lib.ABI_VERSION
 
 

@@ -246,6 +246,36 @@ def test_attention_argument_errors(dev):
     with pytest.raises(RuntimeError):  # kv cache without zero points is never produced by the engine (arg_utils.py:422)
         fa.single_query_attention(q, k, k, table, lens, None, 8192, 64, Hkv * D // 2, 1, D, 1e4, True, True, False)
 
+    from qserve_b200 import backend as ext
+    out_q = torch.zeros((B, Hq * D), dtype=torch.int8, device=dev)
+    scale = torch.zeros(B, dtype=torch.half, device=dev)
+    quant = dict(q=q, k=k, v=k, kv_pointers=table, length_per_sample=lens, memory_max_seqlen=8192, tokens_per_block=64, size_per_token=Hkv * D // 2,
+                 timestep=1, rotary_embedding_dim=D, rotary_base=1e4, int4_kv_cache=True, kv_cache_with_zeros=True, out_q=out_q, out_scale=scale,
+                 out_sum=scale)
+
+    def bad_quant(**kw):
+        with pytest.raises(RuntimeError):
+            ext.single_query_attention_quant(**{**quant, **kw})
+
+    bad_quant(q=q.cpu())                                      # CPU tensors
+    bad_quant(k=k.cpu(), v=k.cpu())
+    bad_quant(kv_pointers=table.cpu())
+    bad_quant(length_per_sample=lens.cpu())
+    bad_quant(out_q=out_q.cpu())
+    bad_quant(out_scale=scale.cpu())
+    bad_quant(k=k.float(), v=k.float())                       # dtypes
+    bad_quant(kv_pointers=table.int())
+    bad_quant(length_per_sample=lens.long())
+    bad_quant(out_scale=scale.float())
+    bad_quant(out_sum=scale.float())
+    bad_quant(length_per_sample=lens[:1].clone())             # one entry per sequence
+    bad_quant(out_sum=scale[:1].clone())
+    bad_quant(length_per_sample=torch.ones((B, 2), dtype=torch.int32, device=dev)[:, 0])  # not contiguous
+    if torch.cuda.device_count() > 1:                         # every tensor on q's device
+        bad_quant(kv_pointers=table.to("cuda:1"))
+        bad_quant(length_per_sample=lens.to("cuda:1"))
+        bad_quant(out_scale=scale.to("cuda:1"))
+
 
 def test_multi_wave_launches_are_stable(dev):
     """Regression (round 2): more CTAs than resident slots (4 per SM).  A late CTA of a multi-wave launch does not sit in

@@ -269,6 +269,10 @@ def test_argument_errors(dev):
     bad(prefix_lens=c.prefix_d.long())
     bad(cu_seqlens=c.cu_d.long())
     bad(k=c.k[:-1], v=c.v[:-1])
+    if torch.cuda.device_count() > 1:                         # every tensor on q's device
+        bad(k=c.k.to("cuda:1"), v=c.v.to("cuda:1"))
+        bad(cu_seqlens=c.cu_d.to("cuda:1"))
+        bad(kv_pointers=c.table.to("cuda:1"))
 
 
 def test_workspace_reused_across_shapes(dev):

@@ -292,6 +292,10 @@ def test_argument_errors(dev):
     bad(max_prefix_len=c.n_blocks * 64)                                          # page table too short
     bad(kv_pointers=c.table[:, :, :1].contiguous())
     bad(k=c.k[:-1], v=c.v[:-1])                                                  # q / k / v cover different tokens
+    if torch.cuda.device_count() > 1:                                            # every tensor on q's device
+        bad(k=c.k.to("cuda:1"), v=c.v.to("cuda:1"))
+        bad(prefix_lens=c.prefix_d.to("cuda:1"))
+        bad(kv_pointers=c.table.to("cuda:1"))
     with pytest.raises(RuntimeError):                                            # append_at: start_pos on the host / of the wrong dtype
         backend.apply_bias_rope_update_kv_cache_at(c.qkv, c.lens_d, c.pad, c.prefix_d.cpu(), c.table, 4, 2, 20, 64, c.spt, D, ROPE, 8192, True, True, True)
     with pytest.raises(RuntimeError):
