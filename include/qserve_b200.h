@@ -293,6 +293,17 @@ QS_API int qs_kv_cache_compact(const int64_t* kv_pointers, const int32_t* start_
                                int batch, int num_nodes, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token,
                                int int4_kv_cache, void* stream);
 
+/* qs_kv_cache_fork: copy-on-write fork of cached prompts (SamplingParams.n / best_of: prefill once, decode n rows).  For every layer, K and V
+ *   and every pair p, with P = lens[parents[p]] (the parent's cached tokens): copies the bytes of slots 0 .. P % 64 - 1 (codes, scale and
+ *   zero of every KV head) of the parent's page at block P / 64 into the child's page at the same block index.  Nothing is copied when
+ *   P % 64 == 0 or block P / 64 lies outside the table.  The caller points the child's entries for blocks 0 .. P / 64 - 1 at the parent's
+ *   pages (shared, read-only from then on) before the call; the child's entry at block P / 64 must be its own page.  kv_pointers is
+ *   [num_layers, batch, 2, max_blocks_per_seq]; parents, children int32 [num_pairs] and lens int32 [batch] are device arrays, trusted (a child
+ *   must not be a parent or appear twice; rows in [0, batch)).  Pages 16-byte aligned.  Everything is read after the dependency wait.      */
+QS_API int qs_kv_cache_fork(const int64_t* kv_pointers, const int32_t* parents, const int32_t* children, const int32_t* lens, int num_layers,
+                            int batch, int num_pairs, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token,
+                            int int4_kv_cache, void* stream);
+
 /* Sampling on the GPU (the sampler's warpers and draw, and sampled acceptance of draft trees).
  *
  * Per row: temperature T (fp32), top_k (int32, -1 disables) and top_p (fp32), device arrays.  A row is GREEDY if T < 1e-5 or top_p < 1e-8,

@@ -636,6 +636,42 @@ def kv_cache_compact(kv_pointers, start_pos, path, accept_len, num_kv_heads: int
           kv_pointers.size(-1), int(num_kv_heads), int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)))
 
 
+def fork_pairs(parents, children, batch: int):
+    """The (parent, child) rows of a fork as two lists of ints, checked on the host: in [0, batch), equally long, no child twice, no row both
+    parent and child (its pages would be read and written by the same copy)."""
+    parents, children = [int(x) for x in parents], [int(x) for x in children]
+    _require(len(parents) == len(children), f"{len(parents)} parents but {len(children)} children")
+    _require(all(0 <= r < batch for r in parents + children), f"parent and child rows must lie in [0, {batch})")
+    _require(len(set(children)) == len(children), "a child row appears twice")
+    both = set(parents) & set(children)
+    _require(not both, f"rows {sorted(both)}: a parent row is also a child")
+    return parents, children
+
+
+def kv_cache_fork(kv_pointers, parents, children, lens, num_kv_heads: int, tokens_per_block: int, size_per_token: int, int4_kv_cache: bool) -> None:
+    """Copy-on-write fork of cached prompts (SamplingParams.n / best_of), every layer in one launch: for each pair (parents[p], children[p]) with
+    P = lens[parents[p]] cached tokens, the bytes of slots 0 .. P % 64 - 1 (codes, scale, zero; K and V; every KV head) of the parent's page at
+    block P // 64 are copied into the child's page at the same block index (nothing when P % 64 == 0).  The caller points the child's entries
+    for blocks 0 .. P // 64 - 1 at the parent's pages first; the child's entry at block P // 64 must be its own page.  kv_pointers int64
+    [L, B, 2, max_blocks] or [B, 2, max_blocks]; parents / children: host sequences of row indices (checked here: in [0, B), equally long, no
+    child twice, no row both parent and child); lens int32 [B] on the device (trusted)."""
+    _require(kv_pointers.dim() in (3, 4) and kv_pointers.size(-2) == 2, "kv_pointers must be int64 [L, B, 2, max_blocks] or [B, 2, max_blocks]")
+    L = kv_pointers.size(0) if kv_pointers.dim() == 4 else 1
+    B = kv_pointers.size(-3)
+    parents, children = fork_pairs(parents, children, B)
+    _tensor(kv_pointers, "kv_pointers", torch.int64)
+    dev = kv_pointers.device
+    _tensor(lens, "lens", torch.int32, (B,), dev)
+    _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
+    _require(int(num_kv_heads) >= 1 and int(size_per_token) == int(num_kv_heads) * 128 * (4 if int4_kv_cache else 8) // 8,
+             "size_per_token does not match the kv heads and the cache type")
+    if not parents or L == 0:
+        return
+    rows = torch.tensor(parents + children, dtype=torch.int32, device=dev)
+    _call(kv_pointers, lib.qs_kv_cache_fork, kv_pointers.data_ptr(), rows.data_ptr(), rows[len(parents):].data_ptr(), lens.data_ptr(), L, B, len(parents),
+          kv_pointers.size(-1), int(num_kv_heads), int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)))
+
+
 def _row_vec(v, n: int, dev, dt, name: str, ok, what: str) -> torch.Tensor:
     """A per-row parameter as a device tensor: a scalar broadcasts (and is checked on the host); a tensor is used as given (its values are
     trusted: checking them would synchronise with the device)."""

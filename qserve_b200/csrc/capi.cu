@@ -287,6 +287,15 @@ int qs_kv_cache_compact(const int64_t* kv_pointers, const int32_t* start_pos, co
   return kv_cache_compact(a);
 }
 
+int qs_kv_cache_fork(const int64_t* kv_pointers, const int32_t* parents, const int32_t* children, const int32_t* lens, int num_layers, int batch,
+                     int num_pairs, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token, int int4_kv_cache, void* stream) {
+  KvForkArgs a;
+  a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers); a.parents = parents; a.children = children; a.lens = lens;
+  a.layers = num_layers; a.batch = batch; a.num_pairs = num_pairs; a.max_blocks = max_blocks_per_seq; a.num_kv_heads = num_kv_heads;
+  a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token; a.int4_kv = int4_kv_cache; a.stream = stream;
+  return kv_cache_fork(a);
+}
+
 int qs_sample_rows(int64_t* out, const void* logits, const float* temperature, const int32_t* top_k, const float* top_p, uint64_t seed,
                    int64_t* offsets, int rows, int vocab, void* stream) {
   QS_REQUIRE(logits == nullptr || aligned16(logits), "sample_rows: logits must be 16-byte aligned");

@@ -175,6 +175,17 @@ struct KvCompactArgs {
 };
 int kv_cache_compact(const KvCompactArgs& a);
 
+// kv_fork.cu: copy-on-write fork of a cached prompt's partial tail page into other sequences (SamplingParams.n / best_of)
+struct KvForkArgs {
+  const long long* kv_pointers = nullptr;  // [layers, batch, 2, max_blocks] absolute page addresses
+  const int* parents = nullptr;            // [num_pairs] parent rows
+  const int* children = nullptr;           // [num_pairs] child rows
+  const int* lens = nullptr;               // [batch] cached tokens of each row (read at the parent rows)
+  int layers = 1, batch = 0, num_pairs = 0, max_blocks = 0, num_kv_heads = 0, tokens_per_block = 64, size_per_token = 0, int4_kv = 1;
+  void* stream = nullptr;
+};
+int kv_cache_fork(const KvForkArgs& a);
+
 // sampling.cu: temperature / top-p / top-k sampling of fp16 logits and sampled (lossless) acceptance of draft trees; Philox4x32-10 draws
 // keyed by `seed` and counted by the per-row `offsets`, which every call advances by one
 struct SampleArgs {

@@ -103,11 +103,34 @@ class _Rows(NamedTuple):
     q_sum: torch.Tensor     # fp16 [M]
 
 
+def prompt_pieces(lens, ctx: int, prompt_tokens: int, chunk: Optional[int] = None) -> list:
+    """The pieces of a prompt step (DecodeRunner.prefill), planned on the host: lens (ints, one prompt length per row) -> [(start, [tokens
+    of each row in this piece])].  chunk=None: one piece (0, lens).  chunk=C: piece k starts at k C and row b takes min(C, lens[b] - k C)
+    tokens (0 once its prompt is done).  Raises RuntimeError if a length lies outside [1, ctx], chunk < 1 or a piece holds more than
+    prompt_tokens tokens."""
+    lens = [int(x) for x in lens]
+    if not lens or min(lens) < 1 or max(lens) > ctx:
+        raise RuntimeError(f"prompt lengths must lie in [1, ctx={ctx}], got {lens}")
+    if chunk is not None and int(chunk) < 1:
+        raise RuntimeError(f"chunk={chunk}: a piece takes at least one token per row")
+    C = max(lens) if chunk is None else int(chunk)
+    pieces = []
+    for start in range(0, max(lens), C):
+        c = [min(C, max(n - start, 0)) for n in lens]
+        if sum(c) > prompt_tokens:
+            raise RuntimeError(f"a prompt piece of {sum(c)} tokens exceeds prompt_tokens={prompt_tokens}: construct a larger runner or pass a smaller chunk")
+        pieces.append((start, c))
+    return pieces
+
+
+_PROMPT_LOGITS_BYTES = 64 << 20  # prompt_logprobs: fp16 logits of at most this many bytes exist at once
+
+
 class DecodeRunner:
     def __init__(self, model: str = "llama-3-8b", precision: str = "w4a8kv4", batch: int = 64, ctx: int = 1024,
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
-                 verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False):
+                 verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False, prompt_tokens: int = 0):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
         ctx + verify_len tokens and the activation buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers
         and its random draws exactly as they are without it.
@@ -123,8 +146,14 @@ class DecodeRunner:
         every row by what it accepted.  The history is [batch, ctx + 1 + T] (the prompt is ctx cached tokens and the root), the page tables
         cover ctx + T + max(1, verify_len) tokens (the pages past blocks_per_seq come from zero-filled pools made after every random draw, so
         the weights and the first blocks_per_seq pages of each row are those of generate=False), and the per-row state is g_budget (tokens a
-        row may generate, default T), g_eos (-1: none) and g_finished."""
+        row may generate, default T), g_eos (-1: none) and g_finished.
+
+        prompt_tokens > 0 (single GPU, fused path) adds the prompt step (`prefill`): at most prompt_tokens prompt tokens per piece, so the
+        activation buffers hold max(batch * max(1, verify_len), prompt_tokens) rows.  It makes no generator draws: the weights, pages and
+        decode / verify / generate steps are those of prompt_tokens = 0."""
         assert precision in PRECISIONS, precision
+        assert prompt_tokens >= 0 and (prompt_tokens == 0 or (tp_size == 1 and fused)), "the prompt step is single-GPU and uses the fused path"
+        self.prompt_tokens = prompt_tokens
         assert 0 <= verify_len <= 16, "verify_len: at most 16 draft tokens per sequence"
         assert verify_len == 0 or (tp_size == 1 and fused), "the verify step is single-GPU and uses the fused path"
         assert max_new_tokens == 0 or 0 < ctx + max_new_tokens <= _ext.MAX_PENALTY_HISTORY, "the token history holds at most 32768 tokens per row"
@@ -212,6 +241,7 @@ class DecodeRunner:
                     more = torch.stack([kp.data_ptr() + blk * self.page_bytes, vp.data_ptr() + blk * self.page_bytes], dim=1)
                     tables[li] = torch.cat([tables[li], more], dim=2)
         self.block_tables = torch.stack(tables, dim=0).contiguous()  # [L, B, 2, blocks]
+        self.own_tables = self.block_tables.clone()  # every row's own pages: fork() shares a parent's pages, prefill() restores these
         self.context_lens = torch.full((batch,), ctx + 1, dtype=torch.int32, device=dev)
         # host bounds of the attention launches: in generation the contexts grow up to ctx + 1 + max_new_tokens
         self.max_seq_len = ctx + 1 + (max_new_tokens if generate else 0)
@@ -219,7 +249,7 @@ class DecodeRunner:
 
         # ---- persistent ActivationBuffer (input_metadata.py:71-109; aliasing kept) for the rows of the widest step --------------------
         # (H is in the max for tensor parallelism: at TP = 8 a 72B model's sharded qkv / gate_up rows are narrower than the full hidden row of out_buf)
-        R = M * max(1, verify_len)
+        R = max(M * max(1, verify_len), prompt_tokens)
         self.act_buffer = torch.empty(R * max(self.q_size + 2 * self.kv_size, 2 * self.Iloc, H), dtype=torch.half, device=dev)
         self.q_act = torch.empty(R * max(H, self.Iloc), dtype=torch.int8, device=dev)
         self.scale_buffer = torch.empty(R, dtype=torch.half, device=dev)
@@ -245,6 +275,7 @@ class DecodeRunner:
         self.s_top_k = torch.full((batch,), 1, dtype=torch.int32, device=dev)
         self.s_top_p = torch.full((batch,), 1.0, dtype=torch.float32, device=dev)
         self.s_offsets = torch.full((batch,), 0, dtype=torch.int64, device=dev)
+        self._p_logprob = None  # prompt_logprobs outputs, allocated by the first prefill that asks for them
         self.max_new_tokens = max_new_tokens
         if max_new_tokens:
             self._alloc_penalty_buffers()
@@ -635,6 +666,166 @@ class DecodeRunner:
     def generate_step(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False) -> None:
         """Replay the captured generation step."""
         self.graphs[self._generate_key(n, branches, ngram, sampled)].replay()
+
+    # ---------------------------------------------------------------------------------------------------------
+    # prompt step: prefill every row's prompt into its pages, whole or in chunks, then the first token and the hand-off to generation
+    # ---------------------------------------------------------------------------------------------------------
+    def prefill(self, prompts: torch.Tensor, lens: torch.Tensor, chunk: Optional[int] = None, sample: bool = False, penalties: bool = False,
+                logprobs: int = 0, prompt_logprobs: int = 0) -> torch.Tensor:
+        """Prefill prompts int64 [batch, >= max(lens)] with lens int32 [batch] (1 <= lens[b] <= ctx) into positions 0 .. lens[b] - 1 of every
+        row's pages in every layer; returns the first tokens int64 [batch].  Eager, one host synchronisation (the lengths plan the pieces).
+
+        Per layer: the qkv GEMM at M = the piece's tokens, then chunk=None: apply_bias_rope_update_kv_cache and flash_attn_varlen_func over
+        the whole prompts (llama_w4a8_unpad.py:199-242); chunk=C: pieces of at most C tokens per row, each appended with
+        apply_bias_rope_update_kv_cache_at at the row's cached length and attended with prefix_prefill_attention over the dequantised prefix
+        (rows whose prompt is done take 0 tokens); then invoke_quant[_fuse_sum], o, gate_up, silu+quant and down as the fused decode step.
+        A piece holds at most prompt_tokens tokens.  Only each row's last position goes through the final norm and lm_head (:471-475); the
+        first token then comes out of the composition of forward (sample, penalties, logprobs as there; penalties see the prompt only).
+
+        prompt_logprobs = n (1 .. 20): p_logprob fp32, p_top_ids int64 [., n] and p_top_logprobs fp32 [., n], flat over the prompts by
+        cu_seqlens = [0, lens[0], lens[0] + lens[1], ...]: entry cu[b] + i (i >= 1) is the log-probability of prompt token i given tokens
+        0 .. i - 1 and the top n there (logprobs_rows of the unpenalised logits); entry cu[b] (the first token) is NaN with top ids -1.  The
+        lm_head runs over blocks of prompt rows, never over all of them at once.
+
+        Hand-off: the block tables get every row's own pages back (undoing fork), context_lens = lens + 1, tokens_in = the first token, and
+        v_start / g_start = lens where they exist.  With max_new_tokens > 0: s_history[b] = the prompt, the first token at lens[b], then -1;
+        s_prompt_lens = lens and s_seq_lens = lens + 1 (the first token counts as generated).  With generate=True, g_finished[b] = 1 when the
+        first token is g_eos[b] or g_budget[b] <= 1; generate_forward continues from there."""
+        assert self.prompt_tokens, "construct the runner with prompt_tokens > 0"
+        assert self.max_new_tokens or not (penalties or logprobs), "construct the runner with max_new_tokens > 0 for penalties / logprobs"
+        B, cfg, dev = self.batch, self.cfg, self.dev
+        if not (lens.dtype == torch.int32 and tuple(lens.shape) == (B,)):
+            raise RuntimeError(f"lens must be int32 [{B}], got {lens.dtype} {tuple(lens.shape)}")
+        lens_h = [int(x) for x in lens.tolist()]
+        pieces = prompt_pieces(lens_h, self.ctx, self.prompt_tokens, chunk)
+        if not (prompts.dtype == torch.int64 and prompts.dim() == 2 and prompts.size(0) == B and prompts.size(1) >= max(lens_h)):
+            raise RuntimeError(f"prompts must be int64 [{B}, >= {max(lens_h)}], got {prompts.dtype} {tuple(prompts.shape)}")
+        if not 0 <= int(prompt_logprobs) <= _ext.MAX_TOP_LOGPROBS:
+            raise RuntimeError(f"prompt_logprobs={prompt_logprobs}: 0 .. {_ext.MAX_TOP_LOGPROBS}")
+        prompts, lens = prompts.to(dev), lens.to(dev)
+        cu_all = [0]
+        for n in lens_h:
+            cu_all.append(cu_all[-1] + n)
+        if prompt_logprobs:
+            self._alloc_prompt_logprobs(cu_all, int(prompt_logprobs))
+        self.block_tables.copy_(self.own_tables)
+        D, int4, max_pos = cfg.head_dim, self.kv_bits == 4, min(8192, cfg.max_pos)
+        last = torch.empty((B, cfg.hidden), dtype=torch.half, device=dev)
+        i32 = lambda v: torch.tensor(v, dtype=torch.int32, device=dev)
+        for start, c in pieces:
+            T, maxc = sum(c), max(c)
+            cu_h = [0]
+            for n in c:
+                cu_h.append(cu_h[-1] + n)
+            rows = [b for b in range(B) for _ in range(c[b])]
+            cols = [start + j for b in range(B) for j in range(c[b])]
+            tokens = prompts[torch.tensor(rows, device=dev), torch.tensor(cols, device=dev)]
+            cu, clens = i32(cu_h), i32(c)
+            pad = _ext.compute_padding_offsets(cu, maxc, T)
+            if chunk is None:
+                def attention(li, r):  # llama_w4a8_unpad.py:199-243
+                    _ext.apply_bias_rope_update_kv_cache(r.qkv, clens, pad, self.block_tables[li], self.Hq, self.Hkv, maxc, 64, self.size_per_token, D,
+                                                         cfg.rope_theta, max_pos, True, int4, True)
+                    attn = _ext.flash_attn_varlen_func(*self._heads(r.qkv), cu_seqlens_q=cu, cu_seqlens_k=cu, max_seqlen_q=maxc, max_seqlen_k=maxc,
+                                                       dropout_p=0.0, causal=True)
+                    self._quant(r, r.q_attn, attn.view(T, -1))
+            else:
+                prefix = i32([min(n, start) for n in lens_h])
+
+                def attention(li, r):
+                    table = self.block_tables[li]
+                    _ext.apply_bias_rope_update_kv_cache_at(r.qkv, clens, pad, prefix, table, self.Hq, self.Hkv, maxc, 64, self.size_per_token, D,
+                                                            cfg.rope_theta, max_pos, True, int4, True)
+                    attn = _ext.prefix_prefill_attention(*self._heads(r.qkv), cu, maxc, prefix, start, table, 64, self.size_per_token, int4)
+                    self._quant(r, r.q_attn, attn.view(T, -1))
+
+            hidden, _ = self._fused_layers(self.embed[tokens], self._row_views(T), attention)
+            done = [b for b in range(B) if c[b] and start + c[b] == lens_h[b]]
+            if done:
+                last[torch.tensor(done, device=dev)] = hidden[torch.tensor([cu_h[b + 1] - 1 for b in done], device=dev)]
+            if prompt_logprobs:
+                self._prompt_logprobs(hidden, prompts, start, c, cu_h, cu_all, int(prompt_logprobs))
+        self.last_prompt_hidden = last
+        logits = self._logits(last)
+        self.last_logits = logits
+        if self.max_new_tokens:
+            W = self.s_history.size(1)
+            w = min(W, prompts.size(1))
+            hist = torch.full((B, W), -1, dtype=torch.int64, device=dev)
+            hist[:, :w] = prompts[:, :w]
+            self.s_history.copy_(torch.where(torch.arange(W, device=dev) < lens.unsqueeze(1), hist, -1))
+            self.s_prompt_lens.copy_(lens)
+            self.s_seq_lens.copy_(lens)
+        tok = self._next_tokens(logits, sample, penalties, logprobs, out=self.tokens_out)
+        if self.max_new_tokens and not (penalties or logprobs):  # _next_tokens appends only when it penalises or scores
+            self.s_history.scatter_(1, self.s_seq_lens.long().unsqueeze(1), tok.unsqueeze(1))
+            self.s_seq_lens.add_(1)
+        self.context_lens.copy_(lens + 1)
+        if self.verify_len:
+            self.v_start.copy_(lens)
+        if self.generate:
+            self.g_start.copy_(lens)
+            self.g_finished.copy_(((tok == self.g_eos) | (self.g_budget <= 1)).to(torch.int32))
+        self.tokens_in.copy_(tok)
+        return tok.clone()
+
+    def _alloc_prompt_logprobs(self, cu_all: list, n: int) -> None:
+        """p_logprob / p_top_ids / p_top_logprobs as views of buffers grown to the prompts of cu_all, the first entry of every prompt NaN / -1."""
+        total = cu_all[-1]
+        if self._p_logprob is None or self._p_logprob.numel() < total:
+            self._p_logprob = torch.zeros(total, dtype=torch.float32, device=self.dev)
+            self._p_top_ids = torch.zeros(total * _ext.MAX_TOP_LOGPROBS, dtype=torch.int64, device=self.dev)
+            self._p_top_logprobs = torch.zeros(total * _ext.MAX_TOP_LOGPROBS, dtype=torch.float32, device=self.dev)
+        self.p_logprob = self._p_logprob[:total]
+        self.p_top_ids = self._p_top_ids[: total * n].view(total, n)
+        self.p_top_logprobs = self._p_top_logprobs[: total * n].view(total, n)
+        first = torch.tensor(cu_all[:-1], device=self.dev)
+        self.p_logprob[first] = float("nan")
+        self.p_top_ids[first] = -1
+        self.p_top_logprobs[first] = float("nan")
+
+    def _prompt_logprobs(self, hidden, prompts, start: int, c: list, cu_h: list, cu_all: list, n: int) -> None:
+        """The prompt log-probabilities the rows of one piece give: position start + j of row b (hidden row cu_h[b] + j) scores prompt
+        token start + j + 1, written at cu_all[b] + start + j + 1; the lm_head runs over blocks of rows."""
+        # (hidden row, output entry, row, position of the scored token) of every position but each prompt's last
+        m = [(cu_h[b] + j, cu_all[b] + start + j + 1, b, start + j + 1) for b in range(self.batch) for j in range(c[b])
+             if start + j + 1 < cu_all[b + 1] - cu_all[b]]
+        if not m:
+            return
+        src, dst, row, pos = torch.tensor(m, device=self.dev).unbind(1)
+        targets = prompts[row, pos]
+        rows = max(1, _PROMPT_LOGITS_BYTES // (2 * self.cfg.vocab))
+        for i in range(0, src.numel(), rows):
+            logits = self._logits(hidden[src[i:i + rows]])
+            lp, ids, tlp = _ext.logprobs_rows(logits, targets[i:i + rows].contiguous(), n)
+            d = dst[i:i + rows]
+            self.p_logprob[d] = lp
+            self.p_top_ids[d] = ids
+            self.p_top_logprobs[d] = tlp
+
+    def fork(self, parent_rows, child_rows) -> None:
+        """Copy-on-write fork between steps (SamplingParams.n / best_of: prefill a prompt once, decode n rows from it).  parent_rows: one row or
+        one per child; child_rows: rows that are not parents.  With P = the parent's cached tokens (context_lens - 1): in every layer the child's
+        block-table entries 0 .. P // 64 - 1 point at the parent's pages (shared and read-only from then on: a child writes only at positions
+        >= P), the rest at the child's own pages; kv_cache_fork copies the parent's partial tail page into the child's own page; the child
+        gets the parent's history, s_prompt_lens, s_seq_lens, context_lens, g_start / v_start, tokens_in, g_budget, g_eos, g_finished and
+        penalty parameters.  s_offsets and the sampling parameters stay the child's own, so sampled children diverge.  Eager; the table
+        entries are written with torch ops (the attention kernels read the tables before their dependency wait)."""
+        children = list(child_rows) if not isinstance(child_rows, int) else [child_rows]
+        parents = [parent_rows] * len(children) if isinstance(parent_rows, int) else list(parent_rows)
+        parents, children = _ext.fork_pairs(parents, children, self.batch)
+        if not children:
+            return
+        dev = self.dev
+        par, chi = torch.tensor(parents, device=dev), torch.tensor(children, device=dev)
+        cached = (self.context_lens - 1).contiguous()
+        shared = torch.arange(self.table_blocks, device=dev).unsqueeze(0) < (cached[par] // 64).unsqueeze(1)  # [pairs, blocks]
+        self.block_tables[:, chi] = torch.where(shared[None, :, None, :], self.block_tables[:, par], self.own_tables[:, chi])
+        _ext.kv_cache_fork(self.block_tables, parents, children, cached, self.Hkv, 64, self.size_per_token, self.kv_bits == 4)
+        names = ["context_lens", "tokens_in", "s_history", "s_prompt_lens", "s_seq_lens", "s_repetition", "s_presence", "s_frequency", "v_start",
+                 "g_start", "g_budget", "g_eos", "g_finished"]
+        for t in {id(getattr(self, a)): getattr(self, a) for a in names if hasattr(self, a)}.values():  # g_start may alias v_start
+            t[chi] = t[par]
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
