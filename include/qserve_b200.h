@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define QS_ABI_VERSION 1
+#define QS_ABI_VERSION 2
 #if defined(__GNUC__)
 #define QS_API __attribute__((visibility("default")))
 #else
@@ -354,6 +354,30 @@ QS_API int qs_apply_penalties(void* logits, const int64_t* history, const int32_
 QS_API int qs_logprobs_rows(float* logprob, int64_t* top_ids, float* top_logprobs, const void* logits, const int64_t* tokens, int rows, int vocab,
                             int n, void* stream);
 
+/* The same penalties and log-probabilities inside a speculative step (same conventions as above).
+ *
+ * qs_apply_penalties_tree: fp16 verify logits [batch, num_nodes, vocab] of a draft tree (num_nodes <= 16; draft_tokens int64 and tree_mask
+ *   int32 [batch, num_nodes], the ancestor words of qs_tree_decode_attention), modified in place before acceptance.  Row b's history follows
+ *   the generation loop: h[0 .. L) with L = seq_lens[b] (clamped to [0, history_len]), h[L - 1] is the root, node 0.  Node i's row is, bit for
+ *   bit, what qs_apply_penalties writes for that row given the EXPANDED history: h[0 .. L), then the tokens of node i's ancestors j >= 1 (bits
+ *   of tree_mask[b, i] below i) in index order, then node i's own token if i >= 1, with the row's prompt_len and parameters.  The expanded
+ *   history is not clipped at history_len.  Ids outside [0, vocab) (-1: padding nodes) are ignored; neutral rows and NaN logits are not
+ *   written; each (node, token) is written once at most (no atomics).  history_len <= 32768.
+ * qs_logprobs_accepted: the log-probabilities of the tokens a speculative step emits, before qs_spec_commit[_stops] commits them.  For every
+ *   unfinished row (finished[b] == 0) with acc = accept_len[b] clamped to [1, num_nodes] (path entries to [0, num_nodes - 1], as the commit
+ *   clamps them): emitted token k < acc (draft_tokens[b, path[b, k + 1]] for k < acc - 1, else bonus[b]) is scored by node row path[b, k] of
+ *   logits fp16 [batch, num_nodes, vocab] with exactly the qs_logprobs_rows arithmetic, and written at column c = min(max(seq_lens[b], 0),
+ *   width) + k of logprob fp32 [batch, width] and top_ids int64 / top_logprobs fp32 [batch, width, n] (n <= 20; NULL when n = 0): the column
+ *   where the commit puts the token.  Columns >= width are dropped; finished rows and tokens past acc write nothing.  After the commit,
+ *   column c is valid for prompt_lens[b] <= c < seq_lens[b]; entries of tokens the commit cut (eos, a stop token, the budget) are
+ *   unspecified.  A plain decode step is the call with num_nodes = 1, path = 0, accept_len = 1 and bonus = its token.                     */
+QS_API int qs_apply_penalties_tree(void* logits, const int64_t* draft_tokens, const int32_t* tree_mask, const int64_t* history,
+                                   const int32_t* prompt_lens, const int32_t* seq_lens, const float* repetition, const float* presence,
+                                   const float* frequency, int batch, int num_nodes, int vocab, int history_len, void* stream);
+QS_API int qs_logprobs_accepted(float* logprob, int64_t* top_ids, float* top_logprobs, const void* logits, const int64_t* draft_tokens,
+                                const int32_t* path, const int32_t* accept_len, const int64_t* bonus, const int32_t* seq_lens,
+                                const int32_t* finished, int batch, int num_nodes, int vocab, int n, int width, void* stream);
+
 /* Prompt-lookup speculative decoding: the drafter and the commit that close the loop around the tree verify and acceptance above.  Both read
  * every input after the PDL dependency wait (the previous step's commit writes the history and the lengths), need no host synchronisation,
  * are CUDA-graph capturable and bitwise deterministic.  Row state: history int64 [batch, history_len] holds the prompt and the generated
@@ -381,6 +405,13 @@ QS_API int qs_ngram_propose(const int64_t* history, const int32_t* seq_lens, int
 QS_API int qs_spec_commit(const int64_t* draft_tokens, const int32_t* path, const int32_t* accept_len, const int64_t* bonus, int64_t* history,
                           int32_t* seq_lens, const int32_t* prompt_lens, const int32_t* budget, const int64_t* eos, int32_t* finished,
                           int32_t* start_pos, int32_t* context_lens, int64_t* roots, int batch, int num_nodes, int history_len, void* stream);
+/* qs_spec_commit_stops: qs_spec_commit with a stop-token set per row, stop_ids int64 [batch, num_stops] (num_stops <= 8, entries < 0 pad):
+ *   the first appended token in {eos[b]} or the row's set ends the row exactly as eos does (appended, the cut after it, finished; the
+ *   budget cut still wins).  stop_ids may be NULL when num_stops = 0, which gives exactly qs_spec_commit.                                */
+QS_API int qs_spec_commit_stops(const int64_t* draft_tokens, const int32_t* path, const int32_t* accept_len, const int64_t* bonus,
+                                int64_t* history, int32_t* seq_lens, const int32_t* prompt_lens, const int32_t* budget, const int64_t* eos,
+                                const int64_t* stop_ids, int num_stops, int32_t* finished, int32_t* start_pos, int32_t* context_lens,
+                                int64_t* roots, int batch, int num_nodes, int history_len, void* stream);
 
 #ifdef __cplusplus
 }

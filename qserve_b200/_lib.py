@@ -45,8 +45,11 @@ SIGNATURES = {
     "qs_tree_accept_sampling": (c_int, [_P, _P, _P, _P, _P, _P, _P, ctypes.c_uint64, _P, _P, _P, _P, _I, _I, _I, _P]),
     "qs_apply_penalties": (c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "qs_logprobs_rows": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "qs_apply_penalties_tree": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "qs_logprobs_accepted": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "qs_ngram_propose": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "qs_spec_commit": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "qs_spec_commit_stops": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _I, _I, _I, _P]),
     "qs_rms_norm": (c_int, [_P, _P, _P, _F, _I, _I, _I, _P]),
     "qs_rms_norm_general": (c_int, [_P, _P, _P, _P, _F, _I, _I, _I, _P]),
     "qs_rms_norm_general_fuse_sum": (c_int, [_P, _P, _P, _P, _P, _F, _I, _I, _I, _P]),
@@ -67,7 +70,7 @@ SIGNATURES = {
     "qs_dequant_silu_and_mul_quant": (c_int, [_P, _P, _F, _F, _F, _P, _P, _I, _I, _P]),
 }
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 
 def _load() -> ctypes.CDLL:

@@ -802,6 +802,66 @@ def logprobs_rows(logits, tokens, n: int, logprob: Optional[torch.Tensor] = None
     return logprob, top_ids, top_logprobs
 
 
+def apply_penalties_tree(logits, draft_tokens, tree_mask, history, prompt_lens, seq_lens, repetition, presence, frequency) -> torch.Tensor:
+    """apply_penalties on every node row of a draft tree, in place on the verify logits fp16 [B, n, V] before greedy or sampled acceptance;
+    returns logits.  draft_tokens int64 [B, n] and tree_mask int32 [B, n] as ngram_propose returns them (n <= 16).  Row b's history follows
+    the generation loop: h[0 .. L) with L = seq_lens[b], h[L - 1] the root (node 0).  Node i's row is, bit for bit, what apply_penalties
+    writes for it given the expanded history h[0 .. L), the tokens of node i's ancestors j >= 1 in index order, node i's own token (i >= 1),
+    with the row's prompt_lens and parameters; the expanded history is not clipped at H.  So node i's row is the distribution the sequential
+    step at that position samples from, and greedy or sampled acceptance stays exact under penalties.  Other arguments and rules as
+    apply_penalties (history int64 [B, H], H <= 32768).  See include/qserve_b200.h."""
+    B, n = _tensor(draft_tokens, "draft_tokens", torch.int64, (None, None)).shape
+    dev = draft_tokens.device
+    _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
+    _tensor(tree_mask, "tree_mask", torch.int32, (B, n), dev)
+    V = _tensor(logits, "logits", _HALF, (B, n, None), dev).size(2)
+    _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
+    H = _tensor(history, "history", torch.int64, (B, None), dev).size(1)
+    _require(H <= MAX_PENALTY_HISTORY, f"history of {H} tokens per row: at most {MAX_PENALTY_HISTORY}")
+    _tensor(prompt_lens, "prompt_lens", torch.int32, (B,), dev)
+    _tensor(seq_lens, "seq_lens", torch.int32, (B,), dev)
+    R = _row_vec(repetition, B, dev, torch.float32, "repetition", lambda v: 0 < float(v) <= 2, "must lie in (0, 2]")
+    P = _row_vec(presence, B, dev, torch.float32, "presence", lambda v: -2 <= float(v) <= 2, "must lie in [-2, 2]")
+    F = _row_vec(frequency, B, dev, torch.float32, "frequency", lambda v: -2 <= float(v) <= 2, "must lie in [-2, 2]")
+    if B:
+        _call(logits, lib.qs_apply_penalties_tree, logits.data_ptr(), draft_tokens.data_ptr(), tree_mask.data_ptr(), history.data_ptr(),
+              prompt_lens.data_ptr(), seq_lens.data_ptr(), R.data_ptr(), P.data_ptr(), F.data_ptr(), B, n, V, H)
+    return logits
+
+
+def logprobs_accepted(logits, draft_tokens, path, accept_len, bonus, seq_lens, finished, n_top: int, logprob, top_ids: Optional[torch.Tensor] = None,
+                      top_logprobs: Optional[torch.Tensor] = None) -> None:
+    """Log-probabilities of the tokens a speculative step emits, in history columns, in place and before spec_commit commits them.  For every
+    unfinished row (finished int32 [B] == 0) with acc = accept_len[b] clamped to [1, n] as spec_commit clamps it: emitted token k < acc
+    (draft_tokens[b, path[b, k + 1]] for k < acc - 1, else bonus[b]) is scored by node row path[b, k] of logits fp16 [B, n, V] with exactly
+    the logprobs_rows arithmetic and written at column seq_lens[b] + k (seq_lens int32 [B] before the commit: where spec_commit puts the
+    token) of logprob fp32 [B, W] and, for 1 <= n_top <= 20, top_ids int64 / top_logprobs fp32 [B, W, n_top].  Columns >= W are dropped;
+    finished rows and tokens past acc are not written.  After the commit, column c holds the entry of history token c for
+    prompt_lens[b] <= c < seq_lens[b]; entries of tokens the commit cut are unspecified.  A plain step passes n = 1, path = 0, accept_len = 1
+    and bonus = its token.  See include/qserve_b200.h."""
+    B, n = _tensor(draft_tokens, "draft_tokens", torch.int64, (None, None)).shape
+    dev = draft_tokens.device
+    _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
+    n_top = int(n_top)
+    _require(0 <= n_top <= MAX_TOP_LOGPROBS, f"n_top={n_top}: 0 .. {MAX_TOP_LOGPROBS} top log-probabilities")
+    V = _tensor(logits, "logits", _HALF, (B, n, None), dev).size(2)
+    _require(V % 8 == 0 and 8 <= V <= 196608, f"vocab={V}: a multiple of 8 up to 196608")
+    _tensor(path, "path", torch.int32, (B, n), dev)
+    for t, nm, dt in ((accept_len, "accept_len", torch.int32), (bonus, "bonus", torch.int64), (seq_lens, "seq_lens", torch.int32),
+                      (finished, "finished", torch.int32)):
+        _tensor(t, nm, dt, (B,), dev)
+    W = _tensor(logprob, "logprob", torch.float32, (B, None), dev).size(1)
+    _require(W >= 1, "logprob must have at least one column")
+    if n_top:
+        _require(top_ids is not None and top_logprobs is not None, f"n_top={n_top} needs top_ids and top_logprobs")
+        _tensor(top_ids, "top_ids", torch.int64, (B, W, n_top), dev)
+        _tensor(top_logprobs, "top_logprobs", torch.float32, (B, W, n_top), dev)
+    if B:
+        _call(logits, lib.qs_logprobs_accepted, logprob.data_ptr(), _ptr(top_ids if n_top else None), _ptr(top_logprobs if n_top else None),
+              logits.data_ptr(), draft_tokens.data_ptr(), path.data_ptr(), accept_len.data_ptr(), bonus.data_ptr(), seq_lens.data_ptr(),
+              finished.data_ptr(), B, n, V, n_top, W)
+
+
 MAX_DRAFT_NGRAM = 8
 MAX_DRAFT_BRANCHES = 8
 
@@ -832,8 +892,11 @@ def ngram_propose(history, seq_lens, num_nodes: int, n_min: int = 1, n_max: int 
     return tokens, tree_mask
 
 
+MAX_STOP_TOKENS = 8  # stop tokens per row besides eos
+
+
 def spec_commit(draft_tokens, path, accept_len, bonus, history, seq_lens, prompt_lens, budget, eos, finished, start_pos,
-                context_lens: Optional[torch.Tensor] = None, roots: Optional[torch.Tensor] = None) -> None:
+                context_lens: Optional[torch.Tensor] = None, roots: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None) -> None:
     """Advance every unfinished row by what its speculative step accepted, in place and without host synchronisation: the tokens
     draft_tokens[b, path[b, 1 .. acc - 1]] and bonus[b] (acc = accept_len[b]; draft_tokens int64 [B, n], path int32 [B, n], accept_len int32 [B]
     and bonus int64 [B] as tree_accept_greedy / tree_accept_sampling return them) are cut after the first eos[b] (int64 [B], -1: none), then
@@ -841,7 +904,9 @@ def spec_commit(draft_tokens, path, accept_len, bonus, history, seq_lens, prompt
     seq_lens advances by the count.  start_pos (int32 [B]) = L - 1, the optional context_lens (int32 [B]) = L and roots (int64 [B]) = the last
     token: what the next verify step (start_pos) or decode step (context_lens, tokens = roots) reads.  finished int32 [B] is set when a row
     appends eos or reaches its budget; finished rows are left untouched.  A plain decode step commits with n = 1, path = 0, accept_len = 1 and
-    bonus = its token.  See include/qserve_b200.h."""
+    bonus = its token.  stop_ids int64 [B, S] (S <= 8, -1 pads; SamplingParams.stop_token_ids): any token of {eos[b]} and stop_ids[b] ends
+    the row as eos does (appended, cut after, finished; the budget cut still wins), in the qs_spec_commit_stops launch.  See
+    include/qserve_b200.h."""
     B, n = _tensor(draft_tokens, "draft_tokens", torch.int64, (None, None)).shape
     _require(1 <= n <= 16, "a draft tree has 1 .. 16 nodes per sequence")
     dev = draft_tokens.device
@@ -855,10 +920,19 @@ def spec_commit(draft_tokens, path, accept_len, bonus, history, seq_lens, prompt
     for t, nm, dt in ((context_lens, "context_lens", torch.int32), (roots, "roots", torch.int64)):
         if t is not None:
             _tensor(t, nm, dt, (B,), dev)
-    if B:
+    if stop_ids is not None:
+        S = _tensor(stop_ids, "stop_ids", torch.int64, (B, None), dev).size(1)
+        _require(S <= MAX_STOP_TOKENS, f"{S} stop tokens per row: at most {MAX_STOP_TOKENS}")
+    if not B:
+        return
+    if stop_ids is None:
         _call(history, lib.qs_spec_commit, draft_tokens.data_ptr(), path.data_ptr(), accept_len.data_ptr(), bonus.data_ptr(), history.data_ptr(),
               seq_lens.data_ptr(), prompt_lens.data_ptr(), budget.data_ptr(), eos.data_ptr(), finished.data_ptr(), start_pos.data_ptr(),
               _ptr(context_lens), _ptr(roots), B, n, H)
+    else:
+        _call(history, lib.qs_spec_commit_stops, draft_tokens.data_ptr(), path.data_ptr(), accept_len.data_ptr(), bonus.data_ptr(),
+              history.data_ptr(), seq_lens.data_ptr(), prompt_lens.data_ptr(), budget.data_ptr(), eos.data_ptr(), _ptr(stop_ids if S else None), S,
+              finished.data_ptr(), start_pos.data_ptr(), _ptr(context_lens), _ptr(roots), B, n, H)
 
 
 class PeerContext:

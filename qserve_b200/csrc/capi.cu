@@ -355,6 +355,41 @@ int qs_spec_commit(const int64_t* draft_tokens, const int32_t* path, const int32
   return spec_commit(a);
 }
 
+int qs_spec_commit_stops(const int64_t* draft_tokens, const int32_t* path, const int32_t* accept_len, const int64_t* bonus, int64_t* history,
+                         int32_t* seq_lens, const int32_t* prompt_lens, const int32_t* budget, const int64_t* eos, const int64_t* stop_ids,
+                         int num_stops, int32_t* finished, int32_t* start_pos, int32_t* context_lens, int64_t* roots, int batch, int num_nodes,
+                         int history_len, void* stream) {
+  SpecCommitArgs a;
+  a.draft = reinterpret_cast<const long long*>(draft_tokens); a.path = path; a.accept_len = accept_len; a.bonus = reinterpret_cast<const long long*>(bonus);
+  a.history = reinterpret_cast<long long*>(history); a.seq_lens = seq_lens; a.prompt_lens = prompt_lens; a.budget = budget;
+  a.eos = reinterpret_cast<const long long*>(eos); a.finished = finished; a.start_pos = start_pos; a.context_lens = context_lens;
+  a.roots = reinterpret_cast<long long*>(roots); a.batch = batch; a.num_nodes = num_nodes; a.history_len = history_len; a.stream = stream;
+  return spec_commit_stops(a, reinterpret_cast<const long long*>(stop_ids), num_stops);
+}
+
+int qs_apply_penalties_tree(void* logits, const int64_t* draft_tokens, const int32_t* tree_mask, const int64_t* history, const int32_t* prompt_lens,
+                            const int32_t* seq_lens, const float* repetition, const float* presence, const float* frequency, int batch, int num_nodes,
+                            int vocab, int history_len, void* stream) {
+  PenaltyTreeArgs a;
+  a.logits = logits; a.draft = reinterpret_cast<const long long*>(draft_tokens); a.tree_mask = tree_mask;
+  a.history = reinterpret_cast<const long long*>(history); a.prompt_lens = prompt_lens; a.seq_lens = seq_lens; a.repetition = repetition;
+  a.presence = presence; a.frequency = frequency; a.batch = batch; a.num_nodes = num_nodes; a.vocab = vocab; a.history_len = history_len;
+  a.stream = stream;
+  return apply_penalties_tree(a);
+}
+
+int qs_logprobs_accepted(float* logprob, int64_t* top_ids, float* top_logprobs, const void* logits, const int64_t* draft_tokens, const int32_t* path,
+                         const int32_t* accept_len, const int64_t* bonus, const int32_t* seq_lens, const int32_t* finished, int batch, int num_nodes,
+                         int vocab, int n, int width, void* stream) {
+  QS_REQUIRE(logits == nullptr || aligned16(logits), "logprobs_accepted: logits must be 16-byte aligned");
+  LogprobAcceptedArgs a;
+  a.logprob = logprob; a.top_ids = reinterpret_cast<long long*>(top_ids); a.top_logprobs = top_logprobs; a.logits = logits;
+  a.draft = reinterpret_cast<const long long*>(draft_tokens); a.path = path; a.accept_len = accept_len;
+  a.bonus = reinterpret_cast<const long long*>(bonus); a.seq_lens = seq_lens; a.finished = finished; a.batch = batch; a.num_nodes = num_nodes;
+  a.vocab = vocab; a.n = n; a.width = width; a.stream = stream;
+  return logprobs_accepted(a);
+}
+
 int qs_prefill_attention(const void* q,const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
                          int64_t out_stride, const int32_t* cu_seqlens, int batch, int num_tokens, int max_seqlen, int num_heads, int num_kv_heads,
                          int head_dim, float softmax_scale, void* stream) {

@@ -241,6 +241,37 @@ struct LogprobArgs {
   void* stream = nullptr;
 };
 int logprobs_rows(const LogprobArgs& a);
+// apply_penalties on every node row of a draft tree, each node's history extended by its ancestors' tokens and its own
+struct PenaltyTreeArgs {
+  void* logits = nullptr;               // fp16 [batch, num_nodes, vocab], modified in place
+  const long long* draft = nullptr;     // [batch, num_nodes]: node 0 is the root (h[seq_lens - 1], not read), -1 / out of range ignored
+  const int* tree_mask = nullptr;       // [batch, num_nodes] ancestor words
+  const long long* history = nullptr;   // [batch, history_len]
+  const int* prompt_lens = nullptr;     // [batch]
+  const int* seq_lens = nullptr;        // [batch], clamped to [0, history_len] on the device
+  const float* repetition = nullptr;    // [batch]
+  const float* presence = nullptr;
+  const float* frequency = nullptr;
+  int batch = 0, num_nodes = 0, vocab = 0, history_len = 0;
+  void* stream = nullptr;
+};
+int apply_penalties_tree(const PenaltyTreeArgs& a);
+// logprobs_rows of the tokens a speculative step emits, scored by their node rows and written at their history columns
+struct LogprobAcceptedArgs {
+  float* logprob = nullptr;             // [batch, width]
+  long long* top_ids = nullptr;         // [batch, width, n]
+  float* top_logprobs = nullptr;        // [batch, width, n]
+  const void* logits = nullptr;         // fp16 [batch, num_nodes, vocab]
+  const long long* draft = nullptr;     // [batch, num_nodes]
+  const int* path = nullptr;            // [batch, num_nodes]
+  const int* accept_len = nullptr;      // [batch]
+  const long long* bonus = nullptr;     // [batch]
+  const int* seq_lens = nullptr;        // [batch], before the commit
+  const int* finished = nullptr;        // [batch]
+  int batch = 0, num_nodes = 0, vocab = 0, n = 0, width = 0;
+  void* stream = nullptr;
+};
+int logprobs_accepted(const LogprobAcceptedArgs& a);
 
 // speculative.cu: prompt-lookup draft trees from the token history, and the commit that advances every sequence by what it accepted
 struct NgramProposeArgs {
@@ -270,5 +301,7 @@ struct SpecCommitArgs {
   void* stream = nullptr;
 };
 int spec_commit(const SpecCommitArgs& a);
+// spec_commit with a stop-token set per row: stop_ids [batch, num_stops <= 8], -1 pads
+int spec_commit_stops(const SpecCommitArgs& a, const long long* stop_ids, int num_stops);
 
 }  // namespace qs

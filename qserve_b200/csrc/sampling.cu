@@ -24,8 +24,10 @@
 // the result exactly tree_accept_greedy(draft, mask, argmax_rows(logits)).
 //
 // apply_penalties_kernel: repetition / presence / frequency penalties on the logits before the sampler, one CTA per row over its history
-// only (sorted keys, one writer per distinct token).  logprobs_rows_kernel: the log-probability of a chosen token and the top-n tokens of the
-// T = 1 softmax, on the sample_rows cluster structure (fixed-point sums, radix select of the n-th largest key).
+// only (sorted keys, one writer per distinct token).  apply_penalties_tree_kernel: the same penalties on every node row of a draft tree, each
+// node's history extended by its path (the history sorted once per sequence).  logprobs_rows_kernel: the log-probability of a chosen token
+// and the top-n tokens of the T = 1 softmax, on the sample_rows cluster structure (fixed-point sums, radix select of the n-th largest key).
+// logprobs_accepted_kernel: the same arithmetic for the tokens a speculative step emits, written at their history columns.
 //
 // All kernels read everything a preceding kernel may write (logits, drafts, mask, history, parameters, offsets) after griddepcontrol.wait,
 // need no host synchronisation and can be captured in a CUDA graph.
@@ -532,25 +534,11 @@ __device__ __forceinline__ int lower_bound(const uint32_t* keys, int lo, int hi,
   return lo;
 }
 
-// One CTA per row.  The history becomes keys (token << 1) | is_output in shared memory (padding, out-of-range ids and the tail past the
-// row's length: kNoKey), sorted ascending (bitonic over the next power of two of the row's length).  The first key of each run of one token
-// applies the penalties to that token's logit: the run's output keys are its upper part, found by binary search.  Every distinct token is
-// written by exactly one thread, and only when its fp16 bits change.
-__global__ void __launch_bounds__(kPenThreads, 1) apply_penalties_kernel(__half* __restrict__ logits, const long long* __restrict__ history,
-                                                                       const int* __restrict__ prompt_lens, const int* __restrict__ seq_lens,
-                                                                       const float* __restrict__ repetition, const float* __restrict__ presence,
-                                                                       const float* __restrict__ frequency, int V, int H) {
-  extern __shared__ uint32_t keys[];
-  if (threadIdx.x == 0) pdl_launch_dependents();
-  pdl_wait();  // logits, history, lengths and parameters may come from the preceding kernels
-  const int row = blockIdx.x;
-  const float rep = repetition[row], pres = presence[row], freq = frequency[row];
-  if (rep == 1.f && pres == 0.f && freq == 0.f) return;  // neutral row: nothing is written
-  const int hl = min(max(seq_lens[row], 0), H);
-  const int pl = min(max(prompt_lens[row], 0), hl);
+// The row's history h[0 .. hl) as keys (token << 1) | is_output (position >= pl) in shared memory (padding, out-of-range ids and the tail
+// past hl: kNoKey), sorted ascending (bitonic over the next power of two of hl).  Returns that power of two.
+__device__ __forceinline__ int sorted_history_keys(uint32_t* keys, const long long* hrow, int hl, int pl, int V) {
   int n = 1;
   while (n < hl) n <<= 1;
-  const long long* hrow = history + static_cast<size_t>(row) * H;
   for (int i = threadIdx.x; i < n; i += kPenThreads) {
     uint32_t k = kNoKey;
     if (i < hl) {
@@ -575,22 +563,114 @@ __global__ void __launch_bounds__(kPenThreads, 1) apply_penalties_kernel(__half*
       __syncthreads();
     }
   }
+  return n;
+}
+
+// the penalties of a token that occurs in the history, c_out times at an output position, on lrow[t]; written only when the bits change
+__device__ __forceinline__ void penalise(__half* lrow, uint32_t t, float rep, float pres, float freq, int c_out) {
+  const __half old = lrow[t];
+  float x = __half2float(old);
+  if (x != x) return;  // NaN logits are not written
+  if (rep != 1.f) x = x > 0.f ? __fdiv_rn(x, rep) : __fmul_rn(x, rep);
+  if (c_out > 0) {
+    x = __fsub_rn(x, __fmul_rn(freq, static_cast<float>(c_out)));
+    x = __fsub_rn(x, pres);
+  }
+  const __half nw = __float2half_rn(x);
+  if (__half_as_ushort(nw) != __half_as_ushort(old)) lrow[t] = nw;
+}
+
+// One CTA per row.  The history becomes sorted keys (sorted_history_keys).  The first key of each run of one token applies the penalties to
+// that token's logit: the run's output keys are its upper part, found by binary search.  Every distinct token is written by exactly one
+// thread, and only when its fp16 bits change.
+__global__ void __launch_bounds__(kPenThreads, 1) apply_penalties_kernel(__half* __restrict__ logits, const long long* __restrict__ history,
+                                                                       const int* __restrict__ prompt_lens, const int* __restrict__ seq_lens,
+                                                                       const float* __restrict__ repetition, const float* __restrict__ presence,
+                                                                       const float* __restrict__ frequency, int V, int H) {
+  extern __shared__ uint32_t keys[];
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // logits, history, lengths and parameters may come from the preceding kernels
+  const int row = blockIdx.x;
+  const float rep = repetition[row], pres = presence[row], freq = frequency[row];
+  if (rep == 1.f && pres == 0.f && freq == 0.f) return;  // neutral row: nothing is written
+  const int hl = min(max(seq_lens[row], 0), H);
+  const int pl = min(max(prompt_lens[row], 0), hl);
+  const int n = sorted_history_keys(keys, history + static_cast<size_t>(row) * H, hl, pl, V);
   __half* lrow = logits + static_cast<size_t>(row) * V;
   for (int i = threadIdx.x; i < n; i += kPenThreads) {
     const uint32_t k = keys[i];
     if (k == kNoKey || (i > 0 && (keys[i - 1] >> 1) == (k >> 1))) continue;
     const uint32_t t = k >> 1;
-    const int c_out = lower_bound(keys, i, n, (t + 1) << 1) - lower_bound(keys, i, n, (t << 1) | 1u);
-    const __half old = lrow[t];
-    float x = __half2float(old);
-    if (x != x) continue;  // NaN logits are not written
-    if (rep != 1.f) x = x > 0.f ? __fdiv_rn(x, rep) : __fmul_rn(x, rep);
-    if (c_out > 0) {
-      x = __fsub_rn(x, __fmul_rn(freq, static_cast<float>(c_out)));
-      x = __fsub_rn(x, pres);
+    penalise(lrow, t, rep, pres, freq, lower_bound(keys, i, n, (t + 1) << 1) - lower_bound(keys, i, n, (t << 1) | 1u));
+  }
+}
+
+// The penalties of every node of a draft tree, one CTA per sequence over its `nodes` verify rows.  Node i's expanded history is the row's
+// history h[0 .. hl), then the tokens of its ancestors j >= 1 in index order, then its own token (i >= 1); path position k sits at hl + k
+// and is an output position iff hl + k >= prompt_len.  The history is sorted once (sorted_history_keys); the <= 16 node tokens, path words
+// and output words are staged beside it.  Pass 1: the first key of each distinct history token applies, for every node, the penalties with
+// the history's output count plus that token's output occurrences on the node's path.  Pass 2: for each (node, path node j) whose token is
+// absent from the history (binary search) and does not occur earlier on the path, the penalties with its output occurrences on the path.
+// Each (node, token) is written by one thread at most, and only when its bits change.
+__global__ void __launch_bounds__(kPenThreads, 1) apply_penalties_tree_kernel(__half* __restrict__ logits, const long long* __restrict__ draft,
+                                                                            const int* __restrict__ tree_mask, const long long* __restrict__ history,
+                                                                            const int* __restrict__ prompt_lens, const int* __restrict__ seq_lens,
+                                                                            const float* __restrict__ repetition, const float* __restrict__ presence,
+                                                                            const float* __restrict__ frequency, int nodes, int V, int H) {
+  extern __shared__ uint32_t keys[];
+  __shared__ uint32_t s_tok[kMaxNodes];   // node tokens, kNoKey outside [0, V)
+  __shared__ uint32_t s_path[kMaxNodes];  // node i: the nodes whose tokens its expanded history appends
+  __shared__ uint32_t s_out[kMaxNodes];   // node i: the path nodes at an output position
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // logits, drafts, masks, history, lengths and parameters may come from the preceding kernels
+  const int b = blockIdx.x;
+  const float rep = repetition[b], pres = presence[b], freq = frequency[b];
+  if (rep == 1.f && pres == 0.f && freq == 0.f) return;  // neutral row: nothing is written
+  const int hl = min(max(seq_lens[b], 0), H);
+  const int p0 = max(prompt_lens[b], 0);
+  const size_t row0 = static_cast<size_t>(b) * nodes;
+  if (threadIdx.x < kMaxNodes) {
+    const int i = threadIdx.x;
+    uint32_t tok = kNoKey, path = 0, out = 0;
+    if (i < nodes) {
+      const long long t = draft[row0 + i];
+      if (t >= 0 && t < V) tok = static_cast<uint32_t>(t);
+      if (i > 0) path = (static_cast<uint32_t>(tree_mask[row0 + i]) & ((1u << i) - 1u) & ~1u) | (1u << i);
+      for (uint32_t m = path; m; m &= m - 1) {
+        const int j = __ffs(m) - 1;
+        if (hl + __popc(path & ((1u << j) - 1u)) >= p0) out |= 1u << j;
+      }
     }
-    const __half nw = __float2half_rn(x);
-    if (__half_as_ushort(nw) != __half_as_ushort(old)) lrow[t] = nw;
+    s_tok[i] = tok;
+    s_path[i] = path;
+    s_out[i] = out;
+  }
+  // (sorted_history_keys synchronises the block before any key, and so any s_* entry, is read)
+  const int n = sorted_history_keys(keys, history + static_cast<size_t>(b) * H, hl, min(p0, hl), V);
+  auto same = [&](uint32_t t) {  // the nodes whose token is t
+    uint32_t m = 0;
+#pragma unroll
+    for (int j = 0; j < kMaxNodes; ++j) m |= (s_tok[j] == t ? 1u : 0u) << j;
+    return m;
+  };
+  __half* lb = logits + row0 * V;
+  for (int i = threadIdx.x; i < n; i += kPenThreads) {  // pass 1: the history's tokens
+    const uint32_t k = keys[i];
+    if (k == kNoKey || (i > 0 && (keys[i - 1] >> 1) == (k >> 1))) continue;
+    const uint32_t t = k >> 1;
+    const int c_hist = lower_bound(keys, i, n, (t + 1) << 1) - lower_bound(keys, i, n, (t << 1) | 1u);
+    const uint32_t on = same(t);
+    for (int node = 0; node < nodes; ++node) penalise(lb + static_cast<size_t>(node) * V, t, rep, pres, freq, c_hist + __popc(on & s_out[node]));
+  }
+  for (int p = threadIdx.x; p < nodes * kMaxNodes; p += kPenThreads) {  // pass 2: path tokens absent from the history
+    const int node = p / kMaxNodes, j = p % kMaxNodes;
+    const uint32_t path = s_path[node], t = s_tok[j];
+    if (!((path >> j) & 1u) || t == kNoKey) continue;
+    const uint32_t on = same(t);
+    if (on & path & ((1u << j) - 1u)) continue;  // an earlier path node has the same token
+    const int at = lower_bound(keys, 0, n, t << 1);
+    if (at < n && (keys[at] >> 1) == t) continue;  // in the history: pass 1
+    penalise(lb + static_cast<size_t>(node) * V, t, rep, pres, freq, __popc(on & s_out[node]));
   }
 }
 
@@ -619,20 +699,15 @@ __device__ __forceinline__ uint32_t top_key(uint32_t b) { return okey(b == 0x800
 // with w = 1 at the maximum, S = sum w in 64-bit fixed point; a logit's log-probability is (x - max) - log S in fp64 (-log S at the
 // maximum).  Top-n: tau = the n-th largest non-NaN key by the two-level radix select over the keys above a lower bound (the n-th largest
 // per-warp maximum); the keys > tau (fewer than n) and the first keys == tau in index order are merged by rank 0.
-__global__ void __launch_bounds__(kThreads, 1) logprobs_rows_kernel(float* __restrict__ logprob, long long* __restrict__ top_ids,
-                                                                  float* __restrict__ top_logprobs, const __half* __restrict__ logits,
-                                                                  const long long* __restrict__ tokens, int n, int V) {
-  extern __shared__ uint4 dyn[];
-  __shared__ Smem s;
-  __shared__ TopSmem ts;
-  if (threadIdx.x == 0) pdl_launch_dependents();
-  pdl_wait();  // logits and tokens may come from the preceding kernels
-  const int row = blockIdx.x / kCluster, rank = blockIdx.x % kCluster;
+//
+// logprob_row: that arithmetic for the fp16 row lrow, called by every thread of the cluster; rank 0 reads the scored token with token() at
+// the end and writes logprob[out] and top_ids / top_logprobs[out * n .. + n).
+template <typename Tok>
+__device__ __forceinline__ void logprob_row(Smem& s, TopSmem& ts, __half* xs, const __half* lrow, int rank, int n, int V, Tok token, int out,
+                                            float* __restrict__ logprob, long long* __restrict__ top_ids, float* __restrict__ top_logprobs) {
   int v0, v1;
   slice_of(V, rank, v0, v1);
   const int n_loc = (v1 - v0) * 8, g0 = v0 * 8;
-  __half* xs = reinterpret_cast<__half*>(dyn);
-  const __half* lrow = logits + static_cast<size_t>(row) * V;
   load_slice(xs, lrow, v0, v1);
   const uint16_t* xb = reinterpret_cast<const uint16_t*>(xs);
   int phase = 0;
@@ -775,16 +850,57 @@ __global__ void __launch_bounds__(kThreads, 1) logprobs_rows_kernel(float* __res
     }
   }
   if (rank == 0 && threadIdx.x == 0) {
-    const long long t = tokens[row];
-    logprob[row] = (t >= 0 && t < V) ? lp_of(__half2float(lrow[t])) : kNan;
+    const long long t = token();
+    logprob[out] = (t >= 0 && t < V) ? lp_of(__half2float(lrow[t])) : kNan;
     for (int j = 0; j < n; ++j) {
       const bool listed = j < ne;
-      top_ids[static_cast<size_t>(row) * n + j] = listed ? ts.top_idx[j] : -1;
-      top_logprobs[static_cast<size_t>(row) * n + j] =
+      top_ids[static_cast<size_t>(out) * n + j] = listed ? ts.top_idx[j] : -1;
+      top_logprobs[static_cast<size_t>(out) * n + j] =
           listed ? lp_of(__half2float(__ushort_as_half(static_cast<unsigned short>(key_bits(ts.top_key[j]))))) : (none ? kNan : -INFINITY);
     }
   }
   cluster_sync();  // the peers' lists stay alive until rank 0 has read them
+}
+
+__global__ void __launch_bounds__(kThreads, 1) logprobs_rows_kernel(float* __restrict__ logprob, long long* __restrict__ top_ids,
+                                                                  float* __restrict__ top_logprobs, const __half* __restrict__ logits,
+                                                                  const long long* __restrict__ tokens, int n, int V) {
+  extern __shared__ uint4 dyn[];
+  __shared__ Smem s;
+  __shared__ TopSmem ts;
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // logits and tokens may come from the preceding kernels
+  const int row = blockIdx.x / kCluster, rank = blockIdx.x % kCluster;
+  logprob_row(s, ts, reinterpret_cast<__half*>(dyn), logits + static_cast<size_t>(row) * V, rank, n, V, [&] { return tokens[row]; }, row, logprob,
+              top_ids, top_logprobs);
+}
+
+// The log-probabilities of the tokens a speculative step emits, one cluster per (sequence b, emitted token k).  With acc = accept_len[b]
+// clamped to [1, nodes] and path entries to [0, nodes - 1] (as spec_commit clamps them), token k < acc is draft[path[k + 1]] for k < acc - 1
+// and bonus[b] for k = acc - 1; it is scored by node row path[k] with the logprobs_rows arithmetic and written at history column
+// min(max(seq_lens[b], 0), W) + k, where spec_commit puts it.  Finished rows, tokens past acc and columns >= W exit after the dependency wait.
+__global__ void __launch_bounds__(kThreads, 1) logprobs_accepted_kernel(float* __restrict__ logprob, long long* __restrict__ top_ids,
+                                                                      float* __restrict__ top_logprobs, const __half* __restrict__ logits,
+                                                                      const long long* __restrict__ draft, const int* __restrict__ path,
+                                                                      const int* __restrict__ accept_len, const long long* __restrict__ bonus,
+                                                                      const int* __restrict__ seq_lens, const int* __restrict__ finished, int nodes,
+                                                                      int n, int V, int W) {
+  extern __shared__ uint4 dyn[];
+  __shared__ Smem s;
+  __shared__ TopSmem ts;
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // logits and the acceptance outputs come from the preceding kernels, the lengths from the previous step
+  const int c = blockIdx.x / kCluster, rank = blockIdx.x % kCluster;
+  const int b = c / nodes, k = c % nodes;
+  if (finished[b]) return;  // uniform over the cluster: every CTA reads the same values
+  const int acc = min(max(accept_len[b], 1), nodes);
+  const int col = min(max(seq_lens[b], 0), W) + k;
+  if (k >= acc || col >= W) return;
+  const size_t row0 = static_cast<size_t>(b) * nodes;
+  const int node = min(max(path[row0 + k], 0), nodes - 1);
+  logprob_row(s, ts, reinterpret_cast<__half*>(dyn), logits + (row0 + node) * V, rank, n, V,
+              [&] { return k + 1 < acc ? draft[row0 + min(max(path[row0 + k + 1], 0), nodes - 1)] : bonus[b]; }, b * W + col, logprob, top_ids,
+              top_logprobs);
 }
 
 int slice_cap_of(int V) { return ((V / 8 + kCluster - 1) / kCluster) * 8; }
@@ -851,6 +967,47 @@ int logprobs_rows(const LogprobArgs& a) {
   if (rc) return rc;
   return launch(logprobs_rows_kernel, dim3(static_cast<unsigned>(a.rows) * kCluster), dim3(kThreads), smem, kCluster, a.stream, "logprobs_rows",
                 a.logprob, a.top_ids, a.top_logprobs, static_cast<const __half*>(a.logits), a.tokens, a.n, a.vocab);
+}
+
+int apply_penalties_tree(const PenaltyTreeArgs& a) {
+  QS_REQUIRE(a.batch >= 0 && a.num_nodes >= 1 && a.num_nodes <= kMaxNodes, "apply_penalties_tree: batch=%d num_nodes=%d (1 .. %d)", a.batch,
+             a.num_nodes, kMaxNodes);
+  QS_REQUIRE(a.vocab >= 8 && a.vocab % 8 == 0 && a.vocab <= kMaxVocab, "apply_penalties_tree: vocab=%d (a multiple of 8, 8 .. %d)", a.vocab,
+             kMaxVocab);
+  QS_REQUIRE(a.history_len >= 0 && a.history_len <= kMaxHistory, "apply_penalties_tree: history_len=%d (0 .. %d)", a.history_len, kMaxHistory);
+  if (a.batch == 0) return QS_OK;
+  QS_REQUIRE(a.logits && a.draft && a.tree_mask && (a.history || a.history_len == 0) && a.prompt_lens && a.seq_lens && a.repetition && a.presence &&
+                 a.frequency,
+             "apply_penalties_tree: null pointer");
+  int n = 1;
+  while (n < a.history_len) n <<= 1;
+  const size_t smem = static_cast<size_t>(n) * sizeof(uint32_t);
+  const int rc = raise_smem_limit(apply_penalties_tree_kernel, smem, "apply_penalties_tree");
+  if (rc) return rc;
+  return launch(apply_penalties_tree_kernel, dim3(static_cast<unsigned>(a.batch)), dim3(kPenThreads), smem, 0, a.stream, "apply_penalties_tree",
+                static_cast<__half*>(a.logits), a.draft, a.tree_mask, a.history, a.prompt_lens, a.seq_lens, a.repetition, a.presence, a.frequency,
+                a.num_nodes, a.vocab, a.history_len);
+}
+
+int logprobs_accepted(const LogprobAcceptedArgs& a) {
+  QS_REQUIRE(a.batch >= 0 && a.num_nodes >= 1 && a.num_nodes <= kMaxNodes, "logprobs_accepted: batch=%d num_nodes=%d (1 .. %d)", a.batch,
+             a.num_nodes, kMaxNodes);
+  QS_REQUIRE(a.vocab >= 8 && a.vocab % 8 == 0 && a.vocab <= kMaxVocab, "logprobs_accepted: vocab=%d (a multiple of 8, 8 .. %d)", a.vocab, kMaxVocab);
+  QS_REQUIRE(a.n >= 0 && a.n <= kMaxTop, "logprobs_accepted: n=%d (0 .. %d)", a.n, kMaxTop);
+  QS_REQUIRE(a.width >= 1, "logprobs_accepted: width=%d", a.width);
+  QS_REQUIRE(static_cast<long long>(a.batch) * a.num_nodes <= 0x7fffffff / kCluster &&
+                 static_cast<long long>(a.batch) * a.width * (a.n > 0 ? a.n : 1) <= 0x7fffffffLL,
+             "logprobs_accepted: batch too large");
+  if (a.batch == 0) return QS_OK;
+  QS_REQUIRE(a.logprob && a.logits && a.draft && a.path && a.accept_len && a.bonus && a.seq_lens && a.finished &&
+                 (a.n == 0 || (a.top_ids && a.top_logprobs)),
+             "logprobs_accepted: null pointer");
+  const size_t smem = static_cast<size_t>(slice_cap_of(a.vocab)) * 2;
+  const int rc = raise_smem_limit(logprobs_accepted_kernel, smem, "logprobs_accepted");
+  if (rc) return rc;
+  return launch(logprobs_accepted_kernel, dim3(static_cast<unsigned>(a.batch * a.num_nodes) * kCluster), dim3(kThreads), smem, kCluster, a.stream,
+                "logprobs_accepted", a.logprob, a.top_ids, a.top_logprobs, static_cast<const __half*>(a.logits), a.draft, a.path, a.accept_len,
+                a.bonus, a.seq_lens, a.finished, a.num_nodes, a.n, a.vocab, a.width);
 }
 
 }  // namespace qs

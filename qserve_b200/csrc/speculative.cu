@@ -9,8 +9,9 @@
 // the tokens and the ancestor words; uncreated nodes are padding (token -1, mask 1).  The output is bitwise deterministic.
 //
 // spec_commit_kernel: one thread per sequence appends draft[path[1 .. acc - 1]] and the bonus token to the history, cut after the first eos
-// and at the row's budget, and writes the positions the next step reads (start_pos, context_lens, roots).  Both kernels read every input after
-// the PDL dependency wait: the previous step's commit writes the history and the lengths.  Both are CUDA-graph capturable.
+// and at the row's budget, and writes the positions the next step reads (start_pos, context_lens, roots).  spec_commit_stops_kernel cuts
+// after the first token of {eos} and the row's stop set instead.  Every kernel reads every input after the PDL dependency wait: the previous
+// step's commit writes the history and the lengths.  All are CUDA-graph capturable.
 #include "common.cuh"
 #include "launch.cuh"
 
@@ -24,6 +25,7 @@ constexpr int kMaxBranches = 8;
 constexpr int kMaxNgram = 8;
 constexpr int kMaxHistory = 32768;  // j < 2^15: a candidate packs into (m << 16) | j
 constexpr int kCommitThreads = 128;
+constexpr int kMaxStops = 8;  // stop tokens per row besides eos
 
 __device__ __forceinline__ int block_max(int v, int* red) {  // every thread calls; returns the block-wide maximum to all
   v = __reduce_max_sync(0xffffffffu, v);
@@ -174,6 +176,65 @@ __global__ void __launch_bounds__(kCommitThreads) spec_commit_kernel(const long 
   if (hit_eos || L2 - prompt_lens[b] >= budget[b]) finished[b] = 1;
 }
 
+// spec_commit_kernel with a per-row stop-token set stop_ids [batch, num_stops] (num_stops <= kMaxStops, -1 pads): the first emitted token
+// in {eos} and the set ends the row as eos does
+__global__ void __launch_bounds__(kCommitThreads) spec_commit_stops_kernel(const long long* __restrict__ draft, const int* __restrict__ path,
+                                                                           const int* __restrict__ accept_len, const long long* __restrict__ bonus,
+                                                                           long long* __restrict__ history, int* __restrict__ seq_lens,
+                                                                           const int* __restrict__ prompt_lens, const int* __restrict__ budget,
+                                                                           const long long* __restrict__ eos, const long long* __restrict__ stop_ids,
+                                                                           int* __restrict__ finished, int* __restrict__ start_pos,
+                                                                           int* __restrict__ context_lens, long long* __restrict__ roots, int batch, int n,
+                                                                           int hist_len, int num_stops) {
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  pdl_wait();  // the acceptance outputs come from the kernels before; the lengths from the previous step
+  const int b = blockIdx.x * kCommitThreads + threadIdx.x;
+  if (b >= batch || finished[b]) return;
+  long long stops[kMaxStops];
+#pragma unroll
+  for (int s = 0; s < kMaxStops; ++s) stops[s] = s < num_stops ? stop_ids[static_cast<size_t>(b) * num_stops + s] : -1;
+  long long* h = history + static_cast<size_t>(b) * hist_len;
+  const int L = min(max(seq_lens[b], 0), hist_len);
+  const int acc = min(max(accept_len[b], 1), n);
+  const long long e = eos[b];
+  const size_t row = static_cast<size_t>(b) * n;
+  long long app[kMaxNodes];  // the accepted drafts after the root, then the bonus token
+  int count = acc;
+  bool hit_stop = false;
+#pragma unroll
+  for (int k = 0; k < kMaxNodes; ++k) {
+    if (k < acc) {
+      app[k] = k + 1 < acc ? draft[row + min(max(path[row + k + 1], 0), n - 1)] : bonus[b];
+      bool stop = e >= 0 && app[k] == e;
+#pragma unroll
+      for (int s = 0; s < kMaxStops; ++s) stop |= stops[s] >= 0 && app[k] == stops[s];
+      if (!hit_stop && stop) {
+        hit_stop = true;
+        count = k + 1;
+      }
+    }
+  }
+  const int room = max(budget[b] - (L - prompt_lens[b]), 0);
+  if (count > room) {
+    count = room;
+    hit_stop = false;  // the stop token fell behind the budget cut
+  }
+  long long last = L > 0 ? h[L - 1] : -1;
+#pragma unroll
+  for (int k = 0; k < kMaxNodes; ++k) {
+    if (k < count) {
+      if (L + k < hist_len) h[L + k] = app[k];
+      last = app[k];
+    }
+  }
+  const int L2 = L + count;
+  seq_lens[b] = L2;
+  start_pos[b] = L2 - 1;
+  if (context_lens) context_lens[b] = L2;
+  if (roots) roots[b] = last;
+  if (hit_stop || L2 - prompt_lens[b] >= budget[b]) finished[b] = 1;
+}
+
 }  // namespace
 
 int ngram_propose(const NgramProposeArgs& a) {
@@ -199,6 +260,20 @@ int spec_commit(const SpecCommitArgs& a) {
   return launch(spec_commit_kernel, dim3((a.batch + kCommitThreads - 1) / kCommitThreads), dim3(kCommitThreads), 0, 0, a.stream, "spec_commit", a.draft,
                 a.path, a.accept_len, a.bonus, a.history, a.seq_lens, a.prompt_lens, a.budget, a.eos, a.finished, a.start_pos, a.context_lens, a.roots,
                 a.batch, a.num_nodes, a.history_len);
+}
+
+int spec_commit_stops(const SpecCommitArgs& a, const long long* stop_ids, int num_stops) {
+  QS_REQUIRE(a.batch >= 0 && a.num_nodes >= 1 && a.num_nodes <= kMaxNodes, "spec_commit_stops: batch=%d num_nodes=%d (1 .. %d)", a.batch,
+             a.num_nodes, kMaxNodes);
+  QS_REQUIRE(a.history_len >= 1, "spec_commit_stops: history_len=%d", a.history_len);
+  QS_REQUIRE(num_stops >= 0 && num_stops <= kMaxStops, "spec_commit_stops: num_stops=%d (0 .. %d)", num_stops, kMaxStops);
+  if (a.batch == 0) return QS_OK;
+  QS_REQUIRE(a.draft && a.path && a.accept_len && a.bonus && a.history && a.seq_lens && a.prompt_lens && a.budget && a.eos && a.finished && a.start_pos &&
+                 (stop_ids || num_stops == 0),
+             "spec_commit_stops: null pointer");
+  return launch(spec_commit_stops_kernel, dim3((a.batch + kCommitThreads - 1) / kCommitThreads), dim3(kCommitThreads), 0, 0, a.stream,
+                "spec_commit_stops", a.draft, a.path, a.accept_len, a.bonus, a.history, a.seq_lens, a.prompt_lens, a.budget, a.eos, stop_ids,
+                a.finished, a.start_pos, a.context_lens, a.roots, a.batch, a.num_nodes, a.history_len, num_stops);
 }
 
 }  // namespace qs

@@ -146,7 +146,9 @@ class DecodeRunner:
         every row by what it accepted.  The history is [batch, ctx + 1 + T] (the prompt is ctx cached tokens and the root), the page tables
         cover ctx + T + max(1, verify_len) tokens (the pages past blocks_per_seq come from zero-filled pools made after every random draw, so
         the weights and the first blocks_per_seq pages of each row are those of generate=False), and the per-row state is g_budget (tokens a
-        row may generate, default T), g_eos (-1: none) and g_finished.
+        row may generate, default T), g_eos (-1: none), g_stop (up to 8 stop tokens, -1 pads) and g_finished.  generate_forward(...,
+        penalties=True, logprobs=n) adds the penalties and log-probabilities of forward to plain and speculative steps; the log-probabilities
+        go to history-aligned buffers (g_logprob, g_top_view).
 
         prompt_tokens > 0 (single GPU, fused path) adds the prompt step (`prefill`): at most prompt_tokens prompt tokens per piece, so the
         activation buffers hold max(batch * max(1, verify_len), prompt_tokens) rows.  It makes no generator draws: the weights, pages and
@@ -326,16 +328,19 @@ class DecodeRunner:
         logits = self._forward_fused(tokens, True) if self.fused else self._forward_reference(tokens, True)
         return self._next_tokens(logits, sample, penalties, logprobs)
 
-    def _next_tokens(self, logits, sample: bool, penalties: bool = False, logprobs: int = 0, out: Optional[torch.Tensor] = None):
-        """logits -> the step's tokens as forward describes them, written into out if given."""
+    def _pick(self, logits, sample: bool, penalties: bool = False, logprobs: int = 0, out: Optional[torch.Tensor] = None):
+        """logits -> apply_penalties (if penalties) -> sample_rows / argmax_rows: the step's tokens, written into out if given."""
         if penalties:
             _ext.apply_penalties(logits, self.s_history, self.s_prompt_lens, self.s_seq_lens, self.s_repetition, self.s_presence, self.s_frequency)
         if sample:
-            tok = _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets, out=out)
-        elif self.fused or penalties or logprobs:
-            tok = _ext.argmax_rows(logits, out=out)  # one launch instead of torch's two-pass reduction
-        else:
-            tok = torch.argmax(logits, dim=-1)  # the reference's greedy step
+            return _ext.sample_rows(logits, self.s_temperature, self.s_top_k, self.s_top_p, self.s_seed, self.s_offsets, out=out)
+        if self.fused or penalties or logprobs:
+            return _ext.argmax_rows(logits, out=out)  # one launch instead of torch's two-pass reduction
+        return torch.argmax(logits, dim=-1)  # the reference's greedy step
+
+    def _next_tokens(self, logits, sample: bool, penalties: bool = False, logprobs: int = 0, out: Optional[torch.Tensor] = None):
+        """logits -> the step's tokens as forward describes them, written into out if given."""
+        tok = self._pick(logits, sample, penalties, logprobs, out)
         if logprobs:
             _ext.logprobs_rows(logits, tok, int(logprobs), self.s_logprob, *self.top_logprobs_view(int(logprobs)))
         if penalties or logprobs:
@@ -601,6 +606,9 @@ class DecodeRunner:
         B, dev, n = self.batch, self.dev, max(1, self.verify_len)
         self.g_budget = torch.full((B,), self.max_new_tokens, dtype=torch.int32, device=dev)
         self.g_eos = torch.full((B,), -1, dtype=torch.int64, device=dev)
+        self.g_stop = torch.full((B, _ext.MAX_STOP_TOKENS), -1, dtype=torch.int64, device=dev)  # SamplingParams.stop_token_ids, -1 pads
+        self.g_logprob = None  # fp32 [B, W] and the top-n buffers: allocated by the first step with logprobs > 0 (before any capture)
+        self.g_top_n = 0
         self.g_finished = torch.zeros(B, dtype=torch.int32, device=dev)
         # the verify step's cached length P = L - 1 (the verify step's v_start when there is one)
         self.g_start = self.v_start if self.verify_len else torch.full((B,), self.ctx, dtype=torch.int32, device=dev)
@@ -610,10 +618,25 @@ class DecodeRunner:
         self.g_tokens = torch.zeros(B * n, dtype=torch.int64, device=dev)
         self.g_mask = torch.zeros(B * n, dtype=torch.int32, device=dev)
 
+    def _alloc_generate_logprobs(self, n: int) -> None:
+        """g_logprob fp32 [B, W] (W = s_history.size(1)) and the flat top-n buffers behind g_top_view, on first use (torch.full: no random
+        draws).  Column c holds the entry of history token c."""
+        B, W = self.s_history.shape
+        if self.g_logprob is None:
+            self.g_logprob = torch.full((B, W), float("nan"), dtype=torch.float32, device=self.dev)
+            self._g_top_ids = torch.full((B * W * _ext.MAX_TOP_LOGPROBS,), -1, dtype=torch.int64, device=self.dev)
+            self._g_top_logprobs = torch.full((B * W * _ext.MAX_TOP_LOGPROBS,), float("nan"), dtype=torch.float32, device=self.dev)
+        self.g_top_n = n
+
+    def g_top_view(self, n: int):
+        """(top ids int64 [B, W, n], top log-probabilities fp32 [B, W, n]): the history-aligned top-n entries a step with logprobs = n writes."""
+        B, W = self.s_history.shape
+        return self._g_top_ids[: B * W * n].view(B, W, n), self._g_top_logprobs[: B * W * n].view(B, W, n)
+
     def reset_generation(self, prompt: torch.Tensor) -> None:
         """Start generating after prompt int64 [batch, ctx + 1]: the ctx tokens the pages hold, then the root (the latest token, not yet
-        cached).  Sets the history and its lengths, the positions of both step kinds and tokens_in, and clears g_finished; g_budget and g_eos
-        stay as the caller set them."""
+        cached).  Sets the history and its lengths, the positions of both step kinds and tokens_in, and clears g_finished; g_budget, g_eos
+        and g_stop stay as the caller set them."""
         assert self.generate, "construct the runner with generate=True"
         B, C = self.batch, self.ctx + 1
         assert tuple(prompt.shape) == (B, C) and prompt.dtype == torch.int64, f"prompt must be int64 [{B}, {C}]"
@@ -626,20 +649,35 @@ class DecodeRunner:
         self.tokens_in.copy_(prompt[:, self.ctx])
         self.g_finished.zero_()
 
-    def generate_forward(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False) -> None:
+    def generate_forward(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False, penalties: bool = False,
+                         logprobs: int = 0) -> None:
         """One generation step for every row; the tokens go to s_history (lengths s_seq_lens).  n = 1: the decode step at the rows' own
         lengths, argmax_rows (or sample_rows with the s_* parameters if sampled), spec_commit of that token.  2 <= n <= verify_len:
         ngram_propose (n nodes, `branches` continuations, match lengths ngram = (n_min, n_max)) -> verify_forward of the draft tree ->
-        accept_and_compact (or accept_sampled_and_compact with one-hot drafts, which keeps sampling lossless) -> spec_commit.  Finished rows
-        (g_finished) are computed but not advanced.  No host synchronisation."""
+        accept_and_compact (or accept_sampled_and_compact with one-hot drafts, which keeps sampling lossless) -> spec_commit.  The commit
+        ends a row at g_eos, at any token of g_stop and at g_budget.  Finished rows (g_finished) are computed but not advanced.  No host
+        synchronisation.
+
+        penalties=True: the logits first go through apply_penalties (n = 1; the history up to and including the root) or apply_penalties_tree
+        (every draft node's row penalised as the sequential step at its position would be, so acceptance stays exact) with s_repetition,
+        s_presence and s_frequency.  logprobs = k (1 .. 20): logprobs_accepted of the (penalised) logits before the commit: the entry of history
+        token c goes to g_logprob[b, c] and g_top_view(k)[.][b, c], valid for s_prompt_lens[b] <= c < s_seq_lens[b]."""
         assert self.generate, "construct the runner with generate=True"
+        logprobs = int(logprobs)
+        assert 0 <= logprobs <= _ext.MAX_TOP_LOGPROBS, f"logprobs={logprobs}: 0 .. {_ext.MAX_TOP_LOGPROBS}"
+        if logprobs:
+            self._alloc_generate_logprobs(logprobs)
         B = self.batch
         common = (self.s_history, self.s_seq_lens, self.s_prompt_lens, self.g_budget, self.g_eos, self.g_finished, self.g_start, self.context_lens,
                   self.tokens_in)
         if n == 1:
-            tok = self._next_tokens(self._forward_fused(self.tokens_in, True), sampled, out=self.tokens_out)
+            logits = self._forward_fused(self.tokens_in, True)
+            tok = self._pick(logits, sampled, penalties, logprobs, out=self.tokens_out)
+            if logprobs:
+                _ext.logprobs_accepted(logits.view(B, 1, -1), tok.view(B, 1), self.g_path1, self.g_accept1, tok, self.s_seq_lens, self.g_finished,
+                                       logprobs, self.g_logprob, *self.g_top_view(logprobs))
             # the path [0] of length 1 never reads the drafts: any [B, 1] tensor that is not an output will do
-            _ext.spec_commit(tok.view(B, 1), self.g_path1, self.g_accept1, tok, *common)
+            _ext.spec_commit(tok.view(B, 1), self.g_path1, self.g_accept1, tok, *common, stop_ids=self.g_stop)
             return
         assert 2 <= n <= self.verify_len, f"n={n}: 1, or 2 .. verify_len={self.verify_len}"
         n_min, n_max = ngram
@@ -647,25 +685,38 @@ class DecodeRunner:
         mask = self.g_mask[: B * n].view(B, n)
         _ext.ngram_propose(self.s_history, self.s_seq_lens, n, n_min, n_max, branches, tokens=toks, tree_mask=mask)
         emb = toks.clamp(min=0)  # padding nodes (-1) are embedded as token 0; they are never accepted
-        if sampled:
+        if sampled or penalties or logprobs:
             logits = self.verify_forward(emb, return_logits=True, tree_mask=mask)
-            acc, path, bonus = self.accept_sampled_and_compact(toks, mask, logits, None)
+            if penalties:
+                _ext.apply_penalties_tree(logits, toks, mask, self.s_history, self.s_prompt_lens, self.s_seq_lens, self.s_repetition, self.s_presence,
+                                          self.s_frequency)
+            if sampled:
+                acc, path, bonus = self.accept_sampled_and_compact(toks, mask, logits, None)
+            else:
+                acc, path, bonus = self.accept_and_compact(toks, mask, _ext.argmax_rows(logits.view(B * n, -1)).view(B, n))
+            if logprobs:
+                _ext.logprobs_accepted(logits, toks, path, acc, bonus, self.s_seq_lens, self.g_finished, logprobs, self.g_logprob,
+                                       *self.g_top_view(logprobs))
         else:
             target = self.verify_forward(emb, tree_mask=mask)
             acc, path, bonus = self.accept_and_compact(toks, mask, target)
-        _ext.spec_commit(toks, path, acc, bonus, *common)
+        _ext.spec_commit(toks, path, acc, bonus, *common, stop_ids=self.g_stop)
 
-    def _generate_key(self, n: int, branches: int, ngram: tuple, sampled: bool):
-        return ("generate", int(n), int(branches), tuple(int(x) for x in ngram), bool(sampled))
+    def _generate_key(self, n: int, branches: int, ngram: tuple, sampled: bool, penalties: bool = False, logprobs: int = 0):
+        extra = (bool(penalties), int(logprobs)) if penalties or logprobs else ()  # the keys without the sampler flags are those of before
+        return ("generate", int(n), int(branches), tuple(int(x) for x in ngram), bool(sampled)) + extra
 
-    def capture_generate(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False, warmup: int = 2) -> None:
-        """Capture generate_forward(n, branches, ngram, sampled) in a CUDA graph.  The warm-up runs the step eagerly, so it advances the rows
-        like a replay does: call reset_generation afterwards."""
-        self._capture(self._generate_key(n, branches, ngram, sampled), lambda: self.generate_forward(n, branches, ngram, sampled), warmup)
+    def capture_generate(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False, warmup: int = 2, penalties: bool = False,
+                         logprobs: int = 0) -> None:
+        """Capture generate_forward(n, branches, ngram, sampled, penalties, logprobs) in a CUDA graph.  The warm-up runs the step eagerly, so
+        it advances the rows like a replay does (and allocates the log-probability buffers): call reset_generation afterwards."""
+        self._capture(self._generate_key(n, branches, ngram, sampled, penalties, logprobs),
+                      lambda: self.generate_forward(n, branches, ngram, sampled, penalties, logprobs), warmup)
 
-    def generate_step(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False) -> None:
+    def generate_step(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False, penalties: bool = False,
+                      logprobs: int = 0) -> None:
         """Replay the captured generation step."""
-        self.graphs[self._generate_key(n, branches, ngram, sampled)].replay()
+        self.graphs[self._generate_key(n, branches, ngram, sampled, penalties, logprobs)].replay()
 
     # ---------------------------------------------------------------------------------------------------------
     # prompt step: prefill every row's prompt into its pages, whole or in chunks, then the first token and the hand-off to generation
@@ -690,7 +741,8 @@ class DecodeRunner:
         Hand-off: the block tables get every row's own pages back (undoing fork), context_lens = lens + 1, tokens_in = the first token, and
         v_start / g_start = lens where they exist.  With max_new_tokens > 0: s_history[b] = the prompt, the first token at lens[b], then -1;
         s_prompt_lens = lens and s_seq_lens = lens + 1 (the first token counts as generated).  With generate=True, g_finished[b] = 1 when the
-        first token is g_eos[b] or g_budget[b] <= 1; generate_forward continues from there."""
+        first token is g_eos[b], one of g_stop[b] or g_budget[b] <= 1, and with logprobs = n the first token's entry goes to column lens[b] of
+        g_logprob / g_top_view(n); generate_forward continues from there."""
         assert self.prompt_tokens, "construct the runner with prompt_tokens > 0"
         assert self.max_new_tokens or not (penalties or logprobs), "construct the runner with max_new_tokens > 0 for penalties / logprobs"
         B, cfg, dev = self.batch, self.cfg, self.dev
@@ -765,7 +817,14 @@ class DecodeRunner:
             self.v_start.copy_(lens)
         if self.generate:
             self.g_start.copy_(lens)
-            self.g_finished.copy_(((tok == self.g_eos) | (self.g_budget <= 1)).to(torch.int32))
+            stop = (tok.unsqueeze(1) == self.g_stop).any(dim=1)  # tokens are >= 0: the -1 pads never match
+            self.g_finished.copy_(((tok == self.g_eos) | stop | (self.g_budget <= 1)).to(torch.int32))
+            if logprobs:  # the first token's entry at its history column lens[b]
+                self._alloc_generate_logprobs(int(logprobs))
+                rows, col = torch.arange(B, device=dev), lens.long()
+                self.g_logprob[rows, col] = self.s_logprob
+                for dst, src in zip(self.g_top_view(int(logprobs)), self.top_logprobs_view(int(logprobs))):
+                    dst[rows, col] = src
         self.tokens_in.copy_(tok)
         return tok.clone()
 
@@ -808,8 +867,8 @@ class DecodeRunner:
         one per child; child_rows: rows that are not parents.  With P = the parent's cached tokens (context_lens - 1): in every layer the child's
         block-table entries 0 .. P // 64 - 1 point at the parent's pages (shared and read-only from then on: a child writes only at positions
         >= P), the rest at the child's own pages; kv_cache_fork copies the parent's partial tail page into the child's own page; the child
-        gets the parent's history, s_prompt_lens, s_seq_lens, context_lens, g_start / v_start, tokens_in, g_budget, g_eos, g_finished and
-        penalty parameters.  s_offsets and the sampling parameters stay the child's own, so sampled children diverge.  Eager; the table
+        gets the parent's history, s_prompt_lens, s_seq_lens, context_lens, g_start / v_start, tokens_in, g_budget, g_eos, g_stop, g_finished,
+        penalty parameters and history-aligned log-probabilities.  s_offsets and the sampling parameters stay the child's own, so sampled children diverge.  Eager; the table
         entries are written with torch ops (the attention kernels read the tables before their dependency wait)."""
         children = list(child_rows) if not isinstance(child_rows, int) else [child_rows]
         parents = [parent_rows] * len(children) if isinstance(parent_rows, int) else list(parent_rows)
@@ -823,8 +882,11 @@ class DecodeRunner:
         self.block_tables[:, chi] = torch.where(shared[None, :, None, :], self.block_tables[:, par], self.own_tables[:, chi])
         _ext.kv_cache_fork(self.block_tables, parents, children, cached, self.Hkv, 64, self.size_per_token, self.kv_bits == 4)
         names = ["context_lens", "tokens_in", "s_history", "s_prompt_lens", "s_seq_lens", "s_repetition", "s_presence", "s_frequency", "v_start",
-                 "g_start", "g_budget", "g_eos", "g_finished"]
-        for t in {id(getattr(self, a)): getattr(self, a) for a in names if hasattr(self, a)}.values():  # g_start may alias v_start
+                 "g_start", "g_budget", "g_eos", "g_stop", "g_finished", "g_logprob"]
+        state = [getattr(self, a) for a in names if getattr(self, a, None) is not None]
+        if getattr(self, "g_logprob", None) is not None:
+            state += list(self.g_top_view(self.g_top_n))
+        for t in {id(t): t for t in state}.values():  # g_start may alias v_start
             t[chi] = t[par]
 
     # ---------------------------------------------------------------------------------------------------------
