@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define QS_ABI_VERSION 2
+#define QS_ABI_VERSION 3
 #if defined(__GNUC__)
 #define QS_API __attribute__((visibility("default")))
 #else
@@ -292,6 +292,33 @@ QS_API int qs_tree_accept_greedy(const int64_t* draft_tokens, const int32_t* tre
 QS_API int qs_kv_cache_compact(const int64_t* kv_pointers, const int32_t* start_pos, const int32_t* path, const int32_t* accept_len, int num_layers,
                                int batch, int num_nodes, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token,
                                int int4_kv_cache, void* stream);
+
+/* Shared-prefix decode attention (SamplingParams.n / best_of, shared system prompts): rows forked from one cached prompt read and dequantise
+ * their common pages once per group instead of once per row.
+ *
+ * For every row b the result is qs_single_query_attention's (or, with out_q, qs_single_query_attention_quant's) for that row, with the same
+ * arguments, the same RoPE at position lengths[b] - 1 and the same quantisation and append of the new K / V into the row's own page.  Only the
+ * fp32 summation order of the attention differs.  length_per_sample is required.  Exactly one of out (fp16 [B, Hq, 128]) and out_q (int8
+ * [B, Hq * 128], with out_scale fp16 [B] and out_sum fp16 [B] or NULL) is given.
+ * Group layout (int32, device): the rows of group g are group_rows[group_offsets[g] .. group_offsets[g + 1]); a row sits in at most one group.
+ *   group_pages[g] = S_g: pages 0 .. S_g - 1 are read once for the whole group through the page table of its first row.  row_pages[b] = the S
+ *   of the row's group (0 outside groups); the row's own table is read from page row_pages[b] on.  The caller guarantees, as for page tables,
+ *   that every member has at least 64 S_g cached tokens and that its table entries below S_g equal those of the group's first row
+ *   (qs_kv_cache_fork guarantees both).  num_groups, max_group (largest group) and max_pages (largest S) are host bounds that plan the launch
+ *   shape, so the call can be captured in a CUDA graph.  The layout and the tables are read before the PDL dependency wait; q / k / v and the
+ *   page contents after it.
+ * workspace: at least qs_shared_prefix_attention_workspace_bytes(batch, num_heads, num_kv_heads, timestep, num_groups, max_group, max_pages,
+ *   int4_kv_cache) bytes, zero-filled once and then owned by the library (its split counters clean themselves up).  The call is bitwise
+ *   deterministic: every merge runs in a fixed order.                                                                                     */
+QS_API int qs_shared_prefix_decode_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride,
+                                             const int64_t* kv_pointers, const int32_t* length_per_sample, const int32_t* group_offsets,
+                                             const int32_t* group_rows, const int32_t* group_pages, const int32_t* row_pages, void* out, int8_t* out_q,
+                                             void* out_scale, void* out_sum, int batch, int num_heads, int num_kv_heads, int head_dim,
+                                             int max_blocks_per_seq, int tokens_per_block, int size_per_token, int timestep, int rotary_embedding_dim,
+                                             float rotary_base, int int4_kv_cache, int num_groups, int max_group, int max_pages, void* workspace,
+                                             size_t workspace_bytes, void* stream);
+QS_API size_t qs_shared_prefix_attention_workspace_bytes(int batch, int num_heads, int num_kv_heads, int timestep, int num_groups, int max_group,
+                                                         int max_pages, int int4_kv_cache);
 
 /* qs_kv_cache_fork: copy-on-write fork of cached prompts (SamplingParams.n / best_of: prefill once, decode n rows).  For every layer, K and V
  *   and every pair p, with P = lens[parents[p]] (the parent's cached tokens): copies the bytes of slots 0 .. P % 64 - 1 (codes, scale and

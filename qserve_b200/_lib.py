@@ -40,6 +40,9 @@ SIGNATURES = {
     "qs_tree_decode_attention": (c_int, [_P, _P, _P, _L, _L, _L, _P, _L, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P, _Z, _P]),
     "qs_tree_accept_greedy": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _P]),
     "qs_kv_cache_compact": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "qs_shared_prefix_decode_attention": (c_int, [_P, _P, _P, _L, _L, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I,
+                                                  _F, _I, _I, _I, _I, _P, _Z, _P]),
+    "qs_shared_prefix_attention_workspace_bytes": (c_size_t, [_I, _I, _I, _I, _I, _I, _I, _I]),
     "qs_kv_cache_fork": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "qs_sample_rows": (c_int, [_P, _P, _P, _P, _P, ctypes.c_uint64, _P, _I, _I, _P]),
     "qs_tree_accept_sampling": (c_int, [_P, _P, _P, _P, _P, _P, _P, ctypes.c_uint64, _P, _P, _P, _P, _I, _I, _I, _P]),
@@ -70,7 +73,7 @@ SIGNATURES = {
     "qs_dequant_silu_and_mul_quant": (c_int, [_P, _P, _F, _F, _F, _P, _P, _I, _I, _P]),
 }
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 def _load() -> ctypes.CDLL:

@@ -8,7 +8,7 @@ stream and the two outputs the reference ops allocate themselves.
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 
@@ -468,6 +468,85 @@ def single_query_attention_quant(q, k, v, kv_pointers, length_per_sample, memory
                                               nheads_kv, headdim, kv_pointers.size(-1), int(memory_max_seqlen), int(tokens_per_block), int(size_per_token),
                                               int(timestep), int(rotary_embedding_dim), float(rotary_base), int(bool(int4_kv_cache)),
                                               int(bool(kv_cache_with_zeros)), ws.data_ptr(), ws.numel())
+
+
+class SharedPrefixLayout(NamedTuple):
+    """The group layout of shared_prefix_decode_attention: device tensors (int32) and the host bounds that plan the launch."""
+    group_offsets: torch.Tensor  # [num_groups + 1]
+    group_rows: torch.Tensor     # rows of group g: group_rows[group_offsets[g] : group_offsets[g + 1]]
+    group_pages: torch.Tensor    # [num_groups] shared pages S_g
+    row_pages: torch.Tensor      # [batch] S of the row's group, 0 outside groups
+    num_groups: int
+    max_group: int
+    max_pages: int
+
+
+def shared_prefix_layout(groups, pages, batch: int, device=None) -> SharedPrefixLayout:
+    """The layout of groups (host sequences of rows) sharing their first pages[g] pages, checked on the host: rows in [0, batch), no row in two
+    groups or twice in one, every group non-empty, every S >= 0.  The tensors are made on `device` (default: the CPU)."""
+    groups = [[int(r) for r in g] for g in groups]
+    pages = [int(s) for s in pages]
+    _require(len(groups) == len(pages), f"{len(groups)} groups but {len(pages)} page counts")
+    _require(all(len(g) > 0 for g in groups), "every group needs at least one row")
+    rows = [r for g in groups for r in g]
+    _require(all(0 <= r < batch for r in rows), f"group rows must lie in [0, {batch})")
+    _require(len(set(rows)) == len(rows), "a row appears in more than one group, or twice in one")
+    _require(all(s >= 0 for s in pages), "shared page counts must be >= 0")
+    offsets = [0]
+    for g in groups:
+        offsets.append(offsets[-1] + len(g))
+    row_pages = [0] * batch
+    for g, s in zip(groups, pages):
+        for r in g:
+            row_pages[r] = s
+    i32 = lambda v: torch.tensor(v, dtype=torch.int32, device=device)
+    return SharedPrefixLayout(i32(offsets), i32(rows), i32(pages), i32(row_pages), len(groups), max((len(g) for g in groups), default=0),
+                              max(pages, default=0))
+
+
+def shared_prefix_decode_attention(q, k, v, kv_pointers, length_per_sample, layout: SharedPrefixLayout, tokens_per_block: int, size_per_token: int,
+                                   timestep: int, rotary_embedding_dim: int, rotary_base: float, int4_kv_cache: bool, kv_cache_with_zeros: bool,
+                                   out_q: Optional[torch.Tensor] = None, out_scale: Optional[torch.Tensor] = None,
+                                   out_sum: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+    """single_query_attention for rows that share the first pages of their group (layout: shared_prefix_layout): each group's shared pages
+    are read and dequantised once for all its members.  Every row gets single_query_attention's result up to the fp32 summation order, with
+    the same RoPE and the same page append.  Returns a new fp16 [B, Hq, D] tensor, or with out_q given (int8 [B, Hq*D], out_scale / out_sum
+    fp16 [B]) writes single_query_attention_quant's outputs and returns None.  The caller guarantees that every member has 64 S cached tokens
+    and the group's first row's table entries below S (fork guarantees both)."""
+    for t, n in ((q, "q"), (k, "k"), (v, "v")):
+        _cuda(t, n)
+    dev = q.device
+    _tensor(kv_pointers, "kv_pointers", torch.int64, device=dev)
+    batch = kv_pointers.size(0)
+    nheads, nheads_kv, headdim = q.size(1), k.size(1), k.size(-1)
+    _require(q.dtype == _HALF and k.dtype == _HALF and v.dtype == _HALF, "q, k, v must be float16")
+    _require(q.stride(2) == 1 and q.stride(1) == headdim and k.stride(1) == headdim and v.stride(1) == headdim, "q, k, v: stride(1) must be head_dim")
+    _tensor(length_per_sample, "length_per_sample", torch.int32, (batch,), dev)
+    G = layout.num_groups
+    _tensor(layout.group_offsets, "group_offsets", torch.int32, (G + 1,), dev)
+    _tensor(layout.group_rows, "group_rows", torch.int32, (None,), dev)
+    _tensor(layout.group_pages, "group_pages", torch.int32, (G,), dev)
+    _tensor(layout.row_pages, "row_pages", torch.int32, (batch,), dev)
+    out = None
+    if out_q is None:
+        out = torch.empty((q.size(0), nheads, headdim), dtype=q.dtype, device=dev)
+    else:
+        _tensor(out_q, "out_q", torch.int8, device=dev)
+        _require(out_q.numel() == batch * nheads * headdim, "out_q must be int8 [B, Hq*D]")
+        _tensor(out_scale, "out_scale", _HALF, (batch,), dev)
+        if out_sum is not None:
+            _tensor(out_sum, "out_sum", _HALF, (batch,), dev)
+    _require(bool(kv_cache_with_zeros), "only kv_cache_with_zeros=True is supported")
+    if batch == 0:
+        return out
+    ws = _workspace("sprefix", dev, lib.qs_shared_prefix_attention_workspace_bytes(batch, nheads, nheads_kv, int(timestep), G, layout.max_group,
+                                                                                   layout.max_pages, int(bool(int4_kv_cache))))
+    _call(q, lib.qs_shared_prefix_decode_attention, q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), k.stride(0), v.stride(0),
+          kv_pointers.data_ptr(), length_per_sample.data_ptr(), layout.group_offsets.data_ptr(), layout.group_rows.data_ptr(),
+          layout.group_pages.data_ptr(), layout.row_pages.data_ptr(), _ptr(out), _ptr(out_q), _ptr(out_scale), _ptr(out_sum), batch, nheads,
+          nheads_kv, headdim, kv_pointers.size(-1), int(tokens_per_block), int(size_per_token), int(timestep), int(rotary_embedding_dim),
+          float(rotary_base), int(bool(int4_kv_cache)), G, layout.max_group, layout.max_pages, ws.data_ptr(), ws.numel())
+    return out
 
 
 def apply_bias_rope_update_kv_cache_at(qkv, seq_lens, padding_offset, start_pos, kv_pointers: Optional[torch.Tensor], head_num: int,

@@ -58,13 +58,17 @@ __device__ __forceinline__ uint32_t kv_quant_code(float x, float inv_s, float z)
 // output bits of this kernel are pinned by tests/test_gpu_attention.py::test_decode_attention_output_bits_are_pinned.
 constexpr int kAttnThreadsV2 = kAttnConsumers;  // no dedicated producer warp: every warp streams its own half pages
 
-template <int BITS>
+// SHARED (the row pass of qs_shared_prefix_decode_attention, DESIGN.md 3.10): the row's pages start at row_pages[b]; a row with
+// row_pages[b] > 0 has part_stride - nsplit more partials per head, written by shared_prefix_attention_kernel at slots nsplit .., and its final
+// merge takes them after its own splits.  Without SHARED the two trailing arguments are not read.
+template <int BITS, bool SHARED = false>
 __global__ void __launch_bounds__(kAttnThreadsV2, 4)
 decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restrict__ k_in, const __half* __restrict__ v_in, long long q_stride,
                         long long k_stride, long long v_stride, const long long* __restrict__ kv_pointers, const int* __restrict__ lengths,
                         __half* __restrict__ out, int num_heads, int num_kv_heads, int max_blocks, PageGeom pg, float rotary_base, int rotary_dim,
                         int timestep, int nsplit, float* __restrict__ ws_part, uint32_t* __restrict__ ws_cnt, uint32_t* __restrict__ tok_cnt, int8_t* __restrict__ q_out,
-                        __half* __restrict__ q_scale, __half* __restrict__ q_sum, unsigned long long* __restrict__ prof) {
+                        __half* __restrict__ q_scale, __half* __restrict__ q_sum, unsigned long long* __restrict__ prof, const int* __restrict__ row_pages,
+                        int part_stride) {
   using SL = StageLayout<BITS>;
   constexpr int R = SL::kStages;
   const int G = num_heads / num_kv_heads;
@@ -111,9 +115,13 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
   const long long* kptrs = kv_pointers + (static_cast<size_t>(b) * 2 + 0) * max_blocks;
   const long long* vptrs = kv_pointers + (static_cast<size_t>(b) * 2 + 1) * max_blocks;
   const int n_pages = (tlen + kPageTokens - 1) / kPageTokens;
-  const int pps = (n_pages + nsplit - 1) / nsplit;
-  const int p_begin = split * pps, p_end = min(n_pages, p_begin + pps);
+  const int p_first = SHARED ? row_pages[b] : 0;  // pages below p_first are the group's: the shared pass reads them
+  const int pps = (n_pages - p_first + nsplit - 1) / nsplit;
+  const int p_begin = p_first + split * pps, p_end = min(n_pages, p_begin + pps);
   const int last_blk = tlen / pg.tokens_per_block;  // page receiving the new token
+  // partials of the final merge per (row, head): this launch's splits, then (SHARED, rows in a group) the shared pass's
+  const int ptot = (SHARED && p_first > 0) ? part_stride : nsplit;
+  const int pstride = SHARED ? part_stride : nsplit;
 
   // ---- this warp's stream: token slice [32 (warp & 1), +32) of the pages p_begin + (warp >> 1), +2, ...  ----
   const int hslice = warp & 1;
@@ -155,19 +163,11 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
     }
     const __half vnew = vg[threadIdx.x];
     float sn, cs;
-    {
-      const float inv_freq = __fdiv_rn(static_cast<float>(tlen), powf(rotary_base, __fdiv_rn(static_cast<float>(2 * ri), static_cast<float>(rotary_dim))));
-      sincosf(inv_freq, &sn, &cs);
-    }
+    rope_sincos(tlen, ri, rotary_base, rotary_dim, sn, cs);
 #pragma unroll
     for (int e = 0; e < kRowsPerThread; ++e) {
       const int r = r0 + 2 * e;
-      if (r <= Gc) {
-        __half* dst = (r < Gc) ? (s_q + r * kD) : s_k;
-        const float f0 = __half2float(x0[e]), f1 = __half2float(x1[e]);
-        dst[ri] = __float2half_rn(__fsub_rn(__fmul_rn(cs, f0), __fmul_rn(sn, f1)));
-        dst[ri + half_rot] = __float2half_rn(__fadd_rn(__fmul_rn(cs, f1), __fmul_rn(sn, f0)));
-      }
+      if (r <= Gc) rope_store((r < Gc) ? (s_q + r * kD) : s_k, ri, half_rot, x0[e], x1[e], sn, cs);
     }
     s_v[threadIdx.x] = vnew;
     for (int i = threadIdx.x + Gc * kD; i < kMaxG * kD; i += kAttnConsumers) s_q[i] = __float2half_rn(0.f);
@@ -303,21 +303,21 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
 
   // ---------------- merge the warps (and the un-quantised new token) ----------------
   const int nparts = kWarps + (split == 0 ? 1 : 0);
-  if (threadIdx.x < kMaxG) merge_weights<kMaxG>(threadIdx.x, nparts, nsplit, s_m, s_l, s_f);
+  if (threadIdx.x < kMaxG) merge_weights<kMaxG>(threadIdx.x, nparts, ptot, s_m, s_l, s_f);
   __syncthreads();
   if (threadIdx.x < kD) {
     const int d = 16 * (threadIdx.x & 7) + (threadIdx.x >> 3);  // the dim whose partials sit at offset threadIdx.x
     float* part = nullptr;
-    if (nsplit > 1) part = ws_part + ((static_cast<size_t>(b) * num_heads + h0) * nsplit + split) * (kD + 2);
+    if (ptot > 1) part = ws_part + ((static_cast<size_t>(b) * num_heads + h0) * pstride + split) * (kD + 2);
     const float vd = __half2float(s_v[d]);
 #pragma unroll
     for (int r = 0; r < kMaxG; ++r) {
       if (r < Gc) {
         const float acc = merge_warps<BITS, kMaxG>(s_ring, r, vd, s_f);
-        if (nsplit == 1) {
+        if (ptot == 1) {
           out[(static_cast<size_t>(b) * num_heads + h0 + r) * kD + d] = __float2half_rn(acc);
         } else {
-          float* pr = part + static_cast<size_t>(r) * nsplit * (kD + 2);
+          float* pr = part + static_cast<size_t>(r) * pstride * (kD + 2);
           pr[d] = acc;
           if (threadIdx.x == 0) {
             pr[kD] = s_m[0][r];
@@ -329,15 +329,16 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
   }
   qs_trace(QS_K_ATTN, 2);
   if (threadIdx.x == 0) ATTN_PROF(8);
-  bool final_written = (nsplit == 1);  // this CTA produced the final fp16 outputs of its head group
-  if (nsplit > 1) {
+  bool final_written = (ptot == 1);  // this CTA produced the final fp16 outputs of its head group
+  if (ptot > 1) {
+    // SHARED: the shared pass finished before this grid passed its dependency wait, so its partials are complete
     final_written = arrive_last(ws_cnt + static_cast<size_t>(b) * gridDim.x + blockIdx.x, nsplit, s_last);
     if (final_written && threadIdx.x < kD) {
       const int d = threadIdx.x;
       __threadfence();
       for (int r = 0; r < Gc; ++r) {
-        const float* pr = ws_part + (static_cast<size_t>(b) * num_heads + h0 + r) * nsplit * (kD + 2);
-        out[(static_cast<size_t>(b) * num_heads + h0 + r) * kD + d] = __float2half_rn(merge_splits(pr, nsplit, d));
+        const float* pr = ws_part + (static_cast<size_t>(b) * num_heads + h0 + r) * pstride * (kD + 2);
+        out[(static_cast<size_t>(b) * num_heads + h0 + r) * kD + d] = __float2half_rn(merge_splits(pr, ptot, d));
       }
     }
   }
@@ -430,6 +431,217 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
   }
   if (threadIdx.x == 0) ATTN_PROF(9);
 #undef ATTN_PROF
+}
+
+// ------------------------------------------------------------------------------------------------
+// K1s: shared pass of qs_shared_prefix_decode_attention (DESIGN.md 3.10).  Rows forked from one prompt share the pages 0 .. S_g - 1 of their
+//   group g.  One CTA owns (KV head, column part, group, context split); column c of part cp is (member j, query head h) with C cp + c = j G + h,
+//   so every code a warp unpacks feeds C = 8 NT columns, as in multi_token_attention_kernel (DESIGN.md 3.6).  Member j's q is rotated at its
+//   own position lengths[row_j] - 1 (members diverge once a finished row stops advancing) through the decode kernel's RoPE functions.
+//   Every shared token is valid for every member (the caller guarantees 64 S_g cached tokens), so there is no causal tail, no own token and
+//   no append.  The CTA writes one unnormalised partial (O, max, sum) per (member row, head) at split slot part_off + split of the row's
+//   partials; the row pass (decode_attention_kernel<BITS, true>) merges them after its own splits.
+// ------------------------------------------------------------------------------------------------
+struct SharedPrefixParams {
+  const __half* q;                // [B, Hq * 128] rows of q_stride halfs (un-rotated)
+  long long q_stride;
+  const int* lengths;             // [B] context length including the new token
+  const long long* kv_pointers;   // [B, 2, max_blocks]
+  const int* group_offsets;       // [num_groups + 1]
+  const int* group_rows;          // rows of group g: group_rows[group_offsets[g] .. group_offsets[g + 1])
+  const int* group_pages;         // [num_groups] shared pages S_g, read through the table of the group's first row
+  int num_heads, num_kv_heads, max_blocks;
+  int cparts, nsplit;             // column parts per KV head, context splits of the shared pages
+  int part_off, part_stride;      // slot of split 0 among a row's partials, partials per (row, head)
+  PageGeom pg;
+  float rotary_base;
+  int rotary_dim;
+  float* ws_part;                 // [B, Hq, part_stride, 130]
+};
+
+// ptxas needs more than 128 registers for two n8 tiles without spilling (the O^T accumulators alone are 32 per tile), as in
+// multi_token_attention_kernel
+template <int NT>
+constexpr int kSharedMinBlocks = NT == 1 ? 3 : 2;
+
+template <int BITS, int NT>
+__global__ void __launch_bounds__(kAttnConsumers, kSharedMinBlocks<NT>) shared_prefix_attention_kernel(const SharedPrefixParams p) {
+  using SL = StageLayout<BITS>;
+  constexpr int R = SL::kStages;
+  constexpr int C = 8 * NT;
+  static_assert(SL::kWarpBytes >= C * kOStride * 4, "the per-warp ring must hold the warp's partial output");
+  const int G = p.num_heads / p.num_kv_heads;
+  const int hk = blockIdx.x / p.cparts;
+  const int col0 = (blockIdx.x - hk * p.cparts) * C;
+  const int grp = blockIdx.y;
+  const int split = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, q4 = lane & 3;
+
+  // the layout and the tables are prepared by the host before the step: read before the dependency wait; q and the pages after it
+  const int mem0 = p.group_offsets[grp];
+  const int nmem = p.group_offsets[grp + 1] - mem0;
+  const int S = p.group_pages[grp];
+  const int ncol = min(C, G * nmem - col0);
+  if (ncol <= 0 || S <= 0) return;  // uniform over the CTA; a group without shared pages has no partials (its rows have row_pages 0)
+
+  extern __shared__ __align__(128) uint8_t smem_attn[];
+  uint8_t* s_ring = smem_attn;
+  __shared__ __align__(16) __half s_q[C * kD];
+  __shared__ uint4 s_qb[NT][4][32];
+  __shared__ float s_m[kWarps + 1][C], s_l[kWarps + 1][C];
+  __shared__ float s_f[kWarps + 1][C];
+  __shared__ float2 s_meta[kWarps][2][kSliceTokens];
+  __shared__ __align__(8) uint64_t s_full[kWarps][R];
+
+  if (lane == 0) {
+    for (int i = 0; i < R; ++i) mbar_init(&s_full[warp][i], 1);
+    fence_barrier_init();
+  }
+  __syncwarp();
+  if (threadIdx.x == 0) pdl_launch_dependents();
+
+  const int row0 = p.group_rows[mem0];
+  const long long* kptrs = p.kv_pointers + (static_cast<size_t>(row0) * 2 + 0) * p.max_blocks;
+  const long long* vptrs = p.kv_pointers + (static_cast<size_t>(row0) * 2 + 1) * p.max_blocks;
+  const int pps = (S + p.nsplit - 1) / p.nsplit;
+  const int p_begin = split * pps, p_end = min(S, p_begin + pps);
+  const int hslice = warp & 1;
+  const int my_first = p_begin + (warp >> 1);
+  const int n_my = (p_end > my_first) ? (p_end - my_first + 1) / 2 : 0;
+  uint8_t* my_ring = s_ring + warp * SL::kWarpBytes;
+  uint64_t* my_full = &s_full[warp][0];
+  const int zoff = p.pg.num_kv_heads * p.pg.tokens_per_block * 2;
+  long long kp_l = 0, vp_l = 0;
+  auto load_ptr_batch = [&](int j0) { slice_ptrs(kptrs, vptrs, my_first + 2 * (j0 + lane), p_end, kp_l, vp_l); };
+  auto issue = [&](int j, int slot) {
+    issue_slice<BITS>(lane, kp_l, vp_l, j, my_ring + slot * SL::kBytes, &my_full[slot], hk, hslice, p.pg.code_bytes, zoff);
+  };
+  load_ptr_batch(0);
+  // thread t rotates the pair (ri, ri + 64) of columns t / 64, t / 64 + 2, ...: the member rows and positions of those columns
+  const int ri = threadIdx.x & 63, c0 = threadIdx.x >> 6;
+  const int half_rot = p.rotary_dim / 2;
+  pdl_wait();
+  for (int j = 0; j < R && j < n_my; ++j) issue(j, j);
+
+  {
+    int last_pos = -1;
+    float sn = 0.f, cs = 1.f;
+    for (int c = c0; c < C; c += 2) {
+      __half* dst = s_q + c * kD;
+      if (c < ncol) {
+        const int j = (col0 + c) / G, h = col0 + c - j * G;
+        const int row = p.group_rows[mem0 + j];
+        const int pos = p.lengths[row] - 1;
+        const __half* src = p.q + static_cast<size_t>(row) * p.q_stride + static_cast<size_t>(hk * G + h) * kD;
+        const __half x0 = src[ri], x1 = src[ri + half_rot];
+        if (pos != last_pos) {
+          rope_sincos(pos, ri, p.rotary_base, p.rotary_dim, sn, cs);
+          last_pos = pos;
+        }
+        rope_store(dst, ri, half_rot, x0, x1, sn, cs);
+      } else {
+        dst[ri] = dst[ri + half_rot] = __float2half_rn(0.f);
+      }
+    }
+  }
+  __syncthreads();
+
+  float sumq[NT][2], biasq[NT][2];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+    uint32_t qb0[8], qb1[8];
+    q_operand<BITS>(s_q + (8 * t + g) * kD + 32 * q4, q4, qb0, qb1, sumq[t], biasq[t]);
+    if (warp == 0) {
+#pragma unroll
+      for (int w = 0; w < 4; ++w) s_qb[t][w][lane] = make_uint4(qb0[2 * w], qb1[2 * w], qb0[2 * w + 1], qb1[2 * w + 1]);
+    }
+  }
+  __syncthreads();
+  auto qb = [&](int t, int ks, uint32_t& b0, uint32_t& b1) {
+    const uint4 qq = s_qb[t][ks >> 1][lane];
+    b0 = (ks & 1) ? qq.z : qq.x;
+    b1 = (ks & 1) ? qq.w : qq.y;
+  };
+
+  const float sm_scale = rsqrtf(static_cast<float>(kD)) * 1.4426950408889634f;  // the decode kernel's
+  float o[NT][8][4];
+  float m[NT][2], l[NT][2], cr[NT][2], spa[NT][4];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) o[t][i][0] = o[t][i][1] = o[t][i][2] = o[t][i][3] = 0.f;
+    m[t][0] = m[t][1] = -CUDART_INF_F;
+    l[t][0] = l[t][1] = cr[t][0] = cr[t][1] = 0.f;
+    spa[t][0] = spa[t][1] = spa[t][2] = spa[t][3] = 0.f;
+  }
+
+  const int tokA = (g & 1) * 4 + (g >> 1);
+  constexpr int kRow = kD * BITS / 8;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < n_my; ++j) {
+    mbar_wait(&my_full[s], ph);
+    const uint8_t* st = my_ring + s * SL::kBytes;
+    slice_meta<BITS>(st, lane, false, sm_scale, s_meta[warp][0], s_meta[warp][1]);
+    __syncwarp();
+    float sc[2][NT][4];
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+#pragma unroll
+      for (int t = 0; t < NT; ++t) sc[c][t][0] = sc[c][t][1] = sc[c][t][2] = sc[c][t][3] = 0.f;
+      qk_chunk<BITS, NT>(st + SL::kOffK + (c * kChunk + tokA) * kRow, q4, sc[c], qb);
+    }
+    float tl[2][NT][4], vs[2][2], vc[2][2];
+#pragma unroll
+    for (int c = 0; c < 2; ++c) chunk_logits<NT>(s_meta[warp][0], s_meta[warp][1], c, tokA, sc[c], biasq, sumq, tl[c], vs[c], vc[c]);
+    uint32_t bp[2][NT][2];
+#pragma unroll
+    for (int t = 0; t < NT; ++t) softmax_tile<NT, false>(t, tl, vs, vc, m[t], l[t], cr[t], spa[t], o[t], bp);
+#pragma unroll
+    for (int c = 0; c < 2; ++c) pv_chunk<BITS, NT>(st + SL::kOffV + (c * kChunk + q4) * kRow, g, o, bp[c]);
+    __syncwarp();
+    if (j + R < n_my) {
+      if (((j + R) & 31) == 0) load_ptr_batch(j + R);
+      issue(j + R, s);
+    }
+    if (++s == R) { s = 0; ph ^= 1; }
+  }
+
+#pragma unroll
+  for (int t = 0; t < NT; ++t) reduce_tile_sums(l[t], cr[t]);
+  if (g == 0) {
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      s_m[warp][8 * t + 2 * q4] = m[t][0]; s_m[warp][8 * t + 2 * q4 + 1] = m[t][1];
+      s_l[warp][8 * t + 2 * q4] = l[t][0]; s_l[warp][8 * t + 2 * q4 + 1] = l[t][1];
+    }
+  }
+  __syncwarp();
+#pragma unroll
+  for (int t = 0; t < NT; ++t) store_partial<BITS>(reinterpret_cast<float*>(my_ring) + (8 * t + 2 * q4) * kOStride + g, o[t], spa[t], cr[t]);
+  __syncthreads();
+
+  // merge the warps; never normalised here (nsplit argument 0): the row pass normalises after its merge of every part
+  if (threadIdx.x < C) merge_weights<C>(threadIdx.x, kWarps, 0, s_m, s_l, s_f);
+  __syncthreads();
+  if (threadIdx.x < kD) {
+    const int d = 16 * (threadIdx.x & 7) + (threadIdx.x >> 3);
+#pragma unroll
+    for (int r = 0; r < C; ++r) {
+      if (r < ncol) {
+        const float acc = merge_warps<BITS, C>(s_ring, r, 0.f, s_f);
+        const int j = (col0 + r) / G, h = col0 + r - j * G;
+        const int row = p.group_rows[mem0 + j];
+        float* pr = p.ws_part + ((static_cast<size_t>(row) * p.num_heads + hk * G + h) * p.part_stride + p.part_off + split) * (kD + 2);
+        pr[d] = acc;
+        if (threadIdx.x == 0) {
+          pr[kD] = s_m[0][r];
+          pr[kD + 1] = s_l[0][r];
+        }
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -551,7 +763,139 @@ __global__ void padding_offsets_kernel(int* __restrict__ out, const int* __restr
 constexpr size_t kAttnCounterBytes = 256 * 1024;  // 49152 (sequence, head-group) split counters + 16384 per-token counters
 constexpr size_t kAttnTokCounterOffset = 192 * 1024;
 
+// ---- launch plan of qs_shared_prefix_decode_attention: a function of host integers only, so the call can be captured in a graph ----
+template <int BITS, int NT>
+int shared_resident_ctas() {
+  static int cached[kMaxDevices] = {};
+  int& r = cached[device_ordinal()];
+  if (r == 0) {
+    const int smem = kWarps * StageLayout<BITS>::kWarpBytes;
+    int n = 0;
+    if (raise_smem_limit(shared_prefix_attention_kernel<BITS, NT>, smem, "shared_prefix_decode_attention smem attribute") != QS_OK ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, shared_prefix_attention_kernel<BITS, NT>, kAttnConsumers, smem) != cudaSuccess || n < 1) {
+      cudaGetLastError();
+      n = 1;
+    }
+    r = n;
+  }
+  return r;
+}
+
+struct SharedPrefixPlan {
+  int gx;          // row pass: KV heads x head groups of <= 8 query heads
+  int nsplit;      // row pass context splits (decode_attention's rule)
+  int ntile;       // shared pass: n8 tiles per CTA (C = 8 ntile columns of (member, query head))
+  int cparts;      // shared pass: column parts per KV head
+  int sp_nsplit;   // shared pass: context splits of the shared pages (0: no shared pass)
+  size_t part_bytes, row_bytes;
+};
+
+SharedPrefixPlan plan_shared_prefix(int bits, int batch, int num_heads, int num_kv_heads, int timestep, int num_groups, int max_group, int max_pages) {
+  SharedPrefixPlan pl{};
+  const int G = num_heads / num_kv_heads;
+  pl.gx = num_kv_heads * ((G + kMaxG - 1) / kMaxG);
+  pl.nsplit = 1;
+  const int ctas = pl.gx * batch, slots = num_sms() * 4;
+  if (2 * ctas <= slots && timestep > 512) pl.nsplit = std::min(std::min((slots + ctas - 1) / ctas, (timestep + 255) / 256), 32);
+  if (num_groups > 0 && max_group > 0 && max_pages > 0) {
+    const int cols = G * max_group;
+    pl.ntile = cols <= 8 ? 1 : 2;
+    pl.cparts = (cols + 8 * pl.ntile - 1) / (8 * pl.ntile);
+    const long long sctas = static_cast<long long>(num_kv_heads) * pl.cparts * num_groups;
+    const int per_sm = bits == 4 ? (pl.ntile == 1 ? shared_resident_ctas<4, 1>() : shared_resident_ctas<4, 2>())
+                                 : (pl.ntile == 1 ? shared_resident_ctas<8, 1>() : shared_resident_ctas<8, 2>());
+    const long long sslots = static_cast<long long>(num_sms()) * per_sm;
+    const int ctx = max_pages * kPageTokens;
+    pl.sp_nsplit = 1;
+    if (2 * sctas <= sslots && ctx > 512)
+      pl.sp_nsplit = static_cast<int>(std::min<long long>(std::min<long long>((sslots + sctas - 1) / sctas, (ctx + 255) / 256), 32));
+  }
+  pl.part_bytes = static_cast<size_t>(batch) * num_heads * (pl.nsplit + pl.sp_nsplit) * (kD + 2) * sizeof(float);
+  pl.row_bytes = static_cast<size_t>(batch) * num_heads * kD * sizeof(__half);
+  return pl;
+}
+
 }  // namespace
+
+size_t shared_prefix_attention_workspace_bytes(int batch, int num_heads, int num_kv_heads, int timestep, int num_groups, int max_group, int max_pages,
+                                               int int4_kv) {
+  if (batch <= 0 || num_kv_heads <= 0 || num_heads % num_kv_heads != 0) return 0;
+  const SharedPrefixPlan pl = plan_shared_prefix(int4_kv ? 4 : 8, batch, num_heads, num_kv_heads, timestep, num_groups, max_group, max_pages);
+  return kAttnCounterBytes + pl.part_bytes + pl.row_bytes;
+}
+
+int shared_prefix_decode_attention(const SharedPrefixAttnArgs& s) {
+  const DecodeAttnArgs& a = s.d;
+  QS_REQUIRE(a.head_dim == kD, "shared_prefix_decode_attention: head_dim=%d, only 128 is supported", a.head_dim);
+  QS_REQUIRE(a.kv_zeros, "shared_prefix_decode_attention: only kv_cache_with_zeros=True is supported");
+  QS_REQUIRE(a.num_kv_heads > 0 && a.num_heads % a.num_kv_heads == 0, "shared_prefix_decode_attention: heads %d / kv heads %d", a.num_heads,
+             a.num_kv_heads);
+  QS_REQUIRE(a.tokens_per_block == kPageTokens, "shared_prefix_decode_attention: tokens_per_block=%d, only 64 is supported", a.tokens_per_block);
+  QS_REQUIRE(a.rotary_dim == kD, "shared_prefix_decode_attention: rotary_dim=%d must equal head_dim", a.rotary_dim);
+  const int bits = a.int4_kv ? 4 : 8;
+  QS_REQUIRE(a.size_per_token == a.num_kv_heads * kD * bits / 8, "shared_prefix_decode_attention: size_per_token=%d does not match %d kv heads x %d bits",
+             a.size_per_token, a.num_kv_heads, bits);
+  QS_REQUIRE(a.batch >= 0 && a.batch <= 16384, "shared_prefix_decode_attention: batch=%d, must be 0 .. 16384", a.batch);
+  QS_REQUIRE(s.num_groups >= 0 && s.num_groups <= 65535 && s.max_group >= 0 && s.max_pages >= 0,
+             "shared_prefix_decode_attention: num_groups=%d, max_group=%d, max_pages=%d", s.num_groups, s.max_group, s.max_pages);
+  QS_REQUIRE(s.max_pages <= a.max_blocks, "shared_prefix_decode_attention: max_pages=%d exceeds the page table (%d blocks)", s.max_pages, a.max_blocks);
+  if (a.batch == 0) return QS_OK;
+  QS_REQUIRE(a.q && a.k && a.v && a.kv_pointers && a.lengths && s.row_pages && (a.out != nullptr) != (a.q_out != nullptr),
+             "shared_prefix_decode_attention: null tensor, or not exactly one of out / out_q");
+  QS_REQUIRE(s.num_groups == 0 || (s.group_offsets && s.group_rows && s.group_pages), "shared_prefix_decode_attention: null group layout");
+  QS_REQUIRE(a.q_out == nullptr || a.q_scale != nullptr, "shared_prefix_decode_attention: q_scale is null");
+  QS_REQUIRE(a.q_stride % 8 == 0 && (reinterpret_cast<uintptr_t>(a.q) & 15) == 0, "shared_prefix_decode_attention: q rows must be 16-byte aligned");
+  const SharedPrefixPlan pl = plan_shared_prefix(bits, a.batch, a.num_heads, a.num_kv_heads, a.timestep, s.num_groups, s.max_group, s.max_pages);
+  QS_REQUIRE(static_cast<size_t>(a.batch) * pl.gx * 4 <= kAttnTokCounterOffset, "shared_prefix_decode_attention: batch %d x %d head groups too large",
+             a.batch, pl.gx);
+  const size_t need = kAttnCounterBytes + pl.part_bytes + pl.row_bytes;
+  QS_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= need,
+             "shared_prefix_decode_attention: workspace of %zu bytes, need %zu (qs_shared_prefix_attention_workspace_bytes)", a.workspace_bytes, need);
+  uint8_t* ws = static_cast<uint8_t*>(a.workspace);
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(ws);
+  uint32_t* tok_cnt = reinterpret_cast<uint32_t*>(ws + kAttnTokCounterOffset);
+  float* part = reinterpret_cast<float*>(ws + kAttnCounterBytes);
+  void* out = a.q_out != nullptr ? ws + kAttnCounterBytes + pl.part_bytes : a.out;
+  const int pstride = pl.nsplit + pl.sp_nsplit;
+  PageGeom pg{kPageTokens, kPageTokens * a.size_per_token, a.num_kv_heads};
+  const size_t smem = static_cast<size_t>(kWarps) * (bits == 4 ? StageLayout<4>::kWarpBytes : StageLayout<8>::kWarpBytes);
+  if (pl.sp_nsplit > 0) {
+    SharedPrefixParams p{};
+    p.q = static_cast<const __half*>(a.q);
+    p.q_stride = a.q_stride;
+    p.lengths = a.lengths;
+    p.kv_pointers = a.kv_pointers;
+    p.group_offsets = s.group_offsets;
+    p.group_rows = s.group_rows;
+    p.group_pages = s.group_pages;
+    p.num_heads = a.num_heads; p.num_kv_heads = a.num_kv_heads; p.max_blocks = a.max_blocks;
+    p.cparts = pl.cparts; p.nsplit = pl.sp_nsplit;
+    p.part_off = pl.nsplit; p.part_stride = pstride;
+    p.pg = pg;
+    p.rotary_base = a.rotary_base; p.rotary_dim = a.rotary_dim;
+    p.ws_part = part;
+    const dim3 grid(static_cast<unsigned>(a.num_kv_heads * pl.cparts), s.num_groups, pl.sp_nsplit);
+    auto run = [&](auto kern) {
+      const int rc = raise_smem_limit(kern, smem, "shared_prefix_decode_attention smem attribute");
+      if (rc) return rc;
+      return launch(kern, grid, dim3(kAttnConsumers), smem, 0, a.stream, "shared_prefix_decode_attention", p);
+    };
+    const int rc = bits == 4 ? (pl.ntile == 1 ? run(shared_prefix_attention_kernel<4, 1>) : run(shared_prefix_attention_kernel<4, 2>))
+                             : (pl.ntile == 1 ? run(shared_prefix_attention_kernel<8, 1>) : run(shared_prefix_attention_kernel<8, 2>));
+    if (rc) return rc;
+  }
+  const dim3 grid(pl.gx, a.batch, pl.nsplit);
+  auto run = [&](auto kern) {
+    const int rc = raise_smem_limit(kern, smem, "attention smem attribute");
+    if (rc) return rc;
+    return launch(kern, grid, dim3(kAttnThreadsV2), smem, 1, a.stream, "shared_prefix_decode_attention rows", static_cast<const __half*>(a.q),
+                  static_cast<const __half*>(a.k), static_cast<const __half*>(a.v), a.q_stride, a.k_stride, a.v_stride, a.kv_pointers, a.lengths,
+                  static_cast<__half*>(out), a.num_heads, a.num_kv_heads, a.max_blocks, pg, a.rotary_base, a.rotary_dim, a.timestep, pl.nsplit, part, cnt,
+                  a.q_out != nullptr ? tok_cnt : nullptr, static_cast<int8_t*>(a.q_out), static_cast<__half*>(a.q_scale), static_cast<__half*>(a.q_sum),
+                  static_cast<unsigned long long*>(nullptr), s.row_pages, pstride);
+  };
+  return bits == 4 ? run(decode_attention_kernel<4, true>) : run(decode_attention_kernel<8, true>);
+}
 
 size_t attention_workspace_bytes(int batch, int num_heads, int head_dim, int max_splits) {
   return kAttnCounterBytes + static_cast<size_t>(batch) * num_heads * max_splits * (head_dim + 2) * sizeof(float) +
@@ -617,7 +961,7 @@ int decode_attention(const DecodeAttnArgs& a) {
                   static_cast<const __half*>(a.k), static_cast<const __half*>(a.v), a.q_stride, a.k_stride, a.v_stride, a.kv_pointers, a.lengths,
                   static_cast<__half*>(out), a.num_heads, a.num_kv_heads, a.max_blocks, pg, a.rotary_base, a.rotary_dim, a.timestep, nsplit, part, cnt,
                   tok_cnt, static_cast<int8_t*>(a.q_out), static_cast<__half*>(a.q_scale), static_cast<__half*>(a.q_sum),
-                  static_cast<unsigned long long*>(a.prof));
+                  static_cast<unsigned long long*>(a.prof), static_cast<const int*>(nullptr), 0);
   };
   QS_REQUIRE(a.tokens_per_block == kPageTokens, "single_query_attention: tokens_per_block=%d, only 64 is supported (cache_engine block_size)", a.tokens_per_block);
   return a.int4_kv ? run(decode_attention_kernel<4>, static_cast<size_t>(kWarps) * StageLayout<4>::kWarpBytes)

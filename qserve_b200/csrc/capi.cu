@@ -287,6 +287,30 @@ int qs_kv_cache_compact(const int64_t* kv_pointers, const int32_t* start_pos, co
   return kv_cache_compact(a);
 }
 
+int qs_shared_prefix_decode_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride,
+                                      const int64_t* kv_pointers, const int32_t* length_per_sample, const int32_t* group_offsets,
+                                      const int32_t* group_rows, const int32_t* group_pages, const int32_t* row_pages, void* out, int8_t* out_q,
+                                      void* out_scale, void* out_sum, int batch, int num_heads, int num_kv_heads, int head_dim, int max_blocks_per_seq,
+                                      int tokens_per_block, int size_per_token, int timestep, int rotary_embedding_dim, float rotary_base,
+                                      int int4_kv_cache, int num_groups, int max_group, int max_pages, void* workspace, size_t workspace_bytes,
+                                      void* stream) {
+  SharedPrefixAttnArgs s;
+  DecodeAttnArgs& a = s.d;
+  a.q = q; a.k = k; a.v = v; a.q_stride = q_stride; a.k_stride = k_stride; a.v_stride = v_stride;
+  a.kv_pointers = reinterpret_cast<const long long*>(kv_pointers); a.lengths = length_per_sample; a.out = out;
+  a.q_out = out_q; a.q_scale = out_scale; a.q_sum = out_sum; a.workspace = workspace; a.workspace_bytes = workspace_bytes;
+  a.batch = batch; a.num_heads = num_heads; a.num_kv_heads = num_kv_heads; a.head_dim = head_dim; a.max_blocks = max_blocks_per_seq;
+  a.tokens_per_block = tokens_per_block; a.size_per_token = size_per_token; a.timestep = timestep;
+  a.rotary_dim = rotary_embedding_dim; a.rotary_base = rotary_base; a.int4_kv = int4_kv_cache; a.kv_zeros = 1; a.stream = stream;
+  s.group_offsets = group_offsets; s.group_rows = group_rows; s.group_pages = group_pages; s.row_pages = row_pages;
+  s.num_groups = num_groups; s.max_group = max_group; s.max_pages = max_pages;
+  return shared_prefix_decode_attention(s);
+}
+size_t qs_shared_prefix_attention_workspace_bytes(int batch, int num_heads, int num_kv_heads, int timestep, int num_groups, int max_group, int max_pages,
+                                                  int int4_kv_cache) {
+  return shared_prefix_attention_workspace_bytes(batch, num_heads, num_kv_heads, timestep, num_groups, max_group, max_pages, int4_kv_cache);
+}
+
 int qs_kv_cache_fork(const int64_t* kv_pointers, const int32_t* parents, const int32_t* children, const int32_t* lens, int num_layers, int batch,
                      int num_pairs, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token, int int4_kv_cache, void* stream) {
   KvForkArgs a;

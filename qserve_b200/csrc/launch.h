@@ -87,6 +87,19 @@ struct DecodeAttnArgs {
 };
 int decode_attention(const DecodeAttnArgs& a);
 size_t attention_workspace_bytes(int batch, int num_heads, int head_dim, int max_splits);
+// decode attention of rows that share the first pages of their group (qs_shared_prefix_decode_attention): d as for decode_attention (exactly
+// one of d.out / d.q_out; d.lengths required; d.workspace >= shared_prefix_attention_workspace_bytes), plus the group layout
+struct SharedPrefixAttnArgs {
+  DecodeAttnArgs d;
+  const int* group_offsets = nullptr;  // [num_groups + 1]
+  const int* group_rows = nullptr;     // [group_offsets[num_groups]]
+  const int* group_pages = nullptr;    // [num_groups] shared pages S_g
+  const int* row_pages = nullptr;      // [batch] S of the row's group, 0 outside groups
+  int num_groups = 0, max_group = 0, max_pages = 0;  // host bounds that plan the launches
+};
+int shared_prefix_decode_attention(const SharedPrefixAttnArgs& a);
+size_t shared_prefix_attention_workspace_bytes(int batch, int num_heads, int num_kv_heads, int timestep, int num_groups, int max_group, int max_pages,
+                                               int int4_kv);
 
 struct PrefillAppendArgs {
   void* qkv = nullptr;  // fp16 [T, (Hq + 2 Hkv) * D], q and k rotated in place

@@ -159,6 +159,19 @@ __device__ __forceinline__ void q_operand(const __half* qrow, int q4, uint32_t (
   }
 }
 
+// ---- NeoX RoPE of one query / key row at position pos: the pair (i, i + half_rot) of x0 = row[i], x1 = row[i + half_rot] goes to dst, rounded to
+//      fp16.  decode_attention_kernel and shared_prefix_attention_kernel both rotate through these two functions, so a member's q has the
+//      same bits in both passes ----
+__device__ __forceinline__ void rope_sincos(int pos, int i, float rotary_base, int rotary_dim, float& sn, float& cs) {
+  const float inv_freq = __fdiv_rn(static_cast<float>(pos), powf(rotary_base, __fdiv_rn(static_cast<float>(2 * i), static_cast<float>(rotary_dim))));
+  sincosf(inv_freq, &sn, &cs);
+}
+__device__ __forceinline__ void rope_store(__half* dst, int i, int half_rot, __half x0, __half x1, float sn, float cs) {
+  const float f0 = __half2float(x0), f1 = __half2float(x1);
+  dst[i] = __float2half_rn(__fsub_rn(__fmul_rn(cs, f0), __fmul_rn(sn, f1)));
+  dst[i + half_rot] = __float2half_rn(__fadd_rn(__fmul_rn(cs, f1), __fmul_rn(sn, f0)));
+}
+
 // ---- per-token (scale, c = -scale * zero) pairs of the 32 K and 32 V tokens of a slice, converted to fp32 ONCE per token (fp16 -> fp32
 //      conversions run on the slow XU pipe: the logit code must not repeat them per thread); K pre-multiplied by the softmax scale.
 //      `unread`: a slot no column reads (its scale may be anything, NaN included): forced to finite zeros, its logits are masked ----

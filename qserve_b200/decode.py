@@ -103,6 +103,32 @@ class _Rows(NamedTuple):
     q_sum: torch.Tensor     # fp16 [M]
 
 
+def fork_groups(groups: list, parents, children, cached) -> list:
+    """The shared-prefix groups after a fork (DecodeRunner(shared_prefix=True)): groups is a list of (rows, S) with the group's first row
+    first; each parent of the fork and its children form one group with S = cached[parent] // 64 (the parent's full pages, which fork points
+    the children's tables at).  A fork dissolves every earlier group that holds a row it touches."""
+    touched = set(parents) | set(children)
+    kept = [(tuple(rows), int(s)) for rows, s in groups if not touched & set(rows)]
+    new: dict = {}
+    for p, c in zip(parents, children):
+        new.setdefault(int(p), [int(p)]).append(int(c))
+    return kept + [(tuple(rows), int(cached[p]) // 64) for p, rows in new.items()]
+
+
+# Layouts the plain decode step sends to qs_shared_prefix_decode_attention; every other layout keeps single_query_attention_quant.  From the
+# sweep of tools/shared_prefix_bench.py in DESIGN.md 5 (Llama-3-8B heads, B = 64, H100 80GB HBM3, 700 W): with 1024 shared tokens the op took
+# 1.08-2.10x the decode launch at every group size; with 4096 shared tokens and groups of >= 2 rows it took 0.69-0.99x, and groups of one row
+# 1.09-1.36x.  End to end (8 prompts x 8 forks, captured step) ctx 1024 went 3.85 -> 4.45 ms and ctx 4096 5.50 -> 5.31 ms.  Shared prefixes
+# between 1024 and 4096 tokens were not measured and keep the decode kernel.
+SHARED_PREFIX_MIN_ROWS = 2
+SHARED_PREFIX_MIN_PAGES = 64
+
+
+def shared_prefix_route(groups: list) -> bool:
+    """True when the layout has a group of at least SHARED_PREFIX_MIN_ROWS rows sharing at least SHARED_PREFIX_MIN_PAGES pages."""
+    return any(len(rows) >= SHARED_PREFIX_MIN_ROWS and s >= SHARED_PREFIX_MIN_PAGES for rows, s in groups)
+
+
 def prompt_pieces(lens, ctx: int, prompt_tokens: int, chunk: Optional[int] = None) -> list:
     """The pieces of a prompt step (DecodeRunner.prefill), planned on the host: lens (ints, one prompt length per row) -> [(start, [tokens
     of each row in this piece])].  chunk=None: one piece (0, lens).  chunk=C: piece k starts at k C and row b takes min(C, lens[b] - k C)
@@ -130,7 +156,7 @@ class DecodeRunner:
     def __init__(self, model: str = "llama-3-8b", precision: str = "w4a8kv4", batch: int = 64, ctx: int = 1024,
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
-                 verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False, prompt_tokens: int = 0):
+                 verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False, prompt_tokens: int = 0, shared_prefix: bool = False):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
         ctx + verify_len tokens and the activation buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers
         and its random draws exactly as they are without it.
@@ -152,8 +178,17 @@ class DecodeRunner:
 
         prompt_tokens > 0 (single GPU, fused path) adds the prompt step (`prefill`): at most prompt_tokens prompt tokens per piece, so the
         activation buffers hold max(batch * max(1, verify_len), prompt_tokens) rows.  It makes no generator draws: the weights, pages and
-        decode / verify / generate steps are those of prompt_tokens = 0."""
+        decode / verify / generate steps are those of prompt_tokens = 0.
+
+        shared_prefix=True (single GPU, fused path): fork records groups (a parent and its children share the parent's full pages) and prefill
+        dissolves them.  While shared_prefix_route(sp_groups) holds, the plain decode step (forward, capture / step, generate_forward(1),
+        capture_generate(1)) runs its attention through shared_prefix_decode_attention, which reads each group's shared pages once; otherwise
+        through single_query_attention_quant.  The layout lives in buffers made with torch.zeros, so the weights, pages and every step
+        without a group are those of shared_prefix=False.  The plain-step graph keys end in the layout's launch plan: after a fork or prefill
+        that changes it, replaying the old key raises instead of running under a stale plan."""
         assert precision in PRECISIONS, precision
+        assert not shared_prefix or (tp_size == 1 and fused), "shared_prefix is single-GPU and uses the fused path"
+        self.shared_prefix = shared_prefix
         assert prompt_tokens >= 0 and (prompt_tokens == 0 or (tp_size == 1 and fused)), "the prompt step is single-GPU and uses the fused path"
         self.prompt_tokens = prompt_tokens
         assert 0 <= verify_len <= 16, "verify_len: at most 16 draft tokens per sequence"
@@ -283,8 +318,35 @@ class DecodeRunner:
             self._alloc_penalty_buffers()
         if generate:
             self._alloc_generate_buffers()
+        self.sp_groups = []  # shared-prefix groups: (rows, S), the group's first row first
+        self._sp_layout = None  # the layout the plain step passes to shared_prefix_decode_attention (None: single_query_attention_quant)
+        if shared_prefix:
+            z = lambda n: torch.zeros(n, dtype=torch.int32, device=dev)
+            self._sp_buf = (z(batch + 1), z(batch), z(batch), z(batch))  # offsets, rows, pages, row_pages: updated in place (graphs hold them)
 
     # ---------------------------------------------------------------------------------------------------------
+    def _set_groups(self, groups: list) -> None:
+        """Record the shared-prefix groups and write their layout into the persistent buffers."""
+        self.sp_groups = groups
+        self._sp_layout = None
+        if not shared_prefix_route(groups):
+            return
+        lay = _ext.shared_prefix_layout([rows for rows, _ in groups], [s for _, s in groups], self.batch)
+        G, n = lay.num_groups, lay.group_rows.numel()
+        off, rows, pages, row_pages = self._sp_buf
+        off[: G + 1].copy_(lay.group_offsets)
+        rows[:n].copy_(lay.group_rows)
+        pages[:G].copy_(lay.group_pages)
+        row_pages.copy_(lay.row_pages)
+        self._sp_layout = lay._replace(group_offsets=off[: G + 1], group_rows=rows[:n], group_pages=pages[:G], row_pages=row_pages)
+
+    def _sp_key(self) -> tuple:
+        """Suffix of the plain-step graph keys: () without shared_prefix, else the launch plan of the current layout."""
+        if not self.shared_prefix:
+            return ()
+        lay = self._sp_layout
+        return ("shared_prefix",) + ((lay.num_groups, lay.max_group, lay.max_pages) if lay is not None else (None,))
+
     def _row_views(self, M: int) -> _Rows:
         H, W = self.cfg.hidden, self.q_size + 2 * self.kv_size
         a, q = self.act_buffer, self.q_act
@@ -388,6 +450,11 @@ class DecodeRunner:
             return
         cfg = self.cfg
         q, k, v = self._heads(r.qkv)
+        if self._sp_layout is not None:
+            _ext.shared_prefix_decode_attention(q, k, v, self.block_tables[li], self.context_lens, self._sp_layout, 64, self.size_per_token,
+                                                self.max_seq_len, cfg.head_dim, cfg.rope_theta, self.kv_bits == 4, True, out_q=r.q_attn,
+                                                out_scale=r.q_scale, out_sum=r.q_sum if self.act_sum else None)
+            return
         _ext.single_query_attention_quant(q, k, v, self.block_tables[li], self.context_lens, min(8192, cfg.max_pos), 64, self.size_per_token,
                                           self.max_seq_len, cfg.head_dim, cfg.rope_theta, self.kv_bits == 4, True, r.q_attn, r.q_scale,
                                           r.q_sum if self.act_sum else None)
@@ -704,7 +771,7 @@ class DecodeRunner:
 
     def _generate_key(self, n: int, branches: int, ngram: tuple, sampled: bool, penalties: bool = False, logprobs: int = 0):
         extra = (bool(penalties), int(logprobs)) if penalties or logprobs else ()  # the keys without the sampler flags are those of before
-        return ("generate", int(n), int(branches), tuple(int(x) for x in ngram), bool(sampled)) + extra
+        return ("generate", int(n), int(branches), tuple(int(x) for x in ngram), bool(sampled)) + extra + (self._sp_key() if n == 1 else ())
 
     def capture_generate(self, n: int = 1, branches: int = 1, ngram: tuple = (1, 4), sampled: bool = False, warmup: int = 2, penalties: bool = False,
                          logprobs: int = 0) -> None:
@@ -761,6 +828,8 @@ class DecodeRunner:
         if prompt_logprobs:
             self._alloc_prompt_logprobs(cu_all, int(prompt_logprobs))
         self.block_tables.copy_(self.own_tables)
+        if self.shared_prefix:
+            self._set_groups([])
         D, int4, max_pos = cfg.head_dim, self.kv_bits == 4, min(8192, cfg.max_pos)
         last = torch.empty((B, cfg.hidden), dtype=torch.half, device=dev)
         i32 = lambda v: torch.tensor(v, dtype=torch.int32, device=dev)
@@ -888,6 +957,8 @@ class DecodeRunner:
             state += list(self.g_top_view(self.g_top_n))
         for t in {id(t): t for t in state}.values():  # g_start may alias v_start
             t[chi] = t[par]
+        if self.shared_prefix:
+            self._set_groups(fork_groups(self.sp_groups, parents, children, cached.tolist()))
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
@@ -979,13 +1050,16 @@ class DecodeRunner:
         ends in sample_rows (see forward); each warm-up call and each replay advances s_offsets by one.  penalties / logprobs: see forward;
         each warm-up call and each replay appends one token to s_history.  The graph is kept under the key (sample, penalties, logprobs) of
         step and becomes self.graph."""
-        self.graph = self._capture(("decode", bool(sample), bool(penalties), int(logprobs)),
-                                   lambda: self.tokens_out.copy_(self.forward(self.tokens_in, sample, penalties, logprobs)), warmup)
+        self._graph_key = ("decode", bool(sample), bool(penalties), int(logprobs)) + self._sp_key()
+        self.graph = self._capture(self._graph_key, lambda: self.tokens_out.copy_(self.forward(self.tokens_in, sample, penalties, logprobs)), warmup)
 
     def step(self, key: Optional[tuple] = None) -> None:
         """Replay the captured step: tokens_in -> tokens_out (both device resident).  key = (sample, penalties, logprobs) selects one of
-        the captures; None replays the latest."""
-        (self.graph if key is None else self.graphs[("decode", *key)]).replay()
+        the captures; None replays the latest.  With shared_prefix, a capture made under another layout plan is not replayed: KeyError for
+        a key, RuntimeError for None."""
+        if key is None and self.shared_prefix and self.graph is not None and self._graph_key[4:] != self._sp_key():
+            raise RuntimeError("the latest capture was made under another shared-prefix layout: capture again after fork / prefill")
+        (self.graph if key is None else self.graphs[("decode", *key) + self._sp_key()]).replay()
 
     def weight_bytes_per_step(self) -> int:
         return sum(l.weight_bytes() for ly in self.layers for l in (ly["qkv"], ly["o"], ly["gate_up"], ly["down"]))
