@@ -331,6 +331,40 @@ QS_API int qs_kv_cache_fork(const int64_t* kv_pointers, const int32_t* parents, 
                             int batch, int num_pairs, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block, int size_per_token,
                             int int4_kv_cache, void* stream);
 
+/* Beam search (SamplingParams.use_beam_search with best_of = W, length_penalty, early_stopping), vLLM 0.3's algorithm restated in
+ * tests/beam_oracle.py.  num_requests R requests of beam_width W (1 .. 8) beams; request r owns rows r W .. r W + W - 1 (batch = R W).  Both
+ * calls read everything after the PDL dependency wait, need no host synchronisation, are CUDA-graph capturable and bitwise deterministic.
+ *
+ * qs_beam_select: one step of every request with done[r] == 0 (a done request only gets parents = -1).  L = seq_lens[r W] and P0 =
+ *   prompt_lens[r W] are the length and prompt length every live beam shares.  Candidates: for every slot j with live[j] != 0, top_ids /
+ *   top_logprobs [batch, 2 W] as qs_logprobs_rows returns them with n = 2 W; ids < 0 are skipped; score s = cum[j] + lp in fp32.  The first 2 W
+ *   by (s descending, j ascending, rank ascending) are the children.  A child finishes on eos[r], on one of stop_ids[r] (int64 [R, num_stops],
+ *   num_stops <= 8, -1 pads; NULL when num_stops = 0) or when L - P0 + 1 >= budget[r] (clamped to [1, max_tokens]); its score is
+ *   cum / len ** length_penalty[r] (len = L + 1, minus 1 for eos).  The pool (pool_tokens int64 [R, W, max_tokens] generated tokens, pool_len
+ *   int32, pool_cum / pool_score fp32 [R, W], pool_count int32 [R]) keeps the W best of its hypotheses followed by the new finished children,
+ *   by a stable sort on score; a new hypothesis takes history[parent, P0 .. L) and its token.  The request is done when no child runs, or the
+ *   pool is full and early_stopping[r] is 1, or it is 0 (2: at len max(P0 + budget, max_model_len) if length_penalty > 0) and the worst
+ *   pool score >= the best running child's score.  Otherwise running child i < W takes slot r W + i: parents = its parent slot, tokens = its
+ *   token, cum = s, live = 1; the other slots (all of them when done) get parents = -1 and live = 0.  Every slot of the request gets
+ *   seq_lens = context_lens = L + 1.
+ * qs_beam_reorder: after qs_beam_select and the step's decode.  Request r's cached length is P = context_lens[r W] - 1 (qs_beam_select gives
+ *   every slot of a request it ran the same context length; the other slots' entries are not read).  For every slot s of the request whose
+ *   parent p = parents[s] is another slot of the same request: block-table entries 0 .. P / 64 - 1 of every layer and K / V become p's, entry
+ *   P / 64 is left alone (it must be s's own page); slots 0 .. P % 64 - 1 of p's page at block P / 64 (codes, scale and zero of every KV head)
+ *   are copied into s's page at that block; history columns [prompt_lens[s], P) come from p.  Every slot whose parent lies in its request
+ *   (p = s included) gets history[s, P] = tokens[s]; slots with p < 0 or p outside the request are left untouched.  Parents are a permutation
+ *   with repeats: all reads of a request's slice happen before its writes.  kv_pointers [num_layers, batch, 2, max_blocks_per_seq], history
+ *   int64 [batch, history_len]; pages 16-byte aligned.  The attention kernels read tables before their dependency wait, so a launch that
+ *   does not use programmatic dependent launch must separate the reorder from the next attention.                                        */
+QS_API int qs_beam_select(const int64_t* top_ids, const float* top_logprobs, int32_t* live, float* cum, int32_t* seq_lens, int32_t* context_lens,
+                          int64_t* tokens, int32_t* parents, const int32_t* prompt_lens, const int64_t* history, const float* length_penalty,
+                          const int32_t* early_stopping, const int64_t* eos, const int64_t* stop_ids, int num_stops, const int32_t* budget,
+                          int32_t* done, int64_t* pool_tokens, int32_t* pool_len, float* pool_cum, float* pool_score, int32_t* pool_count,
+                          int num_requests, int beam_width, int max_tokens, int max_model_len, int history_len, void* stream);
+QS_API int qs_beam_reorder(int64_t* kv_pointers, const int32_t* parents, const int32_t* context_lens, const int32_t* prompt_lens,
+                           const int64_t* tokens, int64_t* history, int num_layers, int batch, int beam_width, int max_blocks_per_seq,
+                           int num_kv_heads, int tokens_per_block, int size_per_token, int int4_kv_cache, int history_len, void* stream);
+
 /* Sampling on the GPU (the sampler's warpers and draw, and sampled acceptance of draft trees).
  *
  * Per row: temperature T (fp32), top_k (int32, -1 disables) and top_p (fp32), device arrays.  A row is GREEDY if T < 1e-5 or top_p < 1e-8,

@@ -751,6 +751,99 @@ def kv_cache_fork(kv_pointers, parents, children, lens, num_kv_heads: int, token
           kv_pointers.size(-1), int(num_kv_heads), int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)))
 
 
+MAX_BEAM_WIDTH = 8  # 2 W candidates per beam fit in logprobs_rows' 20
+
+
+class BeamPool(NamedTuple):
+    """The finished hypotheses of beam_select, per request best first: the first count[r] entries are valid."""
+    tokens: torch.Tensor  # int64 [R, W, T] generated tokens
+    length: torch.Tensor  # int32 [R, W] generated tokens of each hypothesis
+    cum: torch.Tensor     # fp32 [R, W] cumulative log-probability
+    score: torch.Tensor   # fp32 [R, W] cum / len ** length_penalty
+    count: torch.Tensor   # int32 [R]
+
+
+def beam_pool(num_requests: int, beam_width: int, max_tokens: int, device) -> BeamPool:
+    """An empty BeamPool (torch.full / torch.zeros)."""
+    R, W, T = int(num_requests), int(beam_width), int(max_tokens)
+    return BeamPool(torch.full((R, W, T), -1, dtype=torch.int64, device=device), torch.zeros((R, W), dtype=torch.int32, device=device),
+                    torch.zeros((R, W), dtype=torch.float32, device=device), torch.zeros((R, W), dtype=torch.float32, device=device),
+                    torch.zeros(R, dtype=torch.int32, device=device))
+
+
+def beam_select(top_ids, top_logprobs, live, cum, seq_lens, context_lens, tokens, parents, prompt_lens, history, length_penalty, early_stopping, eos,
+                stop_ids, budget, done, pool: BeamPool, max_model_len: int) -> None:
+    """One beam-search step of every request that is not done, in place and without host synchronisation (vLLM 0.3's algorithm, restated
+    in tests/beam_oracle.py; see include/qserve_b200.h).  R = done.numel() requests of W = batch / R beams (1 <= W <= 8); request r owns rows
+    r W .. r W + W - 1.  Per row (int32 unless stated): top_ids int64 / top_logprobs fp32 [batch, 2 W] from logprobs_rows(n = 2 W), live, cum
+    fp32, seq_lens, context_lens, tokens int64 (out), parents (out: parent slot, -1 dead), prompt_lens, history int64 [batch, H].  Per request:
+    length_penalty fp32, early_stopping (0 False, 1 True, 2 "never"), eos int64 (-1 none), stop_ids int64 [R, S <= 8] (-1 pads) or None,
+    budget (max_tokens, clamped to [1, T]), done.  pool: beam_pool(R, W, T).  Follow with beam_reorder."""
+    _require(done.dim() == 1 and top_ids.dim() == 2, "done must be [R] and top_ids [batch, 2 W]")
+    R, (B, C) = done.size(0), top_ids.shape
+    _require(R >= 1, "beam_select needs at least one request")
+    _require(B % R == 0, f"batch={B} is not a multiple of {R} requests")
+    W = B // R
+    _require(1 <= W <= MAX_BEAM_WIDTH, f"beam width {W}: 1 .. {MAX_BEAM_WIDTH}")
+    _require(C == 2 * W, f"top_ids must have 2 W = {2 * W} candidates per row, got {C}")
+    _require(stop_ids is None or (stop_ids.dim() == 2 and stop_ids.size(1) <= MAX_STOP_TOKENS),
+             f"stop_ids must be [R, S] with at most {MAX_STOP_TOKENS} stop tokens per request")
+    dev = _tensor(done, "done", torch.int32, (R,)).device
+    _tensor(top_ids, "top_ids", torch.int64, (B, C), dev)
+    _tensor(top_logprobs, "top_logprobs", torch.float32, (B, C), dev)
+    for t, nm, dt in ((live, "live", torch.int32), (cum, "cum", torch.float32), (seq_lens, "seq_lens", torch.int32), (context_lens, "context_lens", torch.int32),
+                      (tokens, "tokens", torch.int64), (parents, "parents", torch.int32), (prompt_lens, "prompt_lens", torch.int32)):
+        _tensor(t, nm, dt, (B,), dev)
+    H = _tensor(history, "history", torch.int64, (B, None), dev).size(1)
+    _require(H >= 1, "history must have at least one column")
+    for t, nm, dt in ((length_penalty, "length_penalty", torch.float32), (early_stopping, "early_stopping", torch.int32), (eos, "eos", torch.int64),
+                      (budget, "budget", torch.int32)):
+        _tensor(t, nm, dt, (R,), dev)
+    S = 0
+    if stop_ids is not None:
+        S = _tensor(stop_ids, "stop_ids", torch.int64, (R, None), dev).size(1)
+    T = _tensor(pool.tokens, "pool.tokens", torch.int64, (R, W, None), dev).size(2)
+    _require(T >= 1, "the pool must hold at least one token per hypothesis")
+    _tensor(pool.length, "pool.length", torch.int32, (R, W), dev)
+    _tensor(pool.cum, "pool.cum", torch.float32, (R, W), dev)
+    _tensor(pool.score, "pool.score", torch.float32, (R, W), dev)
+    _tensor(pool.count, "pool.count", torch.int32, (R,), dev)
+    _call(done, lib.qs_beam_select, top_ids.data_ptr(), top_logprobs.data_ptr(), live.data_ptr(), cum.data_ptr(), seq_lens.data_ptr(),
+          context_lens.data_ptr(), tokens.data_ptr(), parents.data_ptr(), prompt_lens.data_ptr(), history.data_ptr(), length_penalty.data_ptr(),
+          early_stopping.data_ptr(), eos.data_ptr(), _ptr(stop_ids if S else None), S, budget.data_ptr(), done.data_ptr(), pool.tokens.data_ptr(),
+          pool.length.data_ptr(), pool.cum.data_ptr(), pool.score.data_ptr(), pool.count.data_ptr(), R, W, T, int(max_model_len), H)
+
+
+def beam_reorder(kv_pointers, parents, context_lens, prompt_lens, tokens, history, beam_width: int, num_kv_heads: int, tokens_per_block: int,
+                 size_per_token: int, int4_kv_cache: bool) -> None:
+    """Re-parent every beam after beam_select, every layer in one launch, in place.  Request r's cached length is P = context_lens[r W] - 1
+    (beam_select gives all slots of a request it ran the same context length).  For each row s whose parent p = parents[s] (int32 [batch],
+    -1 dead) is another row of its request, the block-table entries 0 .. P // 64 - 1 become p's, the filled slots 0 .. P % 64 - 1 of p's tail
+    page are copied into s's own page at block P // 64 (codes, scale, zero; K and V; every KV head), and history columns [prompt_lens[s], P)
+    come from p; every row whose parent lies in its request gets history[s, P] = tokens[s]; rows with p < 0 or p outside the request are left
+    untouched.  Parents may repeat and a row may be a parent and a child at once.  kv_pointers int64 [L, batch, 2, max_blocks] or [batch, 2, max_blocks]; context_lens / prompt_lens int32 [batch];
+    tokens int64 [batch]; history int64 [batch, H]; beam_width 1 .. 8 divides batch."""
+    _require(kv_pointers.dim() in (3, 4) and kv_pointers.size(-2) == 2, "kv_pointers must be int64 [L, B, 2, max_blocks] or [B, 2, max_blocks]")
+    L = kv_pointers.size(0) if kv_pointers.dim() == 4 else 1
+    B = kv_pointers.size(-3)
+    W = int(beam_width)
+    _require(1 <= W <= MAX_BEAM_WIDTH, f"beam_width={W}: 1 .. {MAX_BEAM_WIDTH}")
+    _require(B % W == 0, f"batch={B} is not a multiple of beam_width={W}")
+    dev = _tensor(kv_pointers, "kv_pointers", torch.int64).device
+    for t, nm in ((parents, "parents"), (context_lens, "context_lens"), (prompt_lens, "prompt_lens")):
+        _tensor(t, nm, torch.int32, (B,), dev)
+    _tensor(tokens, "tokens", torch.int64, (B,), dev)
+    H = _tensor(history, "history", torch.int64, (B, None), dev).size(1)
+    _require(H >= 1, "history must have at least one column")
+    _require(int(tokens_per_block) == 64, "tokens_per_block must be 64")
+    _require(int(num_kv_heads) >= 1 and int(size_per_token) == int(num_kv_heads) * 128 * (4 if int4_kv_cache else 8) // 8,
+             "size_per_token does not match the kv heads and the cache type")
+    if B == 0 or L == 0:
+        return
+    _call(kv_pointers, lib.qs_beam_reorder, kv_pointers.data_ptr(), parents.data_ptr(), context_lens.data_ptr(), prompt_lens.data_ptr(), tokens.data_ptr(),
+          history.data_ptr(), L, B, W, kv_pointers.size(-1), int(num_kv_heads), int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), H)
+
+
 def _row_vec(v, n: int, dev, dt, name: str, ok, what: str) -> torch.Tensor:
     """A per-row parameter as a device tensor: a scalar broadcasts (and is checked on the host); a tensor is used as given (its values are
     trusted: checking them would synchronise with the device)."""

@@ -320,6 +320,33 @@ int qs_kv_cache_fork(const int64_t* kv_pointers, const int32_t* parents, const i
   return kv_cache_fork(a);
 }
 
+int qs_beam_select(const int64_t* top_ids, const float* top_logprobs, int32_t* live, float* cum, int32_t* seq_lens, int32_t* context_lens,
+                   int64_t* tokens, int32_t* parents, const int32_t* prompt_lens, const int64_t* history, const float* length_penalty,
+                   const int32_t* early_stopping, const int64_t* eos, const int64_t* stop_ids, int num_stops, const int32_t* budget, int32_t* done,
+                   int64_t* pool_tokens, int32_t* pool_len, float* pool_cum, float* pool_score, int32_t* pool_count, int num_requests, int beam_width,
+                   int max_tokens, int max_model_len, int history_len, void* stream) {
+  BeamSelectArgs a;
+  a.top_ids = reinterpret_cast<const long long*>(top_ids); a.top_logprobs = top_logprobs; a.live = live; a.cum = cum; a.seq_lens = seq_lens;
+  a.context_lens = context_lens; a.tokens = reinterpret_cast<long long*>(tokens); a.parents = parents; a.prompt_lens = prompt_lens;
+  a.history = reinterpret_cast<const long long*>(history); a.length_penalty = length_penalty; a.early_stopping = early_stopping;
+  a.eos = reinterpret_cast<const long long*>(eos); a.stop_ids = reinterpret_cast<const long long*>(stop_ids); a.num_stops = num_stops;
+  a.budget = budget; a.done = done; a.pool_tokens = reinterpret_cast<long long*>(pool_tokens); a.pool_len = pool_len; a.pool_cum = pool_cum;
+  a.pool_score = pool_score; a.pool_count = pool_count; a.num_requests = num_requests; a.beam_width = beam_width; a.max_tokens = max_tokens;
+  a.max_model_len = max_model_len; a.history_len = history_len; a.stream = stream;
+  return beam_select(a);
+}
+
+int qs_beam_reorder(int64_t* kv_pointers, const int32_t* parents, const int32_t* context_lens, const int32_t* prompt_lens, const int64_t* tokens,
+                    int64_t* history, int num_layers, int batch, int beam_width, int max_blocks_per_seq, int num_kv_heads, int tokens_per_block,
+                    int size_per_token, int int4_kv_cache, int history_len, void* stream) {
+  BeamReorderArgs a;
+  a.kv_pointers = reinterpret_cast<long long*>(kv_pointers); a.parents = parents; a.context_lens = context_lens; a.prompt_lens = prompt_lens;
+  a.tokens = reinterpret_cast<const long long*>(tokens); a.history = reinterpret_cast<long long*>(history); a.layers = num_layers; a.batch = batch;
+  a.beam_width = beam_width; a.max_blocks = max_blocks_per_seq; a.num_kv_heads = num_kv_heads; a.tokens_per_block = tokens_per_block;
+  a.size_per_token = size_per_token; a.int4_kv = int4_kv_cache; a.history_len = history_len; a.stream = stream;
+  return beam_reorder(a);
+}
+
 int qs_sample_rows(int64_t* out, const void* logits, const float* temperature, const int32_t* top_k, const float* top_p, uint64_t seed,
                    int64_t* offsets, int rows, int vocab, void* stream) {
   QS_REQUIRE(logits == nullptr || aligned16(logits), "sample_rows: logits must be 16-byte aligned");

@@ -199,6 +199,45 @@ struct KvForkArgs {
 };
 int kv_cache_fork(const KvForkArgs& a);
 
+// beam_search.cu: per-request beam selection and the in-place re-parenting of every beam's pages, tables and history
+struct BeamSelectArgs {
+  const long long* top_ids = nullptr;     // [batch, 2 W] candidates of every slot (logprobs_rows, n = 2 W)
+  const float* top_logprobs = nullptr;    // [batch, 2 W]
+  int* live = nullptr;                    // [batch], updated
+  float* cum = nullptr;                   // [batch] cumulative log-probabilities, updated
+  int* seq_lens = nullptr;                // [batch] tokens per beam (prompt + generated), read at the request's first slot, set
+  int* context_lens = nullptr;            // [batch] set
+  long long* tokens = nullptr;            // [batch] out: the token of every live slot
+  int* parents = nullptr;                 // [batch] out: parent slot, -1 dead
+  const int* prompt_lens = nullptr;       // [batch]
+  const long long* history = nullptr;     // [batch, history_len]
+  const float* length_penalty = nullptr;  // [num_requests]
+  const int* early_stopping = nullptr;    // [num_requests] 0 False, 1 True, 2 "never"
+  const long long* eos = nullptr;         // [num_requests], -1 none
+  const long long* stop_ids = nullptr;    // [num_requests, num_stops], -1 pads
+  const int* budget = nullptr;            // [num_requests] max_tokens
+  int* done = nullptr;                    // [num_requests], set
+  long long* pool_tokens = nullptr;       // [num_requests, W, max_tokens] finished hypotheses, best first
+  int* pool_len = nullptr;                // [num_requests, W] generated tokens of each hypothesis
+  float* pool_cum = nullptr;              // [num_requests, W]
+  float* pool_score = nullptr;            // [num_requests, W]
+  int* pool_count = nullptr;              // [num_requests]
+  int num_requests = 0, beam_width = 1, num_stops = 0, max_tokens = 0, max_model_len = 0, history_len = 0;
+  void* stream = nullptr;
+};
+int beam_select(const BeamSelectArgs& a);
+struct BeamReorderArgs {
+  long long* kv_pointers = nullptr;    // [layers, batch, 2, max_blocks] absolute page addresses, entries below P / 64 rewritten
+  const int* parents = nullptr;        // [batch] parent slot inside the request, -1 dead
+  const int* context_lens = nullptr;   // [batch] P + 1
+  const int* prompt_lens = nullptr;    // [batch]
+  const long long* tokens = nullptr;   // [batch] appended at history column P
+  long long* history = nullptr;        // [batch, history_len]
+  int layers = 1, batch = 0, beam_width = 1, max_blocks = 0, num_kv_heads = 0, tokens_per_block = 64, size_per_token = 0, int4_kv = 1, history_len = 0;
+  void* stream = nullptr;
+};
+int beam_reorder(const BeamReorderArgs& a);
+
 // sampling.cu: temperature / top-p / top-k sampling of fp16 logits and sampled (lossless) acceptance of draft trees; Philox4x32-10 draws
 // keyed by `seed` and counted by the per-row `offsets`, which every call advances by one
 struct SampleArgs {

@@ -156,7 +156,8 @@ class DecodeRunner:
     def __init__(self, model: str = "llama-3-8b", precision: str = "w4a8kv4", batch: int = 64, ctx: int = 1024,
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
-                 verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False, prompt_tokens: int = 0, shared_prefix: bool = False):
+                 verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False, prompt_tokens: int = 0, shared_prefix: bool = False,
+                 beam_width: int = 0):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
         ctx + verify_len tokens and the activation buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers
         and its random draws exactly as they are without it.
@@ -185,7 +186,26 @@ class DecodeRunner:
         capture_generate(1)) runs its attention through shared_prefix_decode_attention, which reads each group's shared pages once; otherwise
         through single_query_attention_quant.  The layout lives in buffers made with torch.zeros, so the weights, pages and every step
         without a group are those of shared_prefix=False.  The plain-step graph keys end in the layout's launch plan: after a fork or prefill
-        that changes it, replaying the old key raises instead of running under a stale plan."""
+        that changes it, replaying the old key raises instead of running under a stale plan.
+
+        beam_width = W >= 1 (single GPU, fused path, max_new_tokens = T >= 1, prompt_tokens > 0; not with generate or verify_len) adds beam
+        search (beam_start, beam_forward, capture_beam / beam_step, beam_results): batch / W requests of W beams, request r in rows
+        r W .. r W + W - 1.  The page tables cover ctx + T + 1 tokens as with generate=True, and the beam state (b_live, b_cum, b_parent, the
+        per-request b_length_penalty (1), b_early_stopping (0), b_eos (-1), b_stop (-1 pads), b_budget (T), b_done and the hypothesis pool
+        b_pool) is made with torch.full / torch.zeros, so the weights, pages and every other step are those of beam_width = 0."""
+        beam_width = int(beam_width)
+        if beam_width:
+            if not 1 <= beam_width <= _ext.MAX_BEAM_WIDTH:
+                raise RuntimeError(f"beam_width={beam_width}: 1 .. {_ext.MAX_BEAM_WIDTH}")
+            if batch % beam_width:
+                raise RuntimeError(f"batch={batch} is not a multiple of beam_width={beam_width}")
+            if tp_size != 1 or not fused or generate or verify_len:
+                raise RuntimeError("beam search is single-GPU, uses the fused path and is not combined with generate=True or verify_len")
+            if max_new_tokens < 1 or prompt_tokens < 1:
+                raise RuntimeError("beam search needs max_new_tokens >= 1 and prompt_tokens >= 1")
+            if ctx + max_new_tokens + 1 > min(8192, MODELS[model].max_pos):
+                raise RuntimeError("beam search runs past the positions the attention supports")
+        self.beam_width = beam_width
         assert precision in PRECISIONS, precision
         assert not shared_prefix or (tp_size == 1 and fused), "shared_prefix is single-GPU and uses the fused path"
         self.shared_prefix = shared_prefix
@@ -266,7 +286,7 @@ class DecodeRunner:
             tables.append(torch.stack([pools[0].data_ptr() + blk * self.page_bytes, pools[1].data_ptr() + blk * self.page_bytes], dim=1))
         self.table_blocks = self.blocks_per_seq
         self.kpools_gen, self.vpools_gen = [], []
-        if generate:  # pages for the generated tokens: zero-filled (no generator draws), after the pages above in every row's table
+        if generate or beam_width:  # pages for the generated tokens: zero-filled (no generator draws), after the pages above in every row's table
             self.table_blocks = (ctx + max_new_tokens + max(1, verify_len) + 63) // 64
             extra = self.table_blocks - self.blocks_per_seq
             if extra:
@@ -281,8 +301,8 @@ class DecodeRunner:
         self.own_tables = self.block_tables.clone()  # every row's own pages: fork() shares a parent's pages, prefill() restores these
         self.context_lens = torch.full((batch,), ctx + 1, dtype=torch.int32, device=dev)
         # host bounds of the attention launches: in generation the contexts grow up to ctx + 1 + max_new_tokens
-        self.max_seq_len = ctx + 1 + (max_new_tokens if generate else 0)
-        self.max_prefix_len = ctx + (max_new_tokens if generate else 0)
+        self.max_seq_len = ctx + 1 + (max_new_tokens if generate or beam_width else 0)
+        self.max_prefix_len = ctx + (max_new_tokens if generate or beam_width else 0)
 
         # ---- persistent ActivationBuffer (input_metadata.py:71-109; aliasing kept) for the rows of the widest step --------------------
         # (H is in the max for tensor parallelism: at TP = 8 a 72B model's sharded qkv / gate_up rows are narrower than the full hidden row of out_buf)
@@ -318,6 +338,8 @@ class DecodeRunner:
             self._alloc_penalty_buffers()
         if generate:
             self._alloc_generate_buffers()
+        if beam_width:
+            self._alloc_beam_buffers()
         self.sp_groups = []  # shared-prefix groups: (rows, S), the group's first row first
         self._sp_layout = None  # the layout the plain step passes to shared_prefix_decode_attention (None: single_query_attention_quant)
         if shared_prefix:
@@ -959,6 +981,117 @@ class DecodeRunner:
             t[chi] = t[par]
         if self.shared_prefix:
             self._set_groups(fork_groups(self.sp_groups, parents, children, cached.tolist()))
+
+    # ---------------------------------------------------------------------------------------------------------
+    # beam search: W beams per request; selection and re-parenting of every beam's pages on the GPU, inside the captured step
+    # ---------------------------------------------------------------------------------------------------------
+    def _alloc_beam_buffers(self) -> None:
+        """Beam state (torch.full / torch.zeros: no random draws)."""
+        B, W, T, dev = self.batch, self.beam_width, self.max_new_tokens, self.dev
+        R = B // W
+        self.b_live = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.b_cum = torch.zeros(B, dtype=torch.float32, device=dev)
+        self.b_parent = torch.full((B,), -1, dtype=torch.int32, device=dev)
+        self.b_length_penalty = torch.full((R,), 1.0, dtype=torch.float32, device=dev)
+        self.b_early_stopping = torch.zeros(R, dtype=torch.int32, device=dev)  # 0 False, 1 True, 2 "never"
+        self.b_eos = torch.full((R,), -1, dtype=torch.int64, device=dev)
+        self.b_stop = torch.full((R, _ext.MAX_STOP_TOKENS), -1, dtype=torch.int64, device=dev)
+        self.b_budget = torch.full((R,), T, dtype=torch.int32, device=dev)
+        self.b_done = torch.zeros(R, dtype=torch.int32, device=dev)
+        self.b_pool = _ext.beam_pool(R, W, T, dev)
+        # the step's candidates: logprobs_rows with n = 2 W (b_logprob is its unused per-row output)
+        self.b_top_ids = torch.zeros((B, 2 * W), dtype=torch.int64, device=dev)
+        self.b_top_logprobs = torch.zeros((B, 2 * W), dtype=torch.float32, device=dev)
+        self.b_logprob = torch.zeros(B, dtype=torch.float32, device=dev)
+        self.max_model_len = self.ctx + T
+
+    def _beam_tail(self, logits: torch.Tensor) -> None:
+        """logits -> the 2 W candidates of every beam -> beam_select -> beam_reorder."""
+        W = self.beam_width
+        _ext.logprobs_rows(logits, self.tokens_in, 2 * W, self.b_logprob, self.b_top_ids, self.b_top_logprobs)
+        _ext.beam_select(self.b_top_ids, self.b_top_logprobs, self.b_live, self.b_cum, self.s_seq_lens, self.context_lens, self.tokens_in, self.b_parent,
+                         self.s_prompt_lens, self.s_history, self.b_length_penalty, self.b_early_stopping, self.b_eos, self.b_stop, self.b_budget,
+                         self.b_done, self.b_pool, self.max_model_len)
+        # the next step begins with the embedding gather, a launch without PDL: the attention kernels, which read the tables and context_lens
+        # before their dependency wait, see the reorder's writes
+        _ext.beam_reorder(self.block_tables, self.b_parent, self.context_lens, self.s_prompt_lens, self.tokens_in, self.s_history, W, self.Hkv, 64,
+                          self.size_per_token, self.kv_bits == 4)
+
+    def beam_start(self, prompts: torch.Tensor, lens: torch.Tensor, chunk: Optional[int] = None, penalties: bool = False) -> None:
+        """Start a beam search for R = batch / W prompts: prompts int64 [R, >= max(lens)], lens int32 [R] (1 <= lens[r] <= ctx).  Prompt r is
+        prefilled into row r W (the other rows of the request get a 1-token prompt, so the prompt is computed once); then every row of
+        request r takes its prompt as history (s_history, s_prompt_lens = s_seq_lens = lens[r]), slot r W is the only live beam with cum 0,
+        the pool is emptied, and the first beam step runs on the prefill logits (apply_penalties first if penalties): logprobs_rows with
+        n = 2 W, beam_select and beam_reorder with every running child's parent r W.  b_length_penalty, b_early_stopping, b_eos, b_stop and
+        b_budget stay as the caller set them.  With shared_prefix=True each request's rows become one group sharing lens[r] // 64 pages: the
+        reorder never changes table entries below that, so the layout holds for the whole search.  Eager, with prefill's host synchronisation."""
+        assert self.beam_width, "construct the runner with beam_width > 0"
+        B, W, dev = self.batch, self.beam_width, self.dev
+        R = B // W
+        if not (lens.dtype == torch.int32 and tuple(lens.shape) == (R,)):
+            raise RuntimeError(f"lens must be int32 [{R}], got {lens.dtype} {tuple(lens.shape)}")
+        if not (prompts.dtype == torch.int64 and prompts.dim() == 2 and prompts.size(0) == R):
+            raise RuntimeError(f"prompts must be int64 [{R}, >= max(lens)], got {prompts.dtype} {tuple(prompts.shape)}")
+        lens_h = [int(x) for x in lens.tolist()]
+        prompts, lens = prompts.to(dev), lens.to(dev)
+        first = torch.arange(R, device=dev) * W
+        full = torch.zeros((B, prompts.size(1)), dtype=torch.int64, device=dev)
+        full[first] = prompts
+        full_lens = torch.ones(B, dtype=torch.int32, device=dev)
+        full_lens[first] = lens
+        self.prefill(full, full_lens, chunk, penalties=penalties)
+        logits = self.last_logits  # penalised in place by prefill when penalties
+        rows = torch.arange(B, device=dev) // W * W
+        self.s_prompt_lens.copy_(self.s_prompt_lens[rows])
+        self.s_seq_lens.copy_(self.s_prompt_lens)  # prefill appended its first token: drop it
+        cols = torch.arange(self.s_history.size(1), device=dev)
+        self.s_history.copy_(torch.where(cols < self.s_prompt_lens.unsqueeze(1), self.s_history[rows], -1))
+        self.b_live.zero_()
+        self.b_live[first] = 1
+        self.b_cum.zero_()
+        self.b_parent.fill_(-1)
+        self.b_done.zero_()
+        self.b_pool.tokens.fill_(-1)
+        for t in self.b_pool[1:]:
+            t.zero_()
+        self._beam_tail(logits)
+        if self.shared_prefix:
+            self._set_groups([(tuple(range(r * W, r * W + W)), lens_h[r] // 64) for r in range(R)])
+
+    def beam_forward(self, penalties: bool = False) -> None:
+        """One beam step for every request: the decode step at the beams' own lengths (tokens_in, context_lens), apply_penalties (s_history,
+        s_prompt_lens, s_seq_lens, s_repetition / s_presence / s_frequency) if penalties, logprobs_rows with n = 2 W, beam_select and
+        beam_reorder.  Done requests and dead slots are computed but not advanced.  No host synchronisation."""
+        assert self.beam_width, "construct the runner with beam_width > 0"
+        logits = self._forward_fused(self.tokens_in, True)
+        if penalties:
+            _ext.apply_penalties(logits, self.s_history, self.s_prompt_lens, self.s_seq_lens, self.s_repetition, self.s_presence, self.s_frequency)
+        self._beam_tail(logits)
+
+    def _beam_key(self, penalties: bool) -> tuple:
+        return ("beam", bool(penalties)) + self._sp_key()
+
+    def capture_beam(self, penalties: bool = False, warmup: int = 2) -> None:
+        """Capture beam_forward(penalties) in a CUDA graph.  The warm-up runs the step eagerly and advances the beams like a replay does: call
+        beam_start afterwards.  With shared_prefix=True the key ends in the layout beam_start sets, so when that layout takes the shared route
+        capture after beam_start (the warm-up then advances the search by `warmup` steps)."""
+        self._capture(self._beam_key(penalties), lambda: self.beam_forward(penalties), warmup)
+
+    def beam_step(self, penalties: bool = False) -> None:
+        """Replay the captured beam step."""
+        self.graphs[self._beam_key(penalties)].replay()
+
+    def beam_results(self, n: Optional[int] = None) -> list:
+        """Per request, its best n (default W) finished hypotheses, best first: (generated tokens, cumulative log-probability, score).  Reads
+        the pool back to the host."""
+        assert self.beam_width, "construct the runner with beam_width > 0"
+        n = self.beam_width if n is None else int(n)
+        pool = _ext.BeamPool(*(t.cpu() for t in self.b_pool))
+        out = []
+        for r in range(pool.count.numel()):
+            c = min(int(pool.count[r]), n)
+            out.append([(pool.tokens[r, q, : int(pool.length[r, q])].tolist(), float(pool.cum[r, q]), float(pool.score[r, q])) for q in range(c)])
+        return out
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
