@@ -175,10 +175,11 @@ def cached_rows(kpool: PagePool, vpool: PagePool, block_row, n: int, hk: int):
     return res[0], res[2], res[1], res[3]
 
 
-def paged_exact(q, kpool, vpool, block_row, n: int, hk: int, own_k, own_v, allowed=None, *, n_acc: int, rope_rel: float = 0.0):
+def paged_exact(q, kpool, vpool, block_row, n: int, hk: int, own_k, own_v, allowed=None, *, n_acc: int, rope_rel: float = 0.0, rows=None):
     """exact() for the paged kernels: columns q [C, D] over cache tokens 0..n-1 of kv head hk, then one un-quantised own token per column
-    (own_k / own_v [C, D], None: no own token).  allowed [C, n] masks the cache tokens."""
-    kd, vd, ks, vs = cached_rows(kpool, vpool, block_row, n, hk)
+    (own_k / own_v [C, D], None: no own token).  allowed [C, n] masks the cache tokens.  rows: cached_rows() of these arguments, if the
+    caller already has them."""
+    kd, vd, ks, vs = cached_rows(kpool, vpool, block_row, n, hk) if rows is None else rows
     U = CODE_MAX[vpool.bits]
     q = np.asarray(q, np.float64)
     C = q.shape[0]
