@@ -97,6 +97,8 @@ QS_API int qs_set_trace_buffer(void* dev_buffer, unsigned capacity_records);
  *   device addresses of the K then V pages (kvCacheUtils.h:84-90); length_per_sample int32 [B] = context length
  *   INCLUDING the token being decoded (may be NULL: then `timestep` is used); out fp16 [B,Hq,D] contiguous.
  *   Side effect: RoPE(k) and v of the new token are quantised and appended at index length-1.
+ *   length_per_sample[b] == 0 marks row b idle (an in-flight step's free or prefilling row): no page byte is written, its output row is
+ *   zero, and the workspace counters are left as they were; rows of length >= 1 are computed exactly as without idle rows.
  *   D must be 128, kv_cache_with_zeros must be 1 (ZINT4 / ZINT8), rotary_embedding_dim must equal D.
  *   workspace (optional): qs_attention_workspace_bytes(...) bytes, zero-initialised once; enables context splits.  */
 QS_API int qs_single_query_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride,
@@ -189,7 +191,8 @@ QS_API int qs_add_rms_norm_general(int8_t* out, void* hidden_out, const void* x,
                                    void* scaling, float epsilon, int tokens, int hidden, void* stream);
 /* single_query_attention followed by invoke_quant[_fuse_sum] of the [B, Hq*D] result: out_q int8 [B, Hq*D], out_scale fp16 [B],
  * out_sum fp16 [B] or NULL.  The fp16 attention row stays in `workspace` (>= qs_attention_workspace_bytes, zero-initialised
- * once, L2 resident); the last CTA of a token to finish quantises it, so the result is bit-identical to the two-op sequence. */
+ * once, L2 resident); the last CTA of a token to finish quantises it, so the result is bit-identical to the two-op sequence.
+ * An idle row (length_per_sample[b] == 0) gets a zero int8 row, out_scale = 0 and out_sum = 0 (invoke_quant of a zero row). */
 QS_API int qs_single_query_attention_quant(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride,
                                            const int64_t* kv_pointers, const int32_t* length_per_sample, int8_t* out_q, void* out_scale,
                                            void* out_sum, int batch, int num_heads, int num_kv_heads, int head_dim, int max_blocks_per_seq,
@@ -221,7 +224,8 @@ QS_API int qs_apply_bias_rope_update_kv_cache_at(void* qkv, const int32_t* seq_l
  *   the un-quantised fp16 k / v.  GQA by Hq / Hkv, head_dim 128, tokens_per_block 64, fp32 softmax, P rounded to fp16 before the PV product;
  *   wgmma, sm_90a only; deterministic.  max_prefix_len is a host bound (like flash-attn's max_seqlen_k): the call checks
  *   max_prefix_len + max_seqlen <= max_blocks_per_seq * 64, and the kernel TRUSTS prefix_lens[b] <= max_prefix_len.  prefix_lens and the page
- *   table are read before the PDL dependency wait (see qs_set_pdl), the page contents after it.                                          */
+ *   table are read before the PDL dependency wait (see qs_set_pdl), the page contents after it.  Rows cu_seqlens[batch] .. num_tokens - 1
+ *   belong to no sequence (the padding of an in-flight step's fixed chunk segment): their output rows are written as zeros.            */
 QS_API int qs_prefix_prefill_attention(const void* q, const void* k, const void* v, int64_t q_stride, int64_t k_stride, int64_t v_stride, void* out,
                                        int64_t out_stride, const int32_t* cu_seqlens, const int32_t* prefix_lens, const int64_t* kv_pointers,
                                        int batch, int num_tokens, int max_seqlen, int max_prefix_len, int max_blocks_per_seq, int num_heads,
@@ -473,6 +477,81 @@ QS_API int qs_spec_commit_stops(const int64_t* draft_tokens, const int32_t* path
                                 int64_t* history, int32_t* seq_lens, const int32_t* prompt_lens, const int32_t* budget, const int64_t* eos,
                                 const int64_t* stop_ids, int num_stops, int32_t* finished, int32_t* start_pos, int32_t* context_lens,
                                 int64_t* roots, int batch, int num_nodes, int history_len, void* stream);
+
+/* In-flight batching (DESIGN.md 3.12): the schedule at the start of every in-flight step of the decode runner.  One CTA, device state only, no
+ * host synchronisation; CUDA-graph capturable.  B rows, a request queue of Q slots (request r lives in slot r % Q), segment C = chunk tokens of
+ * the step's chunk segment, chunk_budget = C (mixed step) or 0 (decode-only step, flush).  Phases: 0 FREE, 1 PREFILL, 2 DECODE.
+ *
+ * qs_inflight_schedule, in this order (tests/inflight_oracle.py restates it):
+ *   1. Retire: every DECODE row with finished = 1, in row order, copies history[prompt_lens .. seq_lens) to out_tokens[slot], the count to
+ *      out_len, the reason to out_reason (1 eos: the last token is eos; 2 stop: it is one of the stop ids; 3 budget: otherwise) and, when
+ *      logprob is given, logprob[prompt_lens .. seq_lens) to out_logprob[slot]; out_ids[retired % Q] = the request; retired += 1; FREE.
+ *   2. Admit (chunk_budget > 0 only): while head < tail, the lowest-index FREE row takes request head: history = the prompt then -1, logprob row
+ *      NaN, prompt_lens = seq_lens = len, the request's sampling / penalty / stop parameters into the per-row vectors, budget = max_tokens,
+ *      offsets = 0, done = 0, adm = the next admission number, PREFILL; head += 1.
+ *   3. Plan: PREFILL rows in admission order take c_b = min(len - done, chunk_budget - used) tokens.  The segment is laid out in row order:
+ *      cu_seqlens [B + 1], chunk_lens = c_b, prefix_lens = done (0 for other rows), tokens[B + cu_b + j] = history[b, done + j] and
+ *      padding_offset[cu_b + j] = b C - cu_b (what qs_compute_padding_offsets gives at max_seqlen C).  Segment slots t >= used = cu_seqlens[B]
+ *      are padding: token 0 and padding_offset = C - 1 - t, which maps them to position C - 1 of row 0, at or past that row's chunk length
+ *      (every c_b <= used < C), so qs_apply_bias_rope_update_kv_cache_at skips them.  Decode segment: context_lens = seq_lens and
+ *      tokens[b] = tokens_in[b] for DECODE rows, 0 (idle, see qs_single_query_attention) and token 0 for the others.  done += c_b.
+ *   4. Tail masks: a row whose prompt completes becomes DECODE with logit_rows = B + cu_seqlens[b + 1] - 1, start_pos = len, finished = 0;
+ *      DECODE rows keep logit_rows = b, finished = 0; every other row gets logit_rows = b and finished = 1, so the commit skips it.
+ * counters int32 [4]: head (the kernel's), tail (the host's), retired, admissions.  Limits: 1 <= B <= 512, Q >= 1, C >= 1. */
+typedef struct qs_inflight_args {
+  /* request queue, [Q] unless stated; filled by the host between steps */
+  const int64_t* q_prompts; /* [Q, prompt_cols] */
+  const int32_t* q_lens;    /* 1 .. prompt_cols */
+  const int32_t* q_max_tokens;
+  const int64_t* q_eos;
+  const int64_t* q_stop;    /* [Q, 8], -1 pads */
+  const float* q_temperature;
+  const int32_t* q_top_k;
+  const float* q_top_p;
+  const float* q_repetition;
+  const float* q_presence;
+  const float* q_frequency;
+  int32_t* counters;        /* [4] */
+  /* row state, [B] */
+  int32_t* phase;
+  int32_t* row_req;
+  int32_t* done;
+  int32_t* adm;
+  /* the runner's per-row vectors, [B] unless stated */
+  int64_t* history;         /* [B, history_len] */
+  int32_t* prompt_lens;
+  int32_t* seq_lens;
+  float* temperature;
+  int32_t* top_k;
+  float* top_p;
+  float* repetition;
+  float* presence;
+  float* frequency;
+  int64_t* eos;
+  int64_t* stop;            /* [B, 8] */
+  int32_t* budget;
+  int64_t* offsets;
+  int32_t* finished;
+  int32_t* start_pos;
+  const int64_t* tokens_in;
+  float* logprob;           /* [B, history_len] or NULL */
+  /* the step's plan */
+  int32_t* cu_seqlens;      /* [B + 1] */
+  int32_t* prefix_lens;
+  int32_t* chunk_lens;
+  int32_t* padding_offset;  /* [C] */
+  int32_t* context_lens;
+  int64_t* tokens;          /* [B + C] */
+  int64_t* logit_rows;
+  /* per-request outputs */
+  int64_t* out_tokens;      /* [Q, max_tokens] */
+  int32_t* out_len;
+  int32_t* out_reason;
+  float* out_logprob;       /* [Q, max_tokens] or NULL */
+  int32_t* out_ids;         /* [Q] ring of retired request ids */
+  int batch, queue, prompt_cols, history_len, max_tokens, chunk, chunk_budget;
+} qs_inflight_args;
+QS_API int qs_inflight_schedule(const qs_inflight_args* args, void* stream);
 
 #ifdef __cplusplus
 }

@@ -45,6 +45,7 @@ SIGNATURES = {
     "qs_shared_prefix_attention_workspace_bytes": (c_size_t, [_I, _I, _I, _I, _I, _I, _I, _I]),
     "qs_kv_cache_fork": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "qs_beam_select": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "qs_inflight_schedule": (c_int, [_P, _P]),
     "qs_beam_reorder": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "qs_sample_rows": (c_int, [_P, _P, _P, _P, _P, ctypes.c_uint64, _P, _I, _I, _P]),
     "qs_tree_accept_sampling": (c_int, [_P, _P, _P, _P, _P, _P, _P, ctypes.c_uint64, _P, _P, _P, _P, _I, _I, _I, _P]),

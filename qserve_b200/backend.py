@@ -8,6 +8,7 @@ stream and the two outputs the reference ops allocate themselves.
 """
 from __future__ import annotations
 
+import ctypes
 from typing import NamedTuple, Optional
 
 import torch
@@ -842,6 +843,134 @@ def beam_reorder(kv_pointers, parents, context_lens, prompt_lens, tokens, histor
         return
     _call(kv_pointers, lib.qs_beam_reorder, kv_pointers.data_ptr(), parents.data_ptr(), context_lens.data_ptr(), prompt_lens.data_ptr(), tokens.data_ptr(),
           history.data_ptr(), L, B, W, kv_pointers.size(-1), int(num_kv_heads), int(tokens_per_block), int(size_per_token), int(bool(int4_kv_cache)), H)
+
+
+class InflightQueue(NamedTuple):
+    """The request queue of the in-flight step (qs_inflight_schedule): Q slots, request r in slot r % Q, filled by the host between steps."""
+    prompts: torch.Tensor      # int64 [Q, prompt_cols]
+    lens: torch.Tensor         # int32 [Q], 1 .. prompt_cols
+    max_tokens: torch.Tensor   # int32 [Q]
+    eos: torch.Tensor          # int64 [Q], -1: none
+    stop: torch.Tensor         # int64 [Q, 8], -1 pads
+    temperature: torch.Tensor  # fp32 [Q]
+    top_k: torch.Tensor        # int32 [Q]
+    top_p: torch.Tensor        # fp32 [Q]
+    repetition: torch.Tensor   # fp32 [Q]
+    presence: torch.Tensor     # fp32 [Q]
+    frequency: torch.Tensor    # fp32 [Q]
+    counters: torch.Tensor     # int32 [4]: head (the kernel's), tail (the host's), retired, admissions
+
+
+class InflightRows(NamedTuple):
+    """Row state of the in-flight step, int32 [B] each."""
+    phase: torch.Tensor    # 0 FREE, 1 PREFILL, 2 DECODE
+    request: torch.Tensor  # the row's request id, -1 when free
+    done: torch.Tensor     # prompt tokens cached
+    adm: torch.Tensor      # admission number (first-come-first-served order of the PREFILL rows)
+
+
+class InflightPlan(NamedTuple):
+    """What the schedule plans for one step of B rows and a chunk segment of C slots."""
+    cu_seqlens: torch.Tensor      # int32 [B + 1]
+    prefix_lens: torch.Tensor     # int32 [B]
+    chunk_lens: torch.Tensor      # int32 [B]
+    padding_offset: torch.Tensor  # int32 [C]
+    context_lens: torch.Tensor    # int32 [B], 0: idle
+    tokens: torch.Tensor          # int64 [B + C]: the decode tokens, then the chunk segment
+    logit_rows: torch.Tensor      # int64 [B]
+
+
+class InflightOutputs(NamedTuple):
+    """Per-request outputs, slot r % Q, and the ring of retired request ids."""
+    tokens: torch.Tensor             # int64 [Q, T]
+    length: torch.Tensor             # int32 [Q]
+    reason: torch.Tensor             # int32 [Q]: 1 eos, 2 stop, 3 budget
+    logprob: Optional[torch.Tensor]  # fp32 [Q, T] or None
+    ids: torch.Tensor                # int32 [Q]
+
+
+INFLIGHT_FREE, INFLIGHT_PREFILL, INFLIGHT_DECODE = 0, 1, 2
+INFLIGHT_REASONS = {1: "eos", 2: "stop", 3: "budget"}
+MAX_INFLIGHT_ROWS = 512
+
+
+def inflight_buffers(batch: int, queue: int, chunk: int, prompt_cols: int, max_tokens: int, device, logprobs: bool = True):
+    """Fresh (InflightQueue, InflightRows, InflightPlan, InflightOutputs), made with torch.full / torch.zeros: an empty queue, every row FREE."""
+    B, Q, C, dev = int(batch), int(queue), int(chunk), device
+    z = lambda *shape, dt=torch.int32: torch.zeros(shape, dtype=dt, device=dev)
+    f = lambda shape, v, dt: torch.full(shape, v, dtype=dt, device=dev)
+    queue_ = InflightQueue(z(Q, int(prompt_cols), dt=torch.int64), f((Q,), 1, torch.int32), f((Q,), int(max_tokens), torch.int32),
+                           f((Q,), -1, torch.int64), f((Q, MAX_STOP_TOKENS), -1, torch.int64), f((Q,), 1.0, torch.float32), f((Q,), 1, torch.int32),
+                           f((Q,), 1.0, torch.float32), f((Q,), 1.0, torch.float32), z(Q, dt=torch.float32), z(Q, dt=torch.float32), z(4))
+    rows = InflightRows(z(B), f((B,), -1, torch.int32), z(B), z(B))
+    plan = InflightPlan(z(B + 1), z(B), z(B), z(C), z(B), z(B + C, dt=torch.int64), torch.arange(B, dtype=torch.int64, device=dev))
+    out = InflightOutputs(f((Q, int(max_tokens)), -1, torch.int64), z(Q), z(Q), f((Q, int(max_tokens)), float("nan"), torch.float32) if logprobs else None,
+                          f((Q,), -1, torch.int32))
+    return queue_, rows, plan, out
+
+
+class _InflightArgs(ctypes.Structure):
+    """qs_inflight_args of include/qserve_b200.h, field for field."""
+    _fields_ = [(n, ctypes.c_void_p) for n in (
+        "q_prompts", "q_lens", "q_max_tokens", "q_eos", "q_stop", "q_temperature", "q_top_k", "q_top_p", "q_repetition", "q_presence", "q_frequency",
+        "counters", "phase", "row_req", "done", "adm", "history", "prompt_lens", "seq_lens", "temperature", "top_k", "top_p", "repetition", "presence",
+        "frequency", "eos", "stop", "budget", "offsets", "finished", "start_pos", "tokens_in", "logprob", "cu_seqlens", "prefix_lens", "chunk_lens",
+        "padding_offset", "context_lens", "tokens", "logit_rows", "out_tokens", "out_len", "out_reason", "out_logprob", "out_ids")] + \
+        [(n, ctypes.c_int) for n in ("batch", "queue", "prompt_cols", "history_len", "max_tokens", "chunk", "chunk_budget")]
+
+
+def inflight_schedule(queue: InflightQueue, rows: InflightRows, history, prompt_lens, seq_lens, temperature, top_k, top_p, repetition, presence,
+                      frequency, eos, stop, budget, offsets, finished, start_pos, tokens_in, logprob: Optional[torch.Tensor], plan: InflightPlan,
+                      out: InflightOutputs, chunk_budget: int) -> None:
+    """One in-flight schedule, in place and without host synchronisation (include/qserve_b200.h qs_inflight_schedule; restated in
+    tests/inflight_oracle.py): retire the DECODE rows with finished = 1 into `out`, admit queued requests into FREE rows first-come-first-served
+    (chunk_budget > 0 only), plan the chunk segment (chunk_budget = C or 0) and the decode segment into `plan`, and set the tail masks.  The
+    per-row runner vectors are [B] (history int64 [B, H], stop int64 [B, 8], logprob fp32 [B, H] or None together with out.logprob)."""
+    B = _tensor(rows.phase, "phase", torch.int32, (None,)).size(0)
+    dev = rows.phase.device
+    _require(1 <= B <= MAX_INFLIGHT_ROWS, f"batch={B}: 1 .. {MAX_INFLIGHT_ROWS} rows")
+    Q, P = _tensor(queue.prompts, "queue.prompts", torch.int64, (None, None), dev).shape
+    C = _tensor(plan.padding_offset, "plan.padding_offset", torch.int32, (None,), dev).size(0)
+    T = _tensor(out.tokens, "out.tokens", torch.int64, (Q, None), dev).size(1)
+    H = _tensor(history, "history", torch.int64, (B, None), dev).size(1)
+    _require(Q >= 1 and C >= 1 and T >= 1 and P >= 1, "queue, chunk segment, max_tokens and prompt columns must be >= 1")
+    _require(H >= P + T, f"history of {H} columns cannot hold {P} prompt and {T} generated tokens")
+    _require(int(chunk_budget) in (0, C), f"chunk_budget={chunk_budget}: 0 or the chunk segment ({C})")
+    _require((logprob is None) == (out.logprob is None), "logprob and out.logprob must both be given or both be None")
+    for t, n, dt in ((queue.lens, "queue.lens", torch.int32), (queue.max_tokens, "queue.max_tokens", torch.int32), (queue.eos, "queue.eos", torch.int64),
+                     (queue.temperature, "queue.temperature", torch.float32), (queue.top_k, "queue.top_k", torch.int32),
+                     (queue.top_p, "queue.top_p", torch.float32), (queue.repetition, "queue.repetition", torch.float32),
+                     (queue.presence, "queue.presence", torch.float32), (queue.frequency, "queue.frequency", torch.float32),
+                     (out.length, "out.length", torch.int32), (out.reason, "out.reason", torch.int32), (out.ids, "out.ids", torch.int32)):
+        _tensor(t, n, dt, (Q,), dev)
+    _tensor(queue.stop, "queue.stop", torch.int64, (Q, MAX_STOP_TOKENS), dev)
+    _tensor(queue.counters, "queue.counters", torch.int32, (4,), dev)
+    for t, n, dt in ((rows.request, "rows.request", torch.int32), (rows.done, "rows.done", torch.int32), (rows.adm, "rows.adm", torch.int32),
+                     (prompt_lens, "prompt_lens", torch.int32), (seq_lens, "seq_lens", torch.int32), (temperature, "temperature", torch.float32),
+                     (top_k, "top_k", torch.int32), (top_p, "top_p", torch.float32), (repetition, "repetition", torch.float32),
+                     (presence, "presence", torch.float32), (frequency, "frequency", torch.float32), (eos, "eos", torch.int64),
+                     (budget, "budget", torch.int32), (offsets, "offsets", torch.int64), (finished, "finished", torch.int32),
+                     (start_pos, "start_pos", torch.int32), (tokens_in, "tokens_in", torch.int64), (plan.prefix_lens, "plan.prefix_lens", torch.int32),
+                     (plan.chunk_lens, "plan.chunk_lens", torch.int32), (plan.context_lens, "plan.context_lens", torch.int32),
+                     (plan.logit_rows, "plan.logit_rows", torch.int64)):
+        _tensor(t, n, dt, (B,), dev)
+    _tensor(stop, "stop", torch.int64, (B, MAX_STOP_TOKENS), dev)
+    _tensor(plan.cu_seqlens, "plan.cu_seqlens", torch.int32, (B + 1,), dev)
+    _tensor(plan.tokens, "plan.tokens", torch.int64, (B + C,), dev)
+    if logprob is not None:
+        _tensor(logprob, "logprob", torch.float32, (B, H), dev)
+        _tensor(out.logprob, "out.logprob", torch.float32, (Q, T), dev)
+    ptrs = dict(q_prompts=queue.prompts, q_lens=queue.lens, q_max_tokens=queue.max_tokens, q_eos=queue.eos, q_stop=queue.stop,
+                q_temperature=queue.temperature, q_top_k=queue.top_k, q_top_p=queue.top_p, q_repetition=queue.repetition, q_presence=queue.presence,
+                q_frequency=queue.frequency, counters=queue.counters, phase=rows.phase, row_req=rows.request, done=rows.done, adm=rows.adm,
+                history=history, prompt_lens=prompt_lens, seq_lens=seq_lens, temperature=temperature, top_k=top_k, top_p=top_p, repetition=repetition,
+                presence=presence, frequency=frequency, eos=eos, stop=stop, budget=budget, offsets=offsets, finished=finished, start_pos=start_pos,
+                tokens_in=tokens_in, logprob=logprob, cu_seqlens=plan.cu_seqlens, prefix_lens=plan.prefix_lens, chunk_lens=plan.chunk_lens,
+                padding_offset=plan.padding_offset, context_lens=plan.context_lens, tokens=plan.tokens, logit_rows=plan.logit_rows,
+                out_tokens=out.tokens, out_len=out.length, out_reason=out.reason, out_logprob=out.logprob, out_ids=out.ids)
+    a = _InflightArgs(**{k: _ptr(v) for k, v in ptrs.items()}, batch=B, queue=Q, prompt_cols=P, history_len=H, max_tokens=T, chunk=C,
+                      chunk_budget=int(chunk_budget))
+    _call(rows.phase, lib.qs_inflight_schedule, ctypes.addressof(a))
 
 
 def _row_vec(v, n: int, dev, dt, name: str, ok, what: str) -> torch.Tensor:

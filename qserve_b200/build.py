@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libqserve_b200.so")
-SOURCES = ["capi.cu", "gemm.cu", "attention.cu", "prefill_attention.cu", "prefix_attention.cu", "multi_token_attention.cu", "tree_verify.cu", "kv_fork.cu", "beam_search.cu", "sampling.cu", "speculative.cu", "elementwise.cu"]
+SOURCES = ["capi.cu", "gemm.cu", "attention.cu", "prefill_attention.cu", "prefix_attention.cu", "multi_token_attention.cu", "tree_verify.cu", "kv_fork.cu", "beam_search.cu", "inflight.cu", "sampling.cu", "speculative.cu", "elementwise.cu"]
 HEADERS = ["common.cuh", "launch.h", "launch.cuh", "paged_attention.cuh", "prompt_attention.cuh", os.path.join("..", "..", "include", "qserve_b200.h")]
 
 NVCC_FLAGS = [

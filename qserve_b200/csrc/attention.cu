@@ -112,6 +112,23 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
   // they are read BEFORE the dependency wait, so that the chain length -> page pointers -> first bulk copy (two dependent
   // global round trips) overlaps the tail of the preceding qkv GEMM.  Page CONTENTS and q/k/v are only touched after the wait.
   const int tlen = lengths ? lengths[b] - 1 : timestep;  // tokens already in the cache (Template.hpp:901: length_per_sample ? len - 1 : timestep)
+  if (tlen < 0) {
+    // idle row (length 0, an in-flight step's free or prefilling row): no page byte, a zero output row (with the fused quantisation: the zero
+    // int8 row, scale and sum that invoke_quant gives a zero row), and no split or per-token counter is touched.  Uniform per CTA.
+    pdl_wait();  // the outputs may still be read by the kernel before (q_out aliases the qkv GEMM's input)
+    if (split != 0) return;
+    if (q_out == nullptr) {
+      for (int i = threadIdx.x; i < Gc * kD; i += kAttnThreadsV2) out[(static_cast<size_t>(b) * num_heads + h0) * kD + i] = __float2half_rn(0.f);
+    } else if (blockIdx.x == 0) {
+      int8_t* qrow = q_out + static_cast<size_t>(b) * num_heads * kD;
+      for (int i = threadIdx.x; i < num_heads * kD; i += kAttnThreadsV2) qrow[i] = 0;
+      if (threadIdx.x == 0) {
+        q_scale[b] = __float2half_rn(0.f);
+        if (q_sum) q_sum[b] = __float2half_rn(0.f);
+      }
+    }
+    return;
+  }
   const long long* kptrs = kv_pointers + (static_cast<size_t>(b) * 2 + 0) * max_blocks;
   const long long* vptrs = kv_pointers + (static_cast<size_t>(b) * 2 + 1) * max_blocks;
   const int n_pages = (tlen + kPageTokens - 1) / kPageTokens;

@@ -559,4 +559,9 @@ int qs_dequant_silu_and_mul_quant(int8_t* out, const int32_t* input, float scale
   return dequant_silu_and_mul_quant(out, input, scale_gate, scale_up, scale_out, scale_out_vec, tmp, tokens, d, stream);
 }
 
+int qs_inflight_schedule(const qs_inflight_args* args, void* stream) {
+  QS_REQUIRE(args != nullptr, "inflight_schedule: null arguments");
+  return inflight_schedule(*args, stream);
+}
+
 }  // extern "C"

@@ -3,6 +3,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+struct qs_inflight_args;  // include/qserve_b200.h
+
 namespace qs {
 
 bool pdl_enabled();
@@ -355,5 +357,8 @@ struct SpecCommitArgs {
 int spec_commit(const SpecCommitArgs& a);
 // spec_commit with a stop-token set per row: stop_ids [batch, num_stops <= 8], -1 pads
 int spec_commit_stops(const SpecCommitArgs& a, const long long* stop_ids, int num_stops);
+
+// the in-flight step's schedule (inflight.cu): the arguments of qs_inflight_schedule
+int inflight_schedule(const qs_inflight_args& a, void* stream);
 
 }  // namespace qs

@@ -46,6 +46,7 @@ struct PrefixAttnParams {
   __half* out;                    // [T, Hq * 128] rows of out_stride halfs
   long long out_stride;
   int num_heads, num_kv_heads, max_blocks;
+  int num_tokens;                 // T: rows cu_seqlens[B] .. T - 1 are padding (zero output)
   int code_bytes;                 // bytes of codes per page (64 * size_per_token)
   float scale_log2;               // softmax scale * log2(e)
 };
@@ -125,6 +126,16 @@ prefix_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   const int seq_len = __ldg(p.cu_seqlens + b + 1) - seq_start;
   const int n_qb = (seq_len + kBQ - 1) / kBQ;
   const int qb = n_qb - 1 - static_cast<int>(blockIdx.x);  // the longest (last) query blocks of a chunk are scheduled first
+  if (b == static_cast<int>(gridDim.z) - 1 && seq_start + seq_len < p.num_tokens) {
+    // rows cu_seqlens[B] .. num_tokens - 1 belong to no sequence (an in-flight step's chunk-segment padding): the CTAs (x, h) of the last
+    // sequence write head h of those rows as zeros, so no NaN comes out of rows nobody reads.  Every existing call has cu_seqlens[B] = T.
+    pdl_wait();  // the output buffer may still be read by the kernel before
+    for (long long i = seq_start + seq_len + static_cast<long long>(blockIdx.x) * kBQ; i < p.num_tokens; i += static_cast<long long>(gridDim.x) * kBQ)
+      for (int c = threadIdx.x; c < kBQ * kD / 8; c += kThreads) {
+        const long long row = i + c / (kD / 8);
+        if (row < p.num_tokens) reinterpret_cast<uint4*>(p.out + row * p.out_stride + static_cast<size_t>(h) * kD)[c % (kD / 8)] = make_uint4(0u, 0u, 0u, 0u);
+      }
+  }
   if (qb < 0) return;                                      // uniform per CTA
   if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();
   const int hkv = h / (p.num_heads / p.num_kv_heads);
@@ -239,6 +250,7 @@ int prefix_attention(const PrefixAttnArgs& a) {
   p.num_heads = a.num_heads;
   p.num_kv_heads = a.num_kv_heads;
   p.max_blocks = a.max_blocks;
+  p.num_tokens = a.num_tokens;
   p.code_bytes = kPageTokens * a.size_per_token;
   p.scale_log2 = a.softmax_scale * 1.4426950408889634f;
   auto kern = a.int4_kv ? prefix_attention_kernel<4> : prefix_attention_kernel<8>;

@@ -149,6 +149,12 @@ def prompt_pieces(lens, ctx: int, prompt_tokens: int, chunk: Optional[int] = Non
     return pieces
 
 
+class InflightPoll(NamedTuple):
+    """DecodeRunner.poll: the requests retired since the last poll and the prompt tokens still to prefill."""
+    finished: list
+    pending_tokens: int
+
+
 _PROMPT_LOGITS_BYTES = 64 << 20  # prompt_logprobs: fp16 logits of at most this many bytes exist at once
 
 
@@ -157,7 +163,7 @@ class DecodeRunner:
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
                  verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False, prompt_tokens: int = 0, shared_prefix: bool = False,
-                 beam_width: int = 0):
+                 beam_width: int = 0, inflight: int = 0):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
         ctx + verify_len tokens and the activation buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers
         and its random draws exactly as they are without it.
@@ -192,7 +198,14 @@ class DecodeRunner:
         search (beam_start, beam_forward, capture_beam / beam_step, beam_results): batch / W requests of W beams, request r in rows
         r W .. r W + W - 1.  The page tables cover ctx + T + 1 tokens as with generate=True, and the beam state (b_live, b_cum, b_parent, the
         per-request b_length_penalty (1), b_early_stopping (0), b_eos (-1), b_stop (-1 pads), b_budget (T), b_done and the hypothesis pool
-        b_pool) is made with torch.full / torch.zeros, so the weights, pages and every other step are those of beam_width = 0."""
+        b_pool) is made with torch.full / torch.zeros, so the weights, pages and every other step are those of beam_width = 0.
+
+        inflight = Q >= 1 (single GPU, fused path, generate=True, max_new_tokens = T >= 1, prompt_tokens = C >= 1; not with verify_len,
+        beam_width or shared_prefix) adds in-flight batching (submit, inflight_forward, capture_inflight / inflight_step, poll): a queue of Q
+        requests, rows that take queued prompts as they free up, and a step that carries up to C prompt tokens of the prefilling rows in the
+        same forward pass as the decode tokens of the others (DESIGN.md 3.12).  The activation buffers hold batch + C rows and the page tables
+        cover max(ctx + T + 1, ctx - 1 + C) tokens; every row keeps its own pages.  All its state is made with torch.full / torch.zeros after
+        every random draw, so inflight = 0 leaves the weights, pages and every other step as they are."""
         beam_width = int(beam_width)
         if beam_width:
             if not 1 <= beam_width <= _ext.MAX_BEAM_WIDTH:
@@ -206,6 +219,16 @@ class DecodeRunner:
             if ctx + max_new_tokens + 1 > min(8192, MODELS[model].max_pos):
                 raise RuntimeError("beam search runs past the positions the attention supports")
         self.beam_width = beam_width
+        inflight = int(inflight)
+        if inflight:
+            if tp_size != 1 or not fused or not generate or verify_len or beam_width or shared_prefix:
+                raise RuntimeError("in-flight batching is single-GPU, uses the fused path, needs generate=True and is not combined with verify_len, "
+                                   "beam_width or shared_prefix")
+            if max_new_tokens < 1 or prompt_tokens < 1 or inflight < 1:
+                raise RuntimeError("in-flight batching needs max_new_tokens >= 1, prompt_tokens >= 1 and a queue of at least one request")
+            if not 1 <= batch <= _ext.MAX_INFLIGHT_ROWS:
+                raise RuntimeError(f"in-flight batching runs 1 .. {_ext.MAX_INFLIGHT_ROWS} rows")
+        self.inflight = inflight
         assert precision in PRECISIONS, precision
         assert not shared_prefix or (tp_size == 1 and fused), "shared_prefix is single-GPU and uses the fused path"
         self.shared_prefix = shared_prefix
@@ -287,7 +310,8 @@ class DecodeRunner:
         self.table_blocks = self.blocks_per_seq
         self.kpools_gen, self.vpools_gen = [], []
         if generate or beam_width:  # pages for the generated tokens: zero-filled (no generator draws), after the pages above in every row's table
-            self.table_blocks = (ctx + max_new_tokens + max(1, verify_len) + 63) // 64
+            # (in-flight batching: also the host bound ctx - 1 + C of the chunk segment's prompt attention)
+            self.table_blocks = (max(ctx + max_new_tokens + max(1, verify_len), ctx - 1 + prompt_tokens if inflight else 0) + 63) // 64
             extra = self.table_blocks - self.blocks_per_seq
             if extra:
                 blk = torch.arange(batch * extra, device=dev, dtype=torch.int64).view(batch, extra)
@@ -306,7 +330,7 @@ class DecodeRunner:
 
         # ---- persistent ActivationBuffer (input_metadata.py:71-109; aliasing kept) for the rows of the widest step --------------------
         # (H is in the max for tensor parallelism: at TP = 8 a 72B model's sharded qkv / gate_up rows are narrower than the full hidden row of out_buf)
-        R = max(M * max(1, verify_len), prompt_tokens)
+        R = max(M * max(1, verify_len), prompt_tokens, M + prompt_tokens if inflight else 0)
         self.act_buffer = torch.empty(R * max(self.q_size + 2 * self.kv_size, 2 * self.Iloc, H), dtype=torch.half, device=dev)
         self.q_act = torch.empty(R * max(H, self.Iloc), dtype=torch.int8, device=dev)
         self.scale_buffer = torch.empty(R, dtype=torch.half, device=dev)
@@ -340,6 +364,8 @@ class DecodeRunner:
             self._alloc_generate_buffers()
         if beam_width:
             self._alloc_beam_buffers()
+        if inflight:
+            self._alloc_inflight_buffers()
         self.sp_groups = []  # shared-prefix groups: (rows, S), the group's first row first
         self._sp_layout = None  # the layout the plain step passes to shared_prefix_decode_attention (None: single_query_attention_quant)
         if shared_prefix:
@@ -1092,6 +1118,176 @@ class DecodeRunner:
             c = min(int(pool.count[r]), n)
             out.append([(pool.tokens[r, q, : int(pool.length[r, q])].tolist(), float(pool.cum[r, q]), float(pool.score[r, q])) for q in range(c)])
         return out
+
+    # ---------------------------------------------------------------------------------------------------------
+    # in-flight batching: queued prompts enter rows as they free up; one step carries their prompt chunks and the decode tokens of the others
+    # ---------------------------------------------------------------------------------------------------------
+    def _alloc_inflight_buffers(self) -> None:
+        """Queue, row state, step plan and per-request outputs (torch.full / torch.zeros: no random draws)."""
+        B, C, T = self.batch, self.prompt_tokens, self.max_new_tokens
+        self._alloc_generate_logprobs(0)  # g_logprob: the schedule hands the chosen tokens' log-probabilities to the outputs
+        self.i_queue, self.i_rows, self.i_plan, self.i_out = _ext.inflight_buffers(B, self.inflight, C, self.ctx, T, self.dev)
+        self._i_submitted = 0       # requests submitted (the host's tail)
+        self._i_lens: dict = {}     # prompt length of every request not yet polled
+        self._i_unpolled: set = set()
+        self._i_staged: list = []   # pinned host tensors of copies still in flight (released by poll)
+        self._i_polled = 0          # entries of the retired ring handed out by poll
+
+    def submit(self, prompts, lens, max_tokens=None, eos=-1, stop=None, temperature=1.0, top_k=1, top_p=1.0, repetition=1.0, presence=0.0,
+               frequency=0.0) -> list:
+        """Queue requests: prompts int64 [n, >= max(lens)] (host or device), lens (host ints, 1 .. ctx); per request (a host scalar for all,
+        or a host sequence of n) max_tokens (1 .. max_new_tokens, default max_new_tokens), eos (-1: none), stop (up to 8 ids per request), temperature,
+        top_k, top_p, repetition, presence and frequency as the runner's per-row s_* parameters.  Returns the request ids (consecutive).
+        Stream-ordered copies into the queue slots, then the tail advances; no host synchronisation.  Request r uses slot r % Q, so it may only
+        be submitted once request r - Q has been returned by poll; raises RuntimeError otherwise (at most Q requests are outstanding)."""
+        assert self.inflight, "construct the runner with inflight > 0"
+        lens = [int(x) for x in (lens.tolist() if isinstance(lens, torch.Tensor) else lens)]
+        n, Q, T, dev = len(lens), self.inflight, self.max_new_tokens, self.dev
+        if n == 0:
+            return []
+        if min(lens) < 1 or max(lens) > self.ctx:
+            raise RuntimeError(f"prompt lengths must lie in [1, ctx={self.ctx}], got {lens}")
+        if not (isinstance(prompts, torch.Tensor) and prompts.dtype == torch.int64 and prompts.dim() == 2 and prompts.size(0) == n
+                and prompts.size(1) >= max(lens)):
+            raise RuntimeError(f"prompts must be int64 [{n}, >= {max(lens)}]")
+        ids = list(range(self._i_submitted, self._i_submitted + n))
+        busy = [r for r in ids if r - Q >= 0 and (r - Q) in self._i_unpolled]
+        if busy or n > Q:
+            raise RuntimeError(f"more than {Q} requests would be outstanding: poll the finished ones first")
+
+        def per(v, name, conv):
+            v = list(v) if isinstance(v, (list, tuple)) or (isinstance(v, torch.Tensor) and v.dim() > 0) else [v] * n
+            if len(v) != n:
+                raise RuntimeError(f"{name}: one value per request ({n}), got {len(v)}")
+            return [conv(x) for x in v]
+        mt = per(T if max_tokens is None else max_tokens, "max_tokens", int)
+        if min(mt) < 1 or max(mt) > T:
+            raise RuntimeError(f"max_tokens must lie in [1, max_new_tokens={T}], got {mt}")
+        stops = [list(x) for x in (stop if stop is not None and len(stop) and isinstance(stop[0], (list, tuple)) else [stop or []] * n)]
+        if len(stops) != n or any(len(x) > _ext.MAX_STOP_TOKENS for x in stops):
+            raise RuntimeError(f"stop: up to {_ext.MAX_STOP_TOKENS} ids per request")
+        f32 = lambda name, v: torch.tensor(per(v, name, float), dtype=torch.float32)
+        i32 = lambda name, v: torch.tensor(per(v, name, int), dtype=torch.int32)
+        host = {"lens": torch.tensor(lens, dtype=torch.int32), "max_tokens": torch.tensor(mt, dtype=torch.int32),
+                "eos": torch.tensor(per(eos, "eos", int), dtype=torch.int64),
+                "stop": torch.tensor([x + [-1] * (_ext.MAX_STOP_TOKENS - len(x)) for x in stops], dtype=torch.int64),
+                "temperature": f32("temperature", temperature), "top_k": i32("top_k", top_k), "top_p": f32("top_p", top_p),
+                "repetition": f32("repetition", repetition), "presence": f32("presence", presence), "frequency": f32("frequency", frequency)}
+        # every host tensor goes through a pinned staging buffer and a non-blocking copy: a plain host-to-device copy from pageable memory
+        # (torch.tensor(..., device=cuda) included) would wait for every step already queued on the stream
+        slots = torch.tensor([r % Q for r in ids], dtype=torch.int64).pin_memory()
+        self._i_staged.append(slots)
+        slots = slots.to(dev, non_blocking=True)
+        P = self.ctx
+        rows = torch.full((n, P), -1, dtype=torch.int64, device=prompts.device)
+        w = min(P, prompts.size(1))
+        rows[:, :w] = prompts[:, :w]
+        for name, t in [("prompts", rows)] + list(host.items()):
+            if t.device.type == "cpu":
+                t = t.pin_memory()
+                self._i_staged.append(t)
+            getattr(self.i_queue, name).index_copy_(0, slots, t.to(dev, non_blocking=True))
+        self._i_submitted += n
+        self.i_queue.counters[1].fill_(self._i_submitted)
+        for r, ln in zip(ids, lens):
+            self._i_lens[r] = ln
+            self._i_unpolled.add(r)
+        return ids
+
+    def _inflight_schedule(self, chunk_budget: int) -> None:
+        _ext.inflight_schedule(self.i_queue, self.i_rows, self.s_history, self.s_prompt_lens, self.s_seq_lens, self.s_temperature, self.s_top_k,
+                               self.s_top_p, self.s_repetition, self.s_presence, self.s_frequency, self.g_eos, self.g_stop, self.g_budget,
+                               self.s_offsets, self.g_finished, self.g_start, self.tokens_in, self.g_logprob, self.i_plan, self.i_out, chunk_budget)
+
+    def inflight_forward(self, mixed: bool = True, sampled: bool = False, penalties: bool = False, logprobs: int = 0) -> None:
+        """One in-flight step; no host synchronisation.  inflight_schedule (chunk budget C, or 0 when mixed=False: nothing is admitted and no
+        prompt token is carried), then the layers over M = B + C rows (B without mixed): the B decode rows, idle ones at context length 0,
+        and the chunk segment, whose padding slots are neither appended nor attended.  Per layer: single_query_attention_quant over the decode
+        rows; apply_bias_rope_update_kv_cache_at + prefix_prefill_attention + invoke_quant[_fuse_sum] over the chunk segment (host bounds
+        max_seqlen = C, max_prefix_len = ctx - 1).  The B logit rows (the decode rows, and for a row whose prompt completes the logit of its
+        last prompt token) go through lm_head at M = B, then the sampler of generate_forward(1): apply_penalties if penalties, argmax_rows or
+        sample_rows if sampled, logprobs_accepted if logprobs, spec_commit with the stop ids.  A completing row's first token is committed in
+        the same step.
+
+        sample_rows keys its Philox stream on the row index and s_offsets, which admission resets to 0 and every step advances (idle steps
+        too): a sampled request's tokens are deterministic for a given submission script but depend on its row and on its neighbours."""
+        assert self.inflight, "construct the runner with inflight > 0"
+        logprobs = int(logprobs)
+        assert 0 <= logprobs <= _ext.MAX_TOP_LOGPROBS, f"logprobs={logprobs}: 0 .. {_ext.MAX_TOP_LOGPROBS}"
+        if logprobs:
+            self._alloc_generate_logprobs(logprobs)
+        B, C, cfg = self.batch, self.prompt_tokens, self.cfg
+        M = B + C if mixed else B
+        self._inflight_schedule(C if mixed else 0)
+        plan = self.i_plan
+        D, int4, max_pos = cfg.head_dim, self.kv_bits == 4, min(8192, cfg.max_pos)
+
+        def attention(li, r):
+            table = self.block_tables[li]
+            q, k, v = self._heads(r.qkv)
+            _ext.single_query_attention_quant(q[:B], k[:B], v[:B], table, plan.context_lens, max_pos, 64, self.size_per_token, self.max_seq_len, D,
+                                              cfg.rope_theta, int4, True, r.q_attn[:B], r.q_scale[:B], r.q_sum[:B] if self.act_sum else None)
+            if not mixed:
+                return
+            seg = r.qkv[B:]
+            _ext.apply_bias_rope_update_kv_cache_at(seg, plan.chunk_lens, plan.padding_offset, plan.prefix_lens, table, self.Hq, self.Hkv, C, 64,
+                                                    self.size_per_token, D, cfg.rope_theta, max_pos, True, int4, True)
+            attn = _ext.prefix_prefill_attention(*self._heads(seg), plan.cu_seqlens, C, plan.prefix_lens, self.ctx - 1, table, 64, self.size_per_token,
+                                                 int4)
+            self._quant(r._replace(q_scale=r.q_scale[B:], q_sum=r.q_sum[B:]), r.q_attn[B:], attn.view(C, -1))
+
+        hidden, n = self._fused_layers(self.embed[plan.tokens[:M]], self._row_views(M), attention)
+        logits = self._logits(hidden.index_select(0, plan.logit_rows))
+        self.launches_per_step = n + 3
+        self.last_logits = logits
+        tok = self._pick(logits, sampled, penalties, logprobs, out=self.tokens_out)
+        if logprobs:
+            _ext.logprobs_accepted(logits.view(B, 1, -1), tok.view(B, 1), self.g_path1, self.g_accept1, tok, self.s_seq_lens, self.g_finished,
+                                   logprobs, self.g_logprob, *self.g_top_view(logprobs))
+        _ext.spec_commit(tok.view(B, 1), self.g_path1, self.g_accept1, tok, self.s_history, self.s_seq_lens, self.s_prompt_lens, self.g_budget,
+                         self.g_eos, self.g_finished, self.g_start, self.context_lens, self.tokens_in, stop_ids=self.g_stop)
+
+    def _inflight_key(self, mixed: bool, sampled: bool, penalties: bool, logprobs: int) -> tuple:
+        return ("inflight", bool(mixed), bool(sampled), bool(penalties), int(logprobs))
+
+    def capture_inflight(self, mixed: bool = True, sampled: bool = False, penalties: bool = False, logprobs: int = 0, warmup: int = 2) -> None:
+        """Capture inflight_forward(mixed, sampled, penalties, logprobs) in a CUDA graph.  The warm-up runs the step eagerly on the current
+        state (it schedules, admits and advances rows like a replay does): capture before submitting."""
+        self._capture(self._inflight_key(mixed, sampled, penalties, logprobs), lambda: self.inflight_forward(mixed, sampled, penalties, logprobs),
+                      warmup)
+
+    def inflight_step(self, mixed: bool = True, sampled: bool = False, penalties: bool = False, logprobs: int = 0) -> None:
+        """Replay the captured in-flight step."""
+        self.graphs[self._inflight_key(mixed, sampled, penalties, logprobs)].replay()
+
+    def poll(self, flush: bool = False, logprobs: bool = False) -> "InflightPoll":
+        """The requests retired since the last poll, in retire order, as (request id, tokens, reason) with reason "eos", "stop" or "budget"
+        (with logprobs=True a fourth entry: the chosen tokens' log-probabilities, NaN for tokens of steps without logprobs), and the prompt
+        tokens still to prefill (queued requests and prefilling rows): with none, the decode-only step (mixed=False) does the same work.
+        flush=True first runs the schedule with chunk budget 0, which retires the rows the last step finished and admits nothing.  One host
+        synchronisation."""
+        assert self.inflight, "construct the runner with inflight > 0"
+        if flush:
+            self._inflight_schedule(0)
+        q, rows, out = self.i_queue, self.i_rows, self.i_out
+        snap = [t.to("cpu", non_blocking=True) for t in (q.counters, rows.phase, rows.done, self.s_prompt_lens, out.ids, out.length, out.reason,
+                                                         out.tokens, out.logprob)]
+        torch.cuda.current_stream(self.dev).synchronize()
+        ctr, phase, done, plen, ids, length, reason, toks, lps = snap
+        self._i_staged.clear()
+        Q = self.inflight
+        finished = []
+        for i in range(self._i_polled, int(ctr[2])):
+            r = int(ids[i % Q])
+            s, k = r % Q, int(length[r % Q])
+            entry = (r, toks[s, :k].tolist(), _ext.INFLIGHT_REASONS.get(int(reason[s]), "?"))
+            finished.append(entry + (lps[s, :k].tolist(),) if logprobs else entry)
+            self._i_unpolled.discard(r)
+            self._i_lens.pop(r, None)
+        self._i_polled = int(ctr[2])
+        queued = sum(self._i_lens[r] for r in range(int(ctr[0]), self._i_submitted))
+        prefilling = int(((plen - done) * (phase == _ext.INFLIGHT_PREFILL)).sum())
+        return InflightPoll(finished, queued + prefilling)
 
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
