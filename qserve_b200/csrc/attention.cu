@@ -780,52 +780,33 @@ __global__ void padding_offsets_kernel(int* __restrict__ out, const int* __restr
 constexpr size_t kAttnCounterBytes = 256 * 1024;  // 49152 (sequence, head-group) split counters + 16384 per-token counters
 constexpr size_t kAttnTokCounterOffset = 192 * 1024;
 
-// ---- launch plan of qs_shared_prefix_decode_attention: a function of host integers only, so the call can be captured in a graph ----
-template <int BITS, int NT>
-int shared_resident_ctas() {
-  static int cached[kMaxDevices] = {};
-  int& r = cached[device_ordinal()];
-  if (r == 0) {
-    const int smem = kWarps * StageLayout<BITS>::kWarpBytes;
-    int n = 0;
-    if (raise_smem_limit(shared_prefix_attention_kernel<BITS, NT>, smem, "shared_prefix_decode_attention smem attribute") != QS_OK ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, shared_prefix_attention_kernel<BITS, NT>, kAttnConsumers, smem) != cudaSuccess || n < 1) {
-      cudaGetLastError();
-      n = 1;
-    }
-    r = n;
-  }
-  return r;
-}
-
 struct SharedPrefixPlan {
   int gx;          // row pass: KV heads x head groups of <= 8 query heads
-  int nsplit;      // row pass context splits (decode_attention's rule)
+  int nsplit;      // row pass context splits (decode_attention's)
   int ntile;       // shared pass: n8 tiles per CTA (C = 8 ntile columns of (member, query head))
   int cparts;      // shared pass: column parts per KV head
   int sp_nsplit;   // shared pass: context splits of the shared pages (0: no shared pass)
   size_t part_bytes, row_bytes;
 };
 
+// The launch plan of qs_shared_prefix_decode_attention: a function of host integers only, so the call can be captured in a graph
 SharedPrefixPlan plan_shared_prefix(int bits, int batch, int num_heads, int num_kv_heads, int timestep, int num_groups, int max_group, int max_pages) {
   SharedPrefixPlan pl{};
   const int G = num_heads / num_kv_heads;
   pl.gx = num_kv_heads * ((G + kMaxG - 1) / kMaxG);
-  pl.nsplit = 1;
-  const int ctas = pl.gx * batch, slots = num_sms() * 4;
-  if (2 * ctas <= slots && timestep > 512) pl.nsplit = std::min(std::min((slots + ctas - 1) / ctas, (timestep + 255) / 256), 32);
+  pl.nsplit = context_splits(static_cast<long long>(pl.gx) * batch, num_sms() * 4, timestep);
   if (num_groups > 0 && max_group > 0 && max_pages > 0) {
     const int cols = G * max_group;
     pl.ntile = cols <= 8 ? 1 : 2;
     pl.cparts = (cols + 8 * pl.ntile - 1) / (8 * pl.ntile);
     const long long sctas = static_cast<long long>(num_kv_heads) * pl.cparts * num_groups;
-    const int per_sm = bits == 4 ? (pl.ntile == 1 ? shared_resident_ctas<4, 1>() : shared_resident_ctas<4, 2>())
-                                 : (pl.ntile == 1 ? shared_resident_ctas<8, 1>() : shared_resident_ctas<8, 2>());
-    const long long sslots = static_cast<long long>(num_sms()) * per_sm;
-    const int ctx = max_pages * kPageTokens;
-    pl.sp_nsplit = 1;
-    if (2 * sctas <= sslots && ctx > 512)
-      pl.sp_nsplit = static_cast<int>(std::min<long long>(std::min<long long>((sslots + sctas - 1) / sctas, (ctx + 255) / 256), 32));
+    const int smem = kWarps * (bits == 4 ? StageLayout<4>::kWarpBytes : StageLayout<8>::kWarpBytes);
+    const char* what = "shared_prefix_decode_attention smem attribute";
+    const int per_sm = bits == 4 ? (pl.ntile == 1 ? resident_ctas<shared_prefix_attention_kernel<4, 1>>(smem, what)
+                                                 : resident_ctas<shared_prefix_attention_kernel<4, 2>>(smem, what))
+                                 : (pl.ntile == 1 ? resident_ctas<shared_prefix_attention_kernel<8, 1>>(smem, what)
+                                                 : resident_ctas<shared_prefix_attention_kernel<8, 2>>(smem, what));
+    pl.sp_nsplit = context_splits(sctas, static_cast<long long>(num_sms()) * per_sm, max_pages * kPageTokens);
   }
   pl.part_bytes = static_cast<size_t>(batch) * num_heads * (pl.nsplit + pl.sp_nsplit) * (kD + 2) * sizeof(float);
   pl.row_bytes = static_cast<size_t>(batch) * num_heads * kD * sizeof(__half);
@@ -843,15 +824,12 @@ size_t shared_prefix_attention_workspace_bytes(int batch, int num_heads, int num
 
 int shared_prefix_decode_attention(const SharedPrefixAttnArgs& s) {
   const DecodeAttnArgs& a = s.d;
-  QS_REQUIRE(a.head_dim == kD, "shared_prefix_decode_attention: head_dim=%d, only 128 is supported", a.head_dim);
+  const int rc = check_page_geometry("shared_prefix_decode_attention", a.head_dim, a.num_heads, a.num_kv_heads, a.tokens_per_block, a.size_per_token,
+                                     a.int4_kv);
+  if (rc) return rc;
   QS_REQUIRE(a.kv_zeros, "shared_prefix_decode_attention: only kv_cache_with_zeros=True is supported");
-  QS_REQUIRE(a.num_kv_heads > 0 && a.num_heads % a.num_kv_heads == 0, "shared_prefix_decode_attention: heads %d / kv heads %d", a.num_heads,
-             a.num_kv_heads);
-  QS_REQUIRE(a.tokens_per_block == kPageTokens, "shared_prefix_decode_attention: tokens_per_block=%d, only 64 is supported", a.tokens_per_block);
   QS_REQUIRE(a.rotary_dim == kD, "shared_prefix_decode_attention: rotary_dim=%d must equal head_dim", a.rotary_dim);
   const int bits = a.int4_kv ? 4 : 8;
-  QS_REQUIRE(a.size_per_token == a.num_kv_heads * kD * bits / 8, "shared_prefix_decode_attention: size_per_token=%d does not match %d kv heads x %d bits",
-             a.size_per_token, a.num_kv_heads, bits);
   QS_REQUIRE(a.batch >= 0 && a.batch <= 16384, "shared_prefix_decode_attention: batch=%d, must be 0 .. 16384", a.batch);
   QS_REQUIRE(s.num_groups >= 0 && s.num_groups <= 65535 && s.max_group >= 0 && s.max_pages >= 0,
              "shared_prefix_decode_attention: num_groups=%d, max_group=%d, max_pages=%d", s.num_groups, s.max_group, s.max_pages);
@@ -923,30 +901,16 @@ int attention_trace_install(void* buf, unsigned cap) { return qs_trace_install(b
 
 int decode_attention(const DecodeAttnArgs& a) {
   if (a.batch == 0) return QS_OK;
-  QS_REQUIRE(a.head_dim == kD, "single_query_attention: head_dim=%d, only 128 is supported (as in the reference)", a.head_dim);
+  const int rc = check_page_geometry("single_query_attention", a.head_dim, a.num_heads, a.num_kv_heads, a.tokens_per_block, a.size_per_token, a.int4_kv);
+  if (rc) return rc;
   QS_REQUIRE(a.kv_zeros, "single_query_attention: only kv_cache_with_zeros=True is supported (arg_utils.py:422 always sets it)");
-  QS_REQUIRE(a.num_kv_heads > 0 && a.num_heads % a.num_kv_heads == 0, "single_query_attention: heads %d / kv heads %d", a.num_heads, a.num_kv_heads);
-  QS_REQUIRE(a.tokens_per_block > 0 && a.tokens_per_block % kChunk == 0, "single_query_attention: tokens_per_block=%d must be a multiple of %d",
-             a.tokens_per_block, kChunk);
   QS_REQUIRE(a.rotary_dim == kD, "single_query_attention: rotary_dim=%d must equal head_dim (llama_w4a8_unpad.py:258)", a.rotary_dim);
-  const int bits = a.int4_kv ? 4 : 8;
-  QS_REQUIRE(a.size_per_token == a.num_kv_heads * kD * bits / 8, "single_query_attention: size_per_token=%d does not match %d kv heads x %d bits",
-             a.size_per_token, a.num_kv_heads, bits);
   QS_REQUIRE(a.batch <= 65535, "single_query_attention: batch=%d too large", a.batch);
-  PageGeom pg{a.tokens_per_block, a.tokens_per_block * a.size_per_token, a.num_kv_heads};
+  PageGeom pg{kPageTokens, kPageTokens * a.size_per_token, a.num_kv_heads};
   const int G = a.num_heads / a.num_kv_heads;
   const int gparts = (G + kMaxG - 1) / kMaxG;
   const int gx = a.num_kv_heads * gparts;
-  // context splits: enough CTAs to fill the machine (4 resident CTAs per SM), never more than one split per 256 tokens
-  int nsplit = 1;
-  const int ctas = gx * a.batch;
-  const int slots = num_sms() * 4;
-  if (2 * ctas <= slots && a.timestep > 512) {
-    nsplit = (slots + ctas - 1) / ctas;
-    const int cap = (a.timestep + 255) / 256;
-    if (nsplit > cap) nsplit = cap;
-    if (nsplit > 32) nsplit = 32;
-  }
+  int nsplit = context_splits(static_cast<long long>(gx) * a.batch, num_sms() * 4, a.timestep);  // over 4 resident CTAs per SM
   float* part = nullptr;
   uint32_t* cnt = nullptr;
   if (nsplit > 1) {
@@ -980,7 +944,6 @@ int decode_attention(const DecodeAttnArgs& a) {
                   tok_cnt, static_cast<int8_t*>(a.q_out), static_cast<__half*>(a.q_scale), static_cast<__half*>(a.q_sum),
                   static_cast<unsigned long long*>(a.prof), static_cast<const int*>(nullptr), 0);
   };
-  QS_REQUIRE(a.tokens_per_block == kPageTokens, "single_query_attention: tokens_per_block=%d, only 64 is supported (cache_engine block_size)", a.tokens_per_block);
   return a.int4_kv ? run(decode_attention_kernel<4>, static_cast<size_t>(kWarps) * StageLayout<4>::kWarpBytes)
                    : run(decode_attention_kernel<8>, static_cast<size_t>(kWarps) * StageLayout<8>::kWarpBytes);
 }

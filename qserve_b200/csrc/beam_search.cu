@@ -332,10 +332,9 @@ int beam_reorder(const BeamReorderArgs& a) {
              "beam_reorder: layers=%d (1 .. 32767) batch=%d beam_width=%d (1 .. %d) max_blocks=%d kv_heads=%d history_len=%d", a.layers, a.batch,
              a.beam_width, kMaxBeam, a.max_blocks, a.num_kv_heads, a.history_len);
   QS_REQUIRE(a.batch % a.beam_width == 0, "beam_reorder: batch=%d is not a multiple of beam_width=%d", a.batch, a.beam_width);
-  QS_REQUIRE(a.tokens_per_block == kTokensPerPage, "beam_reorder: tokens_per_block=%d, only 64 is supported", a.tokens_per_block);
-  const int bits = a.int4_kv ? 4 : 8;
-  QS_REQUIRE(a.size_per_token == a.num_kv_heads * 128 * bits / 8, "beam_reorder: size_per_token=%d does not match %d kv heads x %d bits",
-             a.size_per_token, a.num_kv_heads, bits);
+  // page geometry only: these ops have no query heads
+  const int rc = check_page_geometry("beam_reorder", 128, a.num_kv_heads, a.num_kv_heads, a.tokens_per_block, a.size_per_token, a.int4_kv);
+  if (rc) return rc;
   if (a.batch == 0) return QS_OK;
   QS_REQUIRE(a.kv_pointers && a.parents && a.context_lens && a.prompt_lens && a.tokens && a.history, "beam_reorder: null pointer");
   const int code_bytes = kTokensPerPage * a.size_per_token;

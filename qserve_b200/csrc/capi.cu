@@ -49,6 +49,16 @@ int num_sms() {
   return sms[dev];
 }
 
+int check_page_geometry(const char* op, int head_dim, int num_heads, int num_kv_heads, int tokens_per_block, int size_per_token, int int4_kv) {
+  QS_REQUIRE(head_dim == 128, "%s: head_dim=%d, only 128 is supported", op, head_dim);
+  QS_REQUIRE(num_kv_heads > 0 && num_heads % num_kv_heads == 0, "%s: heads %d / kv heads %d", op, num_heads, num_kv_heads);
+  QS_REQUIRE(tokens_per_block == 64, "%s: tokens_per_block=%d, only 64 is supported", op, tokens_per_block);
+  const int bits = int4_kv ? 4 : 8;
+  QS_REQUIRE(size_per_token == num_kv_heads * 128 * bits / 8, "%s: size_per_token=%d does not match %d kv heads x %d bits", op, size_per_token,
+             num_kv_heads, bits);
+  return QS_OK;
+}
+
 int raise_smem_limit(const void* kern, size_t bytes, const char* what) {
   static std::mutex mu;
   static std::map<std::pair<const void*, int>, size_t> limits;

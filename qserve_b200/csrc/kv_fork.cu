@@ -53,10 +53,9 @@ int kv_cache_fork(const KvForkArgs& a) {
              "kv_cache_fork: layers=%d (1 .. 65535) batch=%d num_pairs=%d max_blocks=%d kv_heads=%d", a.layers, a.batch, a.num_pairs, a.max_blocks,
              a.num_kv_heads);
   QS_REQUIRE(a.num_pairs <= 0x3fffffff, "kv_cache_fork: num_pairs=%d too large", a.num_pairs);
-  QS_REQUIRE(a.tokens_per_block == kTokensPerPage, "kv_cache_fork: tokens_per_block=%d, only 64 is supported", a.tokens_per_block);
-  const int bits = a.int4_kv ? 4 : 8;
-  QS_REQUIRE(a.size_per_token == a.num_kv_heads * 128 * bits / 8, "kv_cache_fork: size_per_token=%d does not match %d kv heads x %d bits",
-             a.size_per_token, a.num_kv_heads, bits);
+  // page geometry only: these ops have no query heads
+  const int rc = check_page_geometry("kv_cache_fork", 128, a.num_kv_heads, a.num_kv_heads, a.tokens_per_block, a.size_per_token, a.int4_kv);
+  if (rc) return rc;
   if (a.batch == 0 || a.num_pairs == 0) return QS_OK;
   QS_REQUIRE(a.kv_pointers && a.parents && a.children && a.lens, "kv_cache_fork: null pointer");
   const int code_bytes = kTokensPerPage * a.size_per_token;

@@ -12,6 +12,10 @@ bool pdl_enabled();
 constexpr int kMaxDevices = 64;
 int device_ordinal();
 int num_sms();
+// The paged INT4 / INT8 KV cache the ops that read pages, or move them, are built for (capi.cu; messages start with `op`): 128-dim heads, a
+// multiple of the KV heads as query heads, 64-token pages and size_per_token = Hkv x 128 codes of 4 or 8 bits.  Ops without query heads pass
+// head_dim = 128 and num_heads = num_kv_heads.
+int check_page_geometry(const char* op, int head_dim, int num_heads, int num_kv_heads, int tokens_per_block, int size_per_token, int int4_kv);
 
 struct GemmArgs {
   const void* act = nullptr;        // int8 [M, K]

@@ -306,7 +306,6 @@ __global__ void __launch_bounds__(kAttnConsumers, kMinBlocks<NT>) multi_token_at
   }
 }
 
-constexpr int kMaxSplits = 32;
 // The split counters sit in a fixed region at the start of the workspace, so that the partials of one launch shape never overlap the
 // counters of another (the workspace is reused across shapes and the counters must read zero at every launch).
 constexpr size_t kCounterBytes = 16384;
@@ -318,47 +317,9 @@ struct MultiTokenPlan {
   size_t cnt_bytes, part_bytes;
 };
 
-// Launch shape: C = 8 columns when the (query heads of a group) x (draft tokens) fit one n8 tile, else 16; context splits as
-// decode_attention() chooses them (enough CTAs to fill the resident slots, at most one split per 256 cached tokens, at most 32).
-template <int BITS, int NT>
-int resident_ctas() {
-  // kernel attribute (the KV8 ring exceeds the default 48 KB of dynamic shared memory) and occupancy, once per device
-  static int cached[kMaxDevices] = {};
-  int& r = cached[device_ordinal()];
-  if (r == 0) {
-    const int smem = kWarps * StageLayout<BITS>::kWarpBytes;
-    int n = 0;
-    if (raise_smem_limit(multi_token_attention_kernel<BITS, NT, false>, smem, "multi_token_decode_attention smem attribute") != QS_OK ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, multi_token_attention_kernel<BITS, NT, false>, kAttnConsumers, smem) != cudaSuccess || n < 1) {
-      cudaGetLastError();
-      n = 1;
-    }
-    r = n;
-  }
-  return r;
-}
-
-MultiTokenPlan plan_multi_token(int bits, int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads) {
-  MultiTokenPlan pl{};
-  const int G = num_heads / num_kv_heads;
-  const int cols = G * max_seqlen;
-  pl.ntile = cols <= 8 ? 1 : 2;
-  pl.cparts = (cols + 8 * pl.ntile - 1) / (8 * pl.ntile);
-  const int ctx = max_prefix_len + max_seqlen - 1;
-  const long long ctas = static_cast<long long>(num_kv_heads) * pl.cparts * batch;
-  const int per_sm = bits == 4 ? (pl.ntile == 1 ? resident_ctas<4, 1>() : resident_ctas<4, 2>())
-                                : (pl.ntile == 1 ? resident_ctas<8, 1>() : resident_ctas<8, 2>());
-  const long long slots = static_cast<long long>(num_sms()) * per_sm;
-  pl.nsplit = 1;
-  if (2 * ctas <= slots && ctx > 512 && ctas <= static_cast<long long>(kCounterBytes / sizeof(uint32_t))) {
-    pl.nsplit = static_cast<int>((slots + ctas - 1) / ctas);
-    pl.nsplit = min(pl.nsplit, (ctx + 255) / 256);
-    pl.nsplit = min(pl.nsplit, kMaxSplits);
-  }
-  pl.cnt_bytes = kCounterBytes;
-  pl.part_bytes = pl.nsplit > 1 ? static_cast<size_t>(num_tokens) * num_heads * pl.nsplit * (kD + 2) * sizeof(float) : 0;
-  return pl;
-}
+// Defined at the end of the file: the launch sites below then name the kernels first, and the kernels are emitted in that order.  ptxas's
+// code for an instantiation depends on the order, and this one is the order the kernels were measured in.
+MultiTokenPlan plan_multi_token(int bits, int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads);
 
 }  // namespace
 
@@ -370,15 +331,13 @@ size_t multi_token_attention_workspace_bytes(int batch, int num_tokens, int max_
 }
 
 int multi_token_attention(const MultiTokenAttnArgs& a) {
-  QS_REQUIRE(a.head_dim == kD, "multi_token_decode_attention: head_dim=%d (only 128 is built)", a.head_dim);
-  QS_REQUIRE(a.num_heads > 0 && a.num_kv_heads > 0 && a.num_heads % a.num_kv_heads == 0, "multi_token_decode_attention: heads=%d kv_heads=%d",
-             a.num_heads, a.num_kv_heads);
-  QS_REQUIRE(a.batch >= 0 && a.num_tokens >= 0 && a.max_prefix_len >= 0, "multi_token_decode_attention: negative size");
+  const int rc = check_page_geometry("multi_token_decode_attention", a.head_dim, a.num_heads, a.num_kv_heads, a.tokens_per_block, a.size_per_token,
+                                     a.int4_kv);
+  if (rc) return rc;
+  QS_REQUIRE(a.num_heads > 0 && a.batch >= 0 && a.num_tokens >= 0 && a.max_prefix_len >= 0, "multi_token_decode_attention: heads=%d, or negative size",
+             a.num_heads);
   QS_REQUIRE(a.max_seqlen >= 1 && a.max_seqlen <= 16, "multi_token_decode_attention: max_seqlen=%d, must be 1 .. 16", a.max_seqlen);
-  QS_REQUIRE(a.tokens_per_block == kPageTokens, "multi_token_decode_attention: tokens_per_block=%d, only 64 is supported", a.tokens_per_block);
   const int bits = a.int4_kv ? 4 : 8;
-  QS_REQUIRE(a.size_per_token == a.num_kv_heads * kD * bits / 8, "multi_token_decode_attention: size_per_token=%d does not match %d kv heads x %d bits",
-             a.size_per_token, a.num_kv_heads, bits);
   QS_REQUIRE(static_cast<long long>(a.max_prefix_len) + a.max_seqlen <= static_cast<long long>(a.max_blocks) * kPageTokens,
              "multi_token_decode_attention: max_prefix_len %d + max_seqlen %d exceed the page table (%d blocks of %d tokens)", a.max_prefix_len,
              a.max_seqlen, a.max_blocks, kPageTokens);
@@ -430,5 +389,31 @@ int multi_token_attention(const MultiTokenAttnArgs& a) {
   if (a.int4_kv) return pl.ntile == 1 ? run(multi_token_attention_kernel<4, 1, false>, smem4) : run(multi_token_attention_kernel<4, 2, false>, smem4);
   return pl.ntile == 1 ? run(multi_token_attention_kernel<8, 1, false>, smem8) : run(multi_token_attention_kernel<8, 2, false>, smem8);
 }
+
+namespace {
+
+// Launch shape: C = 8 columns when the (query heads of a group) x (draft tokens) fit one n8 tile, else 16; context_splits over the resident
+// CTAs, as long as the split counters fit their region.
+MultiTokenPlan plan_multi_token(int bits, int batch, int num_tokens, int max_seqlen, int max_prefix_len, int num_heads, int num_kv_heads) {
+  MultiTokenPlan pl{};
+  const int G = num_heads / num_kv_heads;
+  const int cols = G * max_seqlen;
+  pl.ntile = cols <= 8 ? 1 : 2;
+  pl.cparts = (cols + 8 * pl.ntile - 1) / (8 * pl.ntile);
+  const int ctx = max_prefix_len + max_seqlen - 1;
+  const long long ctas = static_cast<long long>(num_kv_heads) * pl.cparts * batch;
+  const int smem = kWarps * (bits == 4 ? StageLayout<4>::kWarpBytes : StageLayout<8>::kWarpBytes);
+  const char* what = "multi_token_decode_attention smem attribute";
+  const int per_sm = bits == 4 ? (pl.ntile == 1 ? resident_ctas<multi_token_attention_kernel<4, 1, false>>(smem, what)
+                                                : resident_ctas<multi_token_attention_kernel<4, 2, false>>(smem, what))
+                                : (pl.ntile == 1 ? resident_ctas<multi_token_attention_kernel<8, 1, false>>(smem, what)
+                                                : resident_ctas<multi_token_attention_kernel<8, 2, false>>(smem, what));
+  pl.nsplit = ctas <= static_cast<long long>(kCounterBytes / sizeof(uint32_t)) ? context_splits(ctas, static_cast<long long>(num_sms()) * per_sm, ctx) : 1;
+  pl.cnt_bytes = kCounterBytes;
+  pl.part_bytes = pl.nsplit > 1 ? static_cast<size_t>(num_tokens) * num_heads * pl.nsplit * (kD + 2) * sizeof(float) : 0;
+  return pl;
+}
+
+}  // namespace
 
 }  // namespace qs

@@ -6,7 +6,10 @@
 
 #include <math_constants.h>
 
+#include <algorithm>
+
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace qs {
 namespace {
@@ -445,6 +448,36 @@ __device__ __forceinline__ float merge_splits(const float* pr, int nsplit, int d
     acc += __ldcg(pr + sp * (kD + 2) + d) * e;
   }
   return acc * __fdividef(1.f, L + 1.e-6f);
+}
+
+// =========================================================================================================================================
+// Host: the launch plan of the paged-attention kernels
+// =========================================================================================================================================
+
+// Context splits of a launch of `ctas` CTAs over `ctx` cached tokens: enough CTAs to fill the `slots` resident CTAs of the machine when the
+// launch fills at most half of them, never more than one split per 256 tokens, at most 32, and none up to 512 tokens
+inline int context_splits(long long ctas, long long slots, int ctx) {
+  if (2 * ctas > slots || ctx <= 512) return 1;
+  return static_cast<int>(std::min<long long>(std::min<long long>((slots + ctas - 1) / ctas, (ctx + 255) / 256), 32));
+}
+
+// Resident CTAs per SM of a paged-attention kernel with `smem` bytes of dynamic shared memory (its rings), asked once per device (this raises
+// the kernel's dynamic shared memory limit: the KV8 rings exceed the default 48 KB; a failure is reported as `what`); 1 if the occupancy
+// calculator fails.  A function of host integers only, so a launch planned with it can be captured in a graph.
+template <auto KERNEL>
+int resident_ctas(int smem, const char* what) {
+  static int cached[kMaxDevices] = {};
+  int& r = cached[device_ordinal()];
+  if (r == 0) {
+    int n = 0;
+    if (raise_smem_limit(KERNEL, smem, what) != QS_OK ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, KERNEL, kAttnConsumers, smem) != cudaSuccess || n < 1) {
+      cudaGetLastError();
+      n = 1;
+    }
+    r = n;
+  }
+  return r;
 }
 
 }  // namespace

@@ -229,16 +229,14 @@ prefix_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
 
 int prefix_attention(const PrefixAttnArgs& a) {
   QS_REQUIRE(a.max_prefix_len >= 0, "prefix_prefill_attention: negative size");
-  QS_REQUIRE(a.tokens_per_block == kPageTokens, "prefix_prefill_attention: tokens_per_block=%d, only 64 is supported", a.tokens_per_block);
-  const int bits = a.int4_kv ? 4 : 8;
-  QS_REQUIRE(a.size_per_token == a.num_kv_heads * kD * bits / 8, "prefix_prefill_attention: size_per_token=%d does not match %d kv heads x %d bits",
-             a.size_per_token, a.num_kv_heads, bits);
+  int rc = check_page_geometry("prefix_prefill_attention", a.head_dim, a.num_heads, a.num_kv_heads, a.tokens_per_block, a.size_per_token, a.int4_kv);
+  if (rc) return rc;
   QS_REQUIRE(static_cast<long long>(a.max_prefix_len) + a.max_seqlen <= static_cast<long long>(a.max_blocks) * kPageTokens,
              "prefix_prefill_attention: max_prefix_len %d + max_seqlen %d exceed the page table (%d blocks of %d tokens)", a.max_prefix_len, a.max_seqlen,
              a.max_blocks, kPageTokens);
   bool empty = false;
   CUtensorMap tq, tk, tv;
-  int rc = prompt_attention_prepare(a, "prefix_prefill_attention", &empty, &tq, &tk, &tv);
+  rc = prompt_attention_prepare(a, "prefix_prefill_attention", &empty, &tq, &tk, &tv);
   if (rc || empty) return rc;
   QS_REQUIRE(a.prefix_lens && a.kv_pointers, "prefix_prefill_attention: null pointer");
   PrefixAttnParams p{};

@@ -134,10 +134,9 @@ int kv_cache_compact(const KvCompactArgs& a) {
   QS_REQUIRE(a.layers >= 1 && a.batch >= 0 && a.num_nodes >= 1 && a.num_nodes <= kMaxNodes && a.max_blocks >= 1 && a.num_kv_heads >= 1,
              "kv_cache_compact: layers=%d batch=%d num_nodes=%d (1 .. 16) max_blocks=%d kv_heads=%d", a.layers, a.batch, a.num_nodes, a.max_blocks,
              a.num_kv_heads);
-  QS_REQUIRE(a.tokens_per_block == kTokensPerPage, "kv_cache_compact: tokens_per_block=%d, only 64 is supported", a.tokens_per_block);
-  const int bits = a.int4_kv ? 4 : 8;
-  QS_REQUIRE(a.size_per_token == a.num_kv_heads * 128 * bits / 8, "kv_cache_compact: size_per_token=%d does not match %d kv heads x %d bits",
-             a.size_per_token, a.num_kv_heads, bits);
+  // page geometry only: these ops have no query heads
+  const int rc = check_page_geometry("kv_cache_compact", 128, a.num_kv_heads, a.num_kv_heads, a.tokens_per_block, a.size_per_token, a.int4_kv);
+  if (rc) return rc;
   if (a.batch == 0) return QS_OK;
   QS_REQUIRE(a.kv_pointers && a.start_pos && a.path && a.accept_len, "kv_cache_compact: null pointer");
   const long long n_warps = static_cast<long long>(a.layers) * a.batch * 2 * a.num_kv_heads;
