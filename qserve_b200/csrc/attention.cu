@@ -54,8 +54,8 @@ __device__ __forceinline__ uint32_t kv_quant_code(float x, float inv_s, float z)
 //   side, output rows rescaled at the end on the V side); sum_d (1024 + w_d u_d) q'_d = B(q) + sum_d u_d q_d with B(q) computed
 //   once per head, and sum_t p'_t (1024 + u_t) = 1024 sum_t p'_t + ... with sum_t p'_t from one MMA against an all-ones tile.
 // ------------------------------------------------------------------------------------------------
-// This kernel and multi_token_attention_kernel are both built on paged_attention.cuh (one n8 tile here: the <= 8 heads of the group); the
-// output bits of this kernel are pinned by tests/test_gpu_attention.py::test_decode_attention_output_bits_are_pinned.
+// This kernel, multi_token_attention_kernel and shared_prefix_attention_kernel are built on paged_attention.cuh (one n8 tile here: the <= 8
+// heads of the group); the output bits of this kernel are pinned by tests/test_gpu_attention.py::test_decode_attention_output_bits_are_pinned.
 constexpr int kAttnThreadsV2 = kAttnConsumers;  // no dedicated producer warp: every warp streams its own half pages
 
 // SHARED (the row pass of qs_shared_prefix_decode_attention, DESIGN.md 3.10): the row's pages start at row_pages[b]; a row with
@@ -453,10 +453,10 @@ decode_attention_kernel(const __half* __restrict__ q_in, const __half* __restric
 // ------------------------------------------------------------------------------------------------
 // K1s: shared pass of qs_shared_prefix_decode_attention (DESIGN.md 3.10).  Rows forked from one prompt share the pages 0 .. S_g - 1 of their
 //   group g.  One CTA owns (KV head, column part, group, context split); column c of part cp is (member j, query head h) with C cp + c = j G + h,
-//   so every code a warp unpacks feeds C = 8 NT columns, as in multi_token_attention_kernel (DESIGN.md 3.6).  Member j's q is rotated at its
-//   own position lengths[row_j] - 1 (members diverge once a finished row stops advancing) through the decode kernel's RoPE functions.
-//   Every shared token is valid for every member (the caller guarantees 64 S_g cached tokens), so there is no causal tail, no own token and
-//   no append.  The CTA writes one unnormalised partial (O, max, sum) per (member row, head) at split slot part_off + split of the row's
+//   so every code a warp unpacks feeds C = 8 NT columns: the page stream is column_tile_stream, shared with multi_token_attention_kernel
+//   (DESIGN.md 3.6).  Member j's q is rotated at its own position lengths[row_j] - 1 (members diverge once a finished row stops advancing)
+//   through the decode kernel's RoPE functions.  Every shared token is valid for every member (the caller guarantees 64 S_g cached tokens),
+//   so there is no causal tail, no own token and no append.  The CTA writes one unnormalised partial (O, max, sum) per (member row, head) at split slot part_off + split of the row's
 //   partials; the row pass (decode_attention_kernel<BITS, true>) merges them after its own splits.
 // ------------------------------------------------------------------------------------------------
 struct SharedPrefixParams {
@@ -476,24 +476,14 @@ struct SharedPrefixParams {
   float* ws_part;                 // [B, Hq, part_stride, 130]
 };
 
-// ptxas needs more than 128 registers for two n8 tiles without spilling (the O^T accumulators alone are 32 per tile), as in
-// multi_token_attention_kernel
-template <int NT>
-constexpr int kSharedMinBlocks = NT == 1 ? 3 : 2;
-
 template <int BITS, int NT>
-__global__ void __launch_bounds__(kAttnConsumers, kSharedMinBlocks<NT>) shared_prefix_attention_kernel(const SharedPrefixParams p) {
-  using SL = StageLayout<BITS>;
-  constexpr int R = SL::kStages;
+__global__ void __launch_bounds__(kAttnConsumers, kColumnMinBlocks<NT>) shared_prefix_attention_kernel(const SharedPrefixParams p) {
   constexpr int C = 8 * NT;
-  static_assert(SL::kWarpBytes >= C * kOStride * 4, "the per-warp ring must hold the warp's partial output");
   const int G = p.num_heads / p.num_kv_heads;
   const int hk = blockIdx.x / p.cparts;
   const int col0 = (blockIdx.x - hk * p.cparts) * C;
   const int grp = blockIdx.y;
   const int split = blockIdx.z;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, q4 = lane & 3;
 
   // the layout and the tables are prepared by the host before the step: read before the dependency wait; q and the pages after it
   const int mem0 = p.group_offsets[grp];
@@ -504,48 +494,16 @@ __global__ void __launch_bounds__(kAttnConsumers, kSharedMinBlocks<NT>) shared_p
 
   extern __shared__ __align__(128) uint8_t smem_attn[];
   uint8_t* s_ring = smem_attn;
-  __shared__ __align__(16) __half s_q[C * kD];
-  __shared__ uint4 s_qb[NT][4][32];
-  __shared__ float s_m[kWarps + 1][C], s_l[kWarps + 1][C];
-  __shared__ float s_f[kWarps + 1][C];
-  __shared__ float2 s_meta[kWarps][2][kSliceTokens];
-  __shared__ __align__(8) uint64_t s_full[kWarps][R];
+  __shared__ ColumnShared<BITS, NT> sh;
 
-  if (lane == 0) {
-    for (int i = 0; i < R; ++i) mbar_init(&s_full[warp][i], 1);
-    fence_barrier_init();
-  }
-  __syncwarp();
-  if (threadIdx.x == 0) pdl_launch_dependents();
-
-  const int row0 = p.group_rows[mem0];
-  const long long* kptrs = p.kv_pointers + (static_cast<size_t>(row0) * 2 + 0) * p.max_blocks;
-  const long long* vptrs = p.kv_pointers + (static_cast<size_t>(row0) * 2 + 1) * p.max_blocks;
-  const int pps = (S + p.nsplit - 1) / p.nsplit;
-  const int p_begin = split * pps, p_end = min(S, p_begin + pps);
-  const int hslice = warp & 1;
-  const int my_first = p_begin + (warp >> 1);
-  const int n_my = (p_end > my_first) ? (p_end - my_first + 1) / 2 : 0;
-  uint8_t* my_ring = s_ring + warp * SL::kWarpBytes;
-  uint64_t* my_full = &s_full[warp][0];
-  const int zoff = p.pg.num_kv_heads * p.pg.tokens_per_block * 2;
-  long long kp_l = 0, vp_l = 0;
-  auto load_ptr_batch = [&](int j0) { slice_ptrs(kptrs, vptrs, my_first + 2 * (j0 + lane), p_end, kp_l, vp_l); };
-  auto issue = [&](int j, int slot) {
-    issue_slice<BITS>(lane, kp_l, vp_l, j, my_ring + slot * SL::kBytes, &my_full[slot], hk, hslice, p.pg.code_bytes, zoff);
-  };
-  load_ptr_batch(0);
-  // thread t rotates the pair (ri, ri + 64) of columns t / 64, t / 64 + 2, ...: the member rows and positions of those columns
-  const int ri = threadIdx.x & 63, c0 = threadIdx.x >> 6;
-  const int half_rot = p.rotary_dim / 2;
-  pdl_wait();
-  for (int j = 0; j < R && j < n_my; ++j) issue(j, j);
-
-  {
+  auto stage = [&] {
+    // thread t rotates the pair (ri, ri + 64) of columns t / 64, t / 64 + 2, ...: the member rows and positions of those columns
+    const int ri = threadIdx.x & 63, c0 = threadIdx.x >> 6;
+    const int half_rot = p.rotary_dim / 2;
     int last_pos = -1;
     float sn = 0.f, cs = 1.f;
     for (int c = c0; c < C; c += 2) {
-      __half* dst = s_q + c * kD;
+      __half* dst = sh.q + c * kD;
       if (c < ncol) {
         const int j = (col0 + c) / G, h = col0 + c - j * G;
         const int row = p.group_rows[mem0 + j];
@@ -561,100 +519,30 @@ __global__ void __launch_bounds__(kAttnConsumers, kSharedMinBlocks<NT>) shared_p
         dst[ri] = dst[ri + half_rot] = __float2half_rn(0.f);
       }
     }
-  }
-  __syncthreads();
-
-  float sumq[NT][2], biasq[NT][2];
-#pragma unroll
-  for (int t = 0; t < NT; ++t) {
-    uint32_t qb0[8], qb1[8];
-    q_operand<BITS>(s_q + (8 * t + g) * kD + 32 * q4, q4, qb0, qb1, sumq[t], biasq[t]);
-    if (warp == 0) {
-#pragma unroll
-      for (int w = 0; w < 4; ++w) s_qb[t][w][lane] = make_uint4(qb0[2 * w], qb1[2 * w], qb0[2 * w + 1], qb1[2 * w + 1]);
-    }
-  }
-  __syncthreads();
-  auto qb = [&](int t, int ks, uint32_t& b0, uint32_t& b1) {
-    const uint4 qq = s_qb[t][ks >> 1][lane];
-    b0 = (ks & 1) ? qq.z : qq.x;
-    b1 = (ks & 1) ? qq.w : qq.y;
   };
-
-  const float sm_scale = rsqrtf(static_cast<float>(kD)) * 1.4426950408889634f;  // the decode kernel's
-  float o[NT][8][4];
-  float m[NT][2], l[NT][2], cr[NT][2], spa[NT][4];
-#pragma unroll
-  for (int t = 0; t < NT; ++t) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) o[t][i][0] = o[t][i][1] = o[t][i][2] = o[t][i][3] = 0.f;
-    m[t][0] = m[t][1] = -CUDART_INF_F;
-    l[t][0] = l[t][1] = cr[t][0] = cr[t][1] = 0.f;
-    spa[t][0] = spa[t][1] = spa[t][2] = spa[t][3] = 0.f;
-  }
-
-  const int tokA = (g & 1) * 4 + (g >> 1);
-  constexpr int kRow = kD * BITS / 8;
-  int s = 0;
-  uint32_t ph = 0;
-  for (int j = 0; j < n_my; ++j) {
-    mbar_wait(&my_full[s], ph);
-    const uint8_t* st = my_ring + s * SL::kBytes;
-    slice_meta<BITS>(st, lane, false, sm_scale, s_meta[warp][0], s_meta[warp][1]);
-    __syncwarp();
-    float sc[2][NT][4];
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-#pragma unroll
-      for (int t = 0; t < NT; ++t) sc[c][t][0] = sc[c][t][1] = sc[c][t][2] = sc[c][t][3] = 0.f;
-      qk_chunk<BITS, NT>(st + SL::kOffK + (c * kChunk + tokA) * kRow, q4, sc[c], qb);
-    }
-    float tl[2][NT][4], vs[2][2], vc[2][2];
-#pragma unroll
-    for (int c = 0; c < 2; ++c) chunk_logits<NT>(s_meta[warp][0], s_meta[warp][1], c, tokA, sc[c], biasq, sumq, tl[c], vs[c], vc[c]);
-    uint32_t bp[2][NT][2];
-#pragma unroll
-    for (int t = 0; t < NT; ++t) softmax_tile<NT, false>(t, tl, vs, vc, m[t], l[t], cr[t], spa[t], o[t], bp);
-#pragma unroll
-    for (int c = 0; c < 2; ++c) pv_chunk<BITS, NT>(st + SL::kOffV + (c * kChunk + q4) * kRow, g, o, bp[c]);
-    __syncwarp();
-    if (j + R < n_my) {
-      if (((j + R) & 31) == 0) load_ptr_batch(j + R);
-      issue(j + R, s);
-    }
-    if (++s == R) { s = 0; ph ^= 1; }
-  }
-
-#pragma unroll
-  for (int t = 0; t < NT; ++t) reduce_tile_sums(l[t], cr[t]);
-  if (g == 0) {
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      s_m[warp][8 * t + 2 * q4] = m[t][0]; s_m[warp][8 * t + 2 * q4 + 1] = m[t][1];
-      s_l[warp][8 * t + 2 * q4] = l[t][0]; s_l[warp][8 * t + 2 * q4 + 1] = l[t][1];
-    }
-  }
-  __syncwarp();
-#pragma unroll
-  for (int t = 0; t < NT; ++t) store_partial<BITS>(reinterpret_cast<float*>(my_ring) + (8 * t + 2 * q4) * kOStride + g, o[t], spa[t], cr[t]);
+  auto none_unread = [](int) { return false; };
+  auto no_tail = [](int, int, float (&)[2][NT][4]) {};
+  // the shared pages through the table of the group's first row; the decode kernel's softmax scale
+  column_tile_stream<BITS, NT, false>(sh, s_ring, p.kv_pointers, p.group_rows[mem0], p.max_blocks, p.pg, hk, S, p.nsplit,
+                                      rsqrtf(static_cast<float>(kD)) * 1.4426950408889634f, stage, none_unread, no_tail);
   __syncthreads();
 
   // merge the warps; never normalised here (nsplit argument 0): the row pass normalises after its merge of every part
-  if (threadIdx.x < C) merge_weights<C>(threadIdx.x, kWarps, 0, s_m, s_l, s_f);
+  if (threadIdx.x < C) merge_weights<C>(threadIdx.x, kWarps, 0, sh.m, sh.l, sh.f);
   __syncthreads();
   if (threadIdx.x < kD) {
     const int d = 16 * (threadIdx.x & 7) + (threadIdx.x >> 3);
 #pragma unroll
     for (int r = 0; r < C; ++r) {
       if (r < ncol) {
-        const float acc = merge_warps<BITS, C>(s_ring, r, 0.f, s_f);
+        const float acc = merge_warps<BITS, C>(s_ring, r, 0.f, sh.f);
         const int j = (col0 + r) / G, h = col0 + r - j * G;
         const int row = p.group_rows[mem0 + j];
         float* pr = p.ws_part + ((static_cast<size_t>(row) * p.num_heads + hk * G + h) * p.part_stride + p.part_off + split) * (kD + 2);
         pr[d] = acc;
         if (threadIdx.x == 0) {
-          pr[kD] = s_m[0][r];
-          pr[kD + 1] = s_l[0][r];
+          pr[kD] = sh.m[0][r];
+          pr[kD + 1] = sh.l[0][r];
         }
       }
     }
@@ -783,11 +671,15 @@ constexpr size_t kAttnTokCounterOffset = 192 * 1024;
 struct SharedPrefixPlan {
   int gx;          // row pass: KV heads x head groups of <= 8 query heads
   int nsplit;      // row pass context splits (decode_attention's)
-  int ntile;       // shared pass: n8 tiles per CTA (C = 8 ntile columns of (member, query head))
-  int cparts;      // shared pass: column parts per KV head
-  int sp_nsplit;   // shared pass: context splits of the shared pages (0: no shared pass)
+  ColumnPlan sp;   // shared pass over (member, query head) columns; sp.nsplit = 0: no shared pass
   size_t part_bytes, row_bytes;
 };
+
+// shared_prefix_attention_kernel<bits, ntile>: the one place the plan's occupancy lookup and the launch pick it
+ColumnKernel<void (*)(SharedPrefixParams)> shared_prefix_kernel(int bits, int ntile) {
+  if (bits == 4) return ntile == 1 ? column_kernel<shared_prefix_attention_kernel<4, 1>>() : column_kernel<shared_prefix_attention_kernel<4, 2>>();
+  return ntile == 1 ? column_kernel<shared_prefix_attention_kernel<8, 1>>() : column_kernel<shared_prefix_attention_kernel<8, 2>>();
+}
 
 // The launch plan of qs_shared_prefix_decode_attention: a function of host integers only, so the call can be captured in a graph
 SharedPrefixPlan plan_shared_prefix(int bits, int batch, int num_heads, int num_kv_heads, int timestep, int num_groups, int max_group, int max_pages) {
@@ -796,19 +688,10 @@ SharedPrefixPlan plan_shared_prefix(int bits, int batch, int num_heads, int num_
   pl.gx = num_kv_heads * ((G + kMaxG - 1) / kMaxG);
   pl.nsplit = context_splits(static_cast<long long>(pl.gx) * batch, num_sms() * 4, timestep);
   if (num_groups > 0 && max_group > 0 && max_pages > 0) {
-    const int cols = G * max_group;
-    pl.ntile = cols <= 8 ? 1 : 2;
-    pl.cparts = (cols + 8 * pl.ntile - 1) / (8 * pl.ntile);
-    const long long sctas = static_cast<long long>(num_kv_heads) * pl.cparts * num_groups;
-    const int smem = kWarps * (bits == 4 ? StageLayout<4>::kWarpBytes : StageLayout<8>::kWarpBytes);
-    const char* what = "shared_prefix_decode_attention smem attribute";
-    const int per_sm = bits == 4 ? (pl.ntile == 1 ? resident_ctas<shared_prefix_attention_kernel<4, 1>>(smem, what)
-                                                 : resident_ctas<shared_prefix_attention_kernel<4, 2>>(smem, what))
-                                 : (pl.ntile == 1 ? resident_ctas<shared_prefix_attention_kernel<8, 1>>(smem, what)
-                                                 : resident_ctas<shared_prefix_attention_kernel<8, 2>>(smem, what));
-    pl.sp_nsplit = context_splits(sctas, static_cast<long long>(num_sms()) * per_sm, max_pages * kPageTokens);
+    auto per_sm = [&](int ntile) { return shared_prefix_kernel(bits, ntile).resident(ring_bytes(bits), "shared_prefix_decode_attention smem attribute"); };
+    pl.sp = plan_columns(G * max_group, static_cast<long long>(num_kv_heads) * num_groups, max_pages * kPageTokens, per_sm);
   }
-  pl.part_bytes = static_cast<size_t>(batch) * num_heads * (pl.nsplit + pl.sp_nsplit) * (kD + 2) * sizeof(float);
+  pl.part_bytes = static_cast<size_t>(batch) * num_heads * (pl.nsplit + pl.sp.nsplit) * (kD + 2) * sizeof(float);
   pl.row_bytes = static_cast<size_t>(batch) * num_heads * kD * sizeof(__half);
   return pl;
 }
@@ -851,10 +734,10 @@ int shared_prefix_decode_attention(const SharedPrefixAttnArgs& s) {
   uint32_t* tok_cnt = reinterpret_cast<uint32_t*>(ws + kAttnTokCounterOffset);
   float* part = reinterpret_cast<float*>(ws + kAttnCounterBytes);
   void* out = a.q_out != nullptr ? ws + kAttnCounterBytes + pl.part_bytes : a.out;
-  const int pstride = pl.nsplit + pl.sp_nsplit;
+  const int pstride = pl.nsplit + pl.sp.nsplit;
   PageGeom pg{kPageTokens, kPageTokens * a.size_per_token, a.num_kv_heads};
-  const size_t smem = static_cast<size_t>(kWarps) * (bits == 4 ? StageLayout<4>::kWarpBytes : StageLayout<8>::kWarpBytes);
-  if (pl.sp_nsplit > 0) {
+  const size_t smem = ring_bytes(bits);
+  if (pl.sp.nsplit > 0) {
     SharedPrefixParams p{};
     p.q = static_cast<const __half*>(a.q);
     p.q_stride = a.q_stride;
@@ -864,20 +747,15 @@ int shared_prefix_decode_attention(const SharedPrefixAttnArgs& s) {
     p.group_rows = s.group_rows;
     p.group_pages = s.group_pages;
     p.num_heads = a.num_heads; p.num_kv_heads = a.num_kv_heads; p.max_blocks = a.max_blocks;
-    p.cparts = pl.cparts; p.nsplit = pl.sp_nsplit;
+    p.cparts = pl.sp.cparts; p.nsplit = pl.sp.nsplit;
     p.part_off = pl.nsplit; p.part_stride = pstride;
     p.pg = pg;
     p.rotary_base = a.rotary_base; p.rotary_dim = a.rotary_dim;
     p.ws_part = part;
-    const dim3 grid(static_cast<unsigned>(a.num_kv_heads * pl.cparts), s.num_groups, pl.sp_nsplit);
-    auto run = [&](auto kern) {
-      const int rc = raise_smem_limit(kern, smem, "shared_prefix_decode_attention smem attribute");
-      if (rc) return rc;
-      return launch(kern, grid, dim3(kAttnConsumers), smem, 0, a.stream, "shared_prefix_decode_attention", p);
-    };
-    const int rc = bits == 4 ? (pl.ntile == 1 ? run(shared_prefix_attention_kernel<4, 1>) : run(shared_prefix_attention_kernel<4, 2>))
-                             : (pl.ntile == 1 ? run(shared_prefix_attention_kernel<8, 1>) : run(shared_prefix_attention_kernel<8, 2>));
-    if (rc) return rc;
+    const dim3 grid(static_cast<unsigned>(a.num_kv_heads * pl.sp.cparts), s.num_groups, pl.sp.nsplit);
+    const auto kern = shared_prefix_kernel(bits, pl.sp.ntile).fn;
+    if (const int err = raise_smem_limit(kern, smem, "shared_prefix_decode_attention smem attribute")) return err;
+    if (const int err = launch(kern, grid, dim3(kAttnConsumers), smem, 0, a.stream, "shared_prefix_decode_attention", p)) return err;
   }
   const dim3 grid(pl.gx, a.batch, pl.nsplit);
   auto run = [&](auto kern) {

@@ -1,7 +1,8 @@
 // qserve_b200 -- device helpers shared by the attention kernels that stream the INT4 / INT8 paged KV cache through per-warp bulk-copy rings
-// and multiply "biased" code operands with mma.sync m16n8k16: decode_attention_kernel (attention.cu, DESIGN.md 3.2) and
-// multi_token_attention_kernel (multi_token_attention.cu, DESIGN.md 3.6).  Everything here is internal to the translation unit that
-// includes it.
+// and multiply "biased" code operands with mma.sync m16n8k16: decode_attention_kernel (attention.cu, DESIGN.md 3.2), built on the pieces
+// below, and the two column-tile kernels built on column_tile_stream, the body they share: multi_token_attention_kernel
+// (multi_token_attention.cu, DESIGN.md 3.6) and shared_prefix_attention_kernel (attention.cu, DESIGN.md 3.10).  Everything here is internal
+// to the translation unit that includes it.
 #pragma once
 
 #include <math_constants.h>
@@ -80,7 +81,7 @@ __device__ __forceinline__ uint32_t movmatrix_trans(uint32_t x) {
 }
 
 // =========================================================================================================================================
-// Pieces of the paged-attention main loop shared by decode_attention_kernel and multi_token_attention_kernel.  Both kernels are 4 warps; the
+// Pieces of the paged-attention main loop shared by decode_attention_kernel and column_tile_stream.  The kernels are 4 warps; the
 // S^T / O^T tiles have the cache tokens on the m16 side and NT n8 tiles of "columns" (query heads, or draft token x query head) on the n side:
 // thread (g = lane / 4, q4 = lane % 4) holds columns 8t + 2q4, 8t + 2q4 + 1 of tile t.  See DESIGN.md 3.2 for the arithmetic.
 // =========================================================================================================================================
@@ -451,6 +452,156 @@ __device__ __forceinline__ float merge_splits(const float* pr, int nsplit, int d
 }
 
 // =========================================================================================================================================
+// The column-tile kernels: one CTA (4 warps) owns (KV head, column part, sequence or group, context split) and streams the pages of its
+// split once for C = 8 NT columns.  ptxas needs 134 - 152 registers for one n8 tile and 215 - 251 for two without spilling (the O^T
+// accumulators alone are 32 fp32 registers per tile), so the launch bound is 3 and 2 CTAs of 128 threads.  Shared memory can lower it
+// further (KV8, one tile: 2); the host asks the occupancy calculator (plan_columns).
+// =========================================================================================================================================
+template <int NT>
+constexpr int kColumnMinBlocks = NT == 1 ? 3 : 2;
+
+// the static shared memory of column_tile_stream; q is staged by the kernel, m / l / f are its merge's
+template <int BITS, int NT>
+struct ColumnShared {
+  __half q[8 * NT * kD];                              // the q row of each column
+  uint4 qb[NT][4][32];                                // Q B fragments, see column_tile_stream
+  float m[kWarps + 1][8 * NT], l[kWarps + 1][8 * NT];  // per-warp (and own-token: part kWarps) running max and sum of each column
+  float f[kWarps + 1][8 * NT];                        // merge weights exp2(m_w - M) [* 1 / L]
+  float2 meta[kWarps][2][kSliceTokens];               // per token (scale, c) of the slice in flight
+  uint64_t full[kWarps][StageLayout<BITS>::kStages];
+};
+
+// ---- the page stream of one column tile, from barrier init to the parked per-warp partials (m, l in sh.m / sh.l of part `warp`, O^T in the
+//      warp's drained ring, as store_partial lays it out): split blockIdx.z of nsplit of the n_pages pages of page-table row `row`.  Warp w
+//      consumes the token slice [32 (w & 1), +32) of the pages p_begin + (w >> 1), +2, ... through its ring.
+//      stage(): after the first R issues, the kernel writes the q row of every column to sh.q (it may read what the dependency wait guards).
+//      unread(t): no column reads cache token t (a slice of such tokens is skipped; their scales are forced to zero).
+//      tail(t0, tokA, tl): masks logits of the slice at cache token t0; EMPTY: a column may then have every key of a slice masked ----
+template <int BITS, int NT, bool EMPTY, class Stage, class Unread, class Tail>
+__device__ __forceinline__ void column_tile_stream(ColumnShared<BITS, NT>& sh, uint8_t* s_ring, const long long* kv_pointers, int row, int max_blocks,
+                                                   const PageGeom& pg, int hk, int n_pages, int nsplit, float sm_scale, const Stage& stage,
+                                                   const Unread& unread, const Tail& tail) {
+  using SL = StageLayout<BITS>;
+  constexpr int R = SL::kStages;
+  static_assert(SL::kWarpBytes >= 8 * NT * kOStride * 4, "the per-warp ring must hold the warp's partial output");
+  const int split = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, q4 = lane & 3;
+
+  if (lane == 0) {
+    for (int i = 0; i < R; ++i) mbar_init(&sh.full[warp][i], 1);
+    fence_barrier_init();
+  }
+  __syncwarp();
+  if (threadIdx.x == 0) pdl_launch_dependents();
+
+  const long long* kptrs = kv_pointers + (static_cast<size_t>(row) * 2 + 0) * max_blocks;
+  const long long* vptrs = kv_pointers + (static_cast<size_t>(row) * 2 + 1) * max_blocks;
+  const int pps = (n_pages + nsplit - 1) / nsplit;
+  const int p_begin = split * pps, p_end = min(n_pages, p_begin + pps);
+  const int hslice = warp & 1;
+  const int my_first = p_begin + (warp >> 1);
+  const int n_my = (p_end > my_first) ? (p_end - my_first + 1) / 2 : 0;
+  uint8_t* my_ring = s_ring + warp * SL::kWarpBytes;
+  uint64_t* my_full = &sh.full[warp][0];
+  const int zoff = pg.num_kv_heads * pg.tokens_per_block * 2;
+  long long kp_l = 0, vp_l = 0;  // lane l: page pointers of this warp's slice (batch * 32 + l)
+  auto load_ptr_batch = [&](int j0) { slice_ptrs(kptrs, vptrs, my_first + 2 * (j0 + lane), p_end, kp_l, vp_l); };
+  auto issue = [&](int j, int slot) {
+    issue_slice<BITS>(lane, kp_l, vp_l, j, my_ring + slot * SL::kBytes, &my_full[slot], hk, hslice, pg.code_bytes, zoff);
+  };
+  load_ptr_batch(0);
+  pdl_wait();
+  for (int j = 0; j < R && j < n_my; ++j) issue(j, j);  // the cache stream starts before the staging
+  stage();
+  __syncthreads();
+
+  // ---- Q as the MMA "B" operand per n8 tile (q_operand).  The B fragments live in shared memory (qb[t][w][lane] = the two k-steps of
+  //      word w), not in registers: with NT = 2 the O^T accumulators alone take 64 registers, and 32 more for Q would spill ----
+  float sumq[NT][2], biasq[NT][2];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+    uint32_t qb0[8], qb1[8];
+    q_operand<BITS>(sh.q + (8 * t + g) * kD + 32 * q4, q4, qb0, qb1, sumq[t], biasq[t]);
+    if (warp == 0) {
+#pragma unroll
+      for (int w = 0; w < 4; ++w) sh.qb[t][w][lane] = make_uint4(qb0[2 * w], qb1[2 * w], qb0[2 * w + 1], qb1[2 * w + 1]);
+    }
+  }
+  __syncthreads();
+  auto qb = [&](int t, int ks, uint32_t& b0, uint32_t& b1) {
+    const uint4 qq = sh.qb[t][ks >> 1][lane];
+    b0 = (ks & 1) ? qq.z : qq.x;
+    b1 = (ks & 1) ? qq.w : qq.y;
+  };
+
+  float o[NT][8][4];
+  float m[NT][2], l[NT][2], cr[NT][2], spa[NT][4];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) o[t][i][0] = o[t][i][1] = o[t][i][2] = o[t][i][3] = 0.f;
+    m[t][0] = m[t][1] = -CUDART_INF_F;
+    l[t][0] = l[t][1] = cr[t][0] = cr[t][1] = 0.f;
+    spa[t][0] = spa[t][1] = spa[t][2] = spa[t][3] = 0.f;
+  }
+
+  const int tokA = (g & 1) * 4 + (g >> 1);
+  constexpr int kRow = kD * BITS / 8;
+  const int hbase = hslice * kSliceTokens;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < n_my; ++j) {
+    const int pidx = my_first + 2 * j;
+    mbar_wait(&my_full[s], ph);
+    const uint8_t* st = my_ring + s * SL::kBytes;
+    const int t0 = pidx * kPageTokens + hbase;
+    if (!unread(t0)) {
+      slice_meta<BITS>(st, lane, unread(t0 + lane), sm_scale, sh.meta[warp][0], sh.meta[warp][1]);
+      __syncwarp();
+      // ---- S^T (2 x 16 tokens x C columns) ----
+      float sc[2][NT][4];
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+#pragma unroll
+        for (int t = 0; t < NT; ++t) sc[c][t][0] = sc[c][t][1] = sc[c][t][2] = sc[c][t][3] = 0.f;
+        qk_chunk<BITS, NT>(st + SL::kOffK + (c * kChunk + tokA) * kRow, q4, sc[c], qb);
+      }
+      float tl[2][NT][4], vs[2][2], vc[2][2];
+#pragma unroll
+      for (int c = 0; c < 2; ++c) chunk_logits<NT>(sh.meta[warp][0], sh.meta[warp][1], c, tokA, sc[c], biasq, sumq, tl[c], vs[c], vc[c]);
+      tail(t0, tokA, tl);
+      uint32_t bp[2][NT][2];
+#pragma unroll
+      for (int t = 0; t < NT; ++t) softmax_tile<NT, EMPTY>(t, tl, vs, vc, m[t], l[t], cr[t], spa[t], o[t], bp);
+      // ---- O^T += V^T P'^T ----
+#pragma unroll
+      for (int c = 0; c < 2; ++c) pv_chunk<BITS, NT>(st + SL::kOffV + (c * kChunk + q4) * kRow, g, o, bp[c]);
+    }
+    __syncwarp();
+    if (j + R < n_my) {
+      if (((j + R) & 31) == 0) load_ptr_batch(j + R);
+      issue(j + R, s);
+    }
+    if (++s == R) { s = 0; ph ^= 1; }
+  }
+
+  // ---- per-warp partials -> the warp's own (drained) ring ----
+#pragma unroll
+  for (int t = 0; t < NT; ++t) reduce_tile_sums(l[t], cr[t]);
+  if (g == 0) {
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      sh.m[warp][8 * t + 2 * q4] = m[t][0]; sh.m[warp][8 * t + 2 * q4 + 1] = m[t][1];
+      sh.l[warp][8 * t + 2 * q4] = l[t][0]; sh.l[warp][8 * t + 2 * q4 + 1] = l[t][1];
+    }
+  }
+  __syncwarp();
+#pragma unroll
+  for (int t = 0; t < NT; ++t) store_partial<BITS>(reinterpret_cast<float*>(my_ring) + (8 * t + 2 * q4) * kOStride + g, o[t], spa[t], cr[t]);
+}
+
+// =========================================================================================================================================
 // Host: the launch plan of the paged-attention kernels
 // =========================================================================================================================================
 
@@ -460,6 +611,9 @@ inline int context_splits(long long ctas, long long slots, int ctx) {
   if (2 * ctas > slots || ctx <= 512) return 1;
   return static_cast<int>(std::min<long long>(std::min<long long>((slots + ctas - 1) / ctas, (ctx + 255) / 256), 32));
 }
+
+// Dynamic shared memory of a paged-attention CTA: the kWarps rings
+inline int ring_bytes(int bits) { return kWarps * (bits == 4 ? StageLayout<4>::kWarpBytes : StageLayout<8>::kWarpBytes); }
 
 // Resident CTAs per SM of a paged-attention kernel with `smem` bytes of dynamic shared memory (its rings), asked once per device (this raises
 // the kernel's dynamic shared memory limit: the KV8 rings exceed the default 48 KB; a failure is reported as `what`); 1 if the occupancy
@@ -478,6 +632,33 @@ int resident_ctas(int smem, const char* what) {
     r = n;
   }
   return r;
+}
+
+// One instantiation of a column-tile kernel, as its plan (resident_ctas) and its launch use it
+template <class Kernel>
+struct ColumnKernel {
+  Kernel fn;
+  int (*resident)(int smem, const char* what);  // resident_ctas<fn>
+};
+template <auto KERNEL>
+constexpr ColumnKernel<decltype(KERNEL)> column_kernel() { return {KERNEL, resident_ctas<KERNEL>}; }
+
+// The launch shape of a column-tile kernel over `cols` columns per (KV head, sequence or group), `rows` such pairs and `ctx` cached tokens:
+// C = 8 columns when they fit one n8 tile, else 16, in ceil(cols / C) column parts; context_splits over per_sm(ntile) resident CTAs per SM
+struct ColumnPlan {
+  int ntile;       // n8 tiles per CTA (C = 8 ntile columns)
+  int cparts;      // column parts per KV head
+  long long ctas;  // CTAs per context split
+  int nsplit;      // context splits
+};
+template <class PerSm>
+ColumnPlan plan_columns(int cols, long long rows, int ctx, const PerSm& per_sm) {
+  ColumnPlan c{};
+  c.ntile = cols <= 8 ? 1 : 2;
+  c.cparts = (cols + 8 * c.ntile - 1) / (8 * c.ntile);
+  c.ctas = rows * c.cparts;
+  c.nsplit = context_splits(c.ctas, static_cast<long long>(num_sms()) * per_sm(c.ntile), ctx);
+  return c;
 }
 
 }  // namespace
