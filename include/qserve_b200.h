@@ -553,6 +553,44 @@ typedef struct qs_inflight_args {
 } qs_inflight_args;
 QS_API int qs_inflight_schedule(const qs_inflight_args* args, void* stream);
 
+/* In-flight batching over a shared KV page pool (DESIGN.md 3.12): the rows draw their 64-token pages from one pool of `pages` pages per
+ * layer and K / V instead of owning them.  Page state, in device memory: the free stack (free[0 .. top) are free, free[top - 1] is popped
+ * first), per row its page list pages[b, 0 .. count[b]) and its prefill target (the tokens it must cache before it decodes), and counters.
+ *
+ * qs_inflight_schedule_pool takes the arguments of qs_inflight_schedule and this pool, and follows its rules with these changes and
+ * additions, in this order (tests/kv_pool_oracle.py restates them):
+ *   1. Retire as qs_inflight_schedule; a retired row's pages go back onto the free stack, in row order and then page order; count = 0.
+ *   2. Admit as qs_inflight_schedule, without a page check, and target = len.
+ *   3. Decode growth, over the DECODE rows in admission order: a row whose context seq_len needs page ceil(seq_len / 64) - 1 and does not own
+ *      it (count <= that index) pops one page.  If the stack is empty, it first preempts the page-holding row with the highest admission
+ *      number (itself included): that row's pages go back onto the stack in page order, count = 0, and it becomes PREFILL with done = 0 and
+ *      target = seq_len (its history holds the prompt and the generated tokens), keeping its admission number, request, prompt_lens, budget and
+ *      sampling state; it is idle in this step.  A PREFILL row that holds pages can be a victim too.  A row that preempted itself pops nothing.
+ *   4. Starts, over the PREFILL rows that hold no pages, in admission order: a row starts when top >= ceil(target / 64) and then pops all
+ *      those pages at once; the first row that cannot start blocks every later one (strict first-come-first-served).
+ *   5. Plan and tail masks as qs_inflight_schedule over the started PREFILL rows (rows that hold no pages take no tokens and stay idle), with
+ *      c_b = min(target - done, chunk_budget - used), completion at done + c_b == target and start_pos = target.  Retirement still hands out
+ *      history[prompt_lens .. seq_lens), so outputs and the budget are those of a row that was never preempted.
+ *   6. Table writes: for every row, the entries [keep, count) of its table row in all `layers` layers, K and V, become
+ *      layer_base[l][kv] + page * page_bytes, where keep is the row's count before the call, or 0 if it lost its pages in this call.  Entries
+ *      past a row's count are unspecified and never read.
+ * counters int32 [4]: top, peak pages in use (the largest pages - top after any pop), preemptions, starts.  The tables are written by this
+ * launch, which must precede the step's attention kernels by a launch without PDL (they read the tables before their dependency wait).
+ * Limits: pages >= ceil((prompt_cols + max_tokens + 1) / 64), blocks >= that too, so the oldest row can always get its pages (a row never
+ * preempts an older one).                                                                                                                */
+typedef struct qs_kv_pool_args {
+  int32_t* free_pages;       /* [pages] the free stack */
+  int32_t* counters;         /* [4] */
+  int32_t* row_pages;        /* [batch, blocks] */
+  int32_t* row_count;        /* [batch] */
+  int32_t* target;           /* [batch] */
+  int64_t* tables;           /* [layers, batch, 2, blocks] page addresses */
+  const int64_t* layer_base; /* [layers, 2] address of page 0 of each layer's K and V pool */
+  long long page_bytes;
+  int pages, blocks, layers;
+} qs_kv_pool_args;
+QS_API int qs_inflight_schedule_pool(const qs_inflight_args* args, const qs_kv_pool_args* pool, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

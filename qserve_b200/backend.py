@@ -919,13 +919,49 @@ class _InflightArgs(ctypes.Structure):
         [(n, ctypes.c_int) for n in ("batch", "queue", "prompt_cols", "history_len", "max_tokens", "chunk", "chunk_budget")]
 
 
+class KvPool(NamedTuple):
+    """The shared KV page pool of the in-flight step (qs_inflight_schedule_pool): P pages per layer and K / V, drawn by B rows."""
+    free: torch.Tensor        # int32 [P]: the free stack, free[:top] free, free[top - 1] popped first
+    counters: torch.Tensor    # int32 [4]: top, peak pages in use, preemptions, starts
+    pages: torch.Tensor       # int32 [B, blocks]: every row's page list, valid up to count
+    count: torch.Tensor       # int32 [B]: pages a row holds
+    target: torch.Tensor      # int32 [B]: tokens a PREFILL row caches before it decodes
+    tables: torch.Tensor      # int64 [L, B, 2, blocks]: the page tables the schedule writes
+    layer_base: torch.Tensor  # int64 [L, 2]: address of page 0 of every layer's K and V pool
+    page_bytes: int
+
+
+def kv_pool_buffers(tables: torch.Tensor, layer_base: torch.Tensor, pages: int, page_bytes: int) -> KvPool:
+    """A fresh KvPool over the page tables `tables` int64 [L, B, 2, blocks] and pools at `layer_base` int64 [L, 2]: every page free (pages
+    0, 1, ... are popped first), no row holding any, counters 0 (torch.full / torch.zeros: no random draws)."""
+    L, B, _, nb = _tensor(tables, "tables", torch.int64, (None, None, 2, None)).shape
+    dev = tables.device
+    _tensor(layer_base, "layer_base", torch.int64, (L, 2), dev)
+    P = int(pages)
+    _require(P >= 1 and int(page_bytes) >= 1, f"pages={pages} and page_bytes={page_bytes} must be >= 1")
+    counters = torch.zeros(4, dtype=torch.int32, device=dev)
+    counters[0] = P
+    return KvPool(torch.arange(P - 1, -1, -1, dtype=torch.int32, device=dev), counters, torch.full((B, nb), -1, dtype=torch.int32, device=dev),
+                  torch.zeros(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev), tables, layer_base, int(page_bytes))
+
+
+class _KvPoolArgs(ctypes.Structure):
+    """qs_kv_pool_args of include/qserve_b200.h, field for field."""
+    _fields_ = [(n, ctypes.c_void_p) for n in ("free_pages", "counters", "row_pages", "row_count", "target", "tables", "layer_base")] + \
+        [("page_bytes", ctypes.c_longlong)] + [(n, ctypes.c_int) for n in ("pages", "blocks", "layers")]
+
+
 def inflight_schedule(queue: InflightQueue, rows: InflightRows, history, prompt_lens, seq_lens, temperature, top_k, top_p, repetition, presence,
                       frequency, eos, stop, budget, offsets, finished, start_pos, tokens_in, logprob: Optional[torch.Tensor], plan: InflightPlan,
-                      out: InflightOutputs, chunk_budget: int) -> None:
+                      out: InflightOutputs, chunk_budget: int, pool: Optional[KvPool] = None) -> None:
     """One in-flight schedule, in place and without host synchronisation (include/qserve_b200.h qs_inflight_schedule; restated in
     tests/inflight_oracle.py): retire the DECODE rows with finished = 1 into `out`, admit queued requests into FREE rows first-come-first-served
     (chunk_budget > 0 only), plan the chunk segment (chunk_budget = C or 0) and the decode segment into `plan`, and set the tail masks.  The
-    per-row runner vectors are [B] (history int64 [B, H], stop int64 [B, 8], logprob fp32 [B, H] or None together with out.logprob)."""
+    per-row runner vectors are [B] (history int64 [B, H], stop int64 [B, 8], logprob fp32 [B, H] or None together with out.logprob).
+
+    pool (kv_pool_buffers): qs_inflight_schedule_pool instead (restated in tests/kv_pool_oracle.py): the rows draw their pages from the pool,
+    with decode growth, preemption by recompute and first-come-first-served starts, and the schedule writes the new entries of pool.tables.
+    The pool needs at least ceil((prompt_cols + max_tokens + 1) / 64) pages, and the tables as many blocks."""
     B = _tensor(rows.phase, "phase", torch.int32, (None,)).size(0)
     dev = rows.phase.device
     _require(1 <= B <= MAX_INFLIGHT_ROWS, f"batch={B}: 1 .. {MAX_INFLIGHT_ROWS} rows")
@@ -970,7 +1006,24 @@ def inflight_schedule(queue: InflightQueue, rows: InflightRows, history, prompt_
                 out_tokens=out.tokens, out_len=out.length, out_reason=out.reason, out_logprob=out.logprob, out_ids=out.ids)
     a = _InflightArgs(**{k: _ptr(v) for k, v in ptrs.items()}, batch=B, queue=Q, prompt_cols=P, history_len=H, max_tokens=T, chunk=C,
                       chunk_budget=int(chunk_budget))
-    _call(rows.phase, lib.qs_inflight_schedule, ctypes.addressof(a))
+    if pool is None:
+        _call(rows.phase, lib.qs_inflight_schedule, ctypes.addressof(a))
+        return
+    L, _, _, nb = _tensor(pool.tables, "pool.tables", torch.int64, (None, B, 2, None), dev).shape
+    n_pages = _tensor(pool.free, "pool.free", torch.int32, (None,), dev).size(0)
+    need = -(-(P + T + 1) // 64)
+    _require(n_pages >= need, f"a pool of {n_pages} pages cannot hold one request of {P} prompt and {T} generated tokens ({need} pages)")
+    _require(nb >= need, f"page tables of {nb} blocks cannot hold one request of {P} prompt and {T} generated tokens ({need} blocks)")
+    _require(int(pool.page_bytes) >= 1, f"page_bytes={pool.page_bytes}")
+    _tensor(pool.counters, "pool.counters", torch.int32, (4,), dev)
+    _tensor(pool.pages, "pool.pages", torch.int32, (B, nb), dev)
+    _tensor(pool.count, "pool.count", torch.int32, (B,), dev)
+    _tensor(pool.target, "pool.target", torch.int32, (B,), dev)
+    _tensor(pool.layer_base, "pool.layer_base", torch.int64, (L, 2), dev)
+    pa = _KvPoolArgs(free_pages=pool.free.data_ptr(), counters=pool.counters.data_ptr(), row_pages=pool.pages.data_ptr(), row_count=pool.count.data_ptr(),
+                     target=pool.target.data_ptr(), tables=pool.tables.data_ptr(), layer_base=pool.layer_base.data_ptr(), page_bytes=int(pool.page_bytes),
+                     pages=n_pages, blocks=nb, layers=L)
+    _call(rows.phase, lib.qs_inflight_schedule_pool, ctypes.addressof(a), ctypes.addressof(pa))
 
 
 def _row_vec(v, n: int, dev, dt, name: str, ok, what: str) -> torch.Tensor:

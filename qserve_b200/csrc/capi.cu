@@ -574,4 +574,9 @@ int qs_inflight_schedule(const qs_inflight_args* args, void* stream) {
   return inflight_schedule(*args, stream);
 }
 
+int qs_inflight_schedule_pool(const qs_inflight_args* args, const qs_kv_pool_args* pool, void* stream) {
+  QS_REQUIRE(args != nullptr && pool != nullptr, "inflight_schedule_pool: null arguments");
+  return inflight_schedule_pool(*args, *pool, stream);
+}
+
 }  // extern "C"

@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 struct qs_inflight_args;  // include/qserve_b200.h
+struct qs_kv_pool_args;
 
 namespace qs {
 
@@ -364,5 +365,7 @@ int spec_commit_stops(const SpecCommitArgs& a, const long long* stop_ids, int nu
 
 // the in-flight step's schedule (inflight.cu): the arguments of qs_inflight_schedule
 int inflight_schedule(const qs_inflight_args& a, void* stream);
+// ... and of qs_inflight_schedule_pool
+int inflight_schedule_pool(const qs_inflight_args& a, const qs_kv_pool_args& p, void* stream);
 
 }  // namespace qs

@@ -168,6 +168,15 @@ class InflightPoll(NamedTuple):
     pending_tokens: int
 
 
+class KvPoolStats(NamedTuple):
+    """DecodeRunner.pool_stats: the shared KV page pool's free pages now, and since construction the most pages in use at once, the
+    preemptions and the starts (a PREFILL row taking the pages of its target)."""
+    free_pages: int
+    peak_pages: int
+    preemptions: int
+    starts: int
+
+
 _PROMPT_LOGITS_BYTES = 64 << 20  # prompt_logprobs: fp16 logits of at most this many bytes exist at once
 
 
@@ -176,7 +185,7 @@ class DecodeRunner:
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
                  verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False, prompt_tokens: int = 0, shared_prefix: bool = False,
-                 beam_width: int = 0, inflight: int = 0):
+                 beam_width: int = 0, inflight: int = 0, kv_pool_pages: int = 0):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
         ctx + verify_len tokens and the activation buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers
         and its random draws exactly as they are without it.
@@ -218,7 +227,15 @@ class DecodeRunner:
         requests, rows that take queued prompts as they free up, and a step that carries up to C prompt tokens of the prefilling rows in the
         same forward pass as the decode tokens of the others (DESIGN.md 3.12).  The activation buffers hold batch + C rows and the page tables
         cover max(ctx + T + 1, ctx - 1 + C) tokens; every row keeps its own pages.  All its state is made with torch.full / torch.zeros after
-        every random draw, so inflight = 0 leaves the weights, pages and every other step as they are."""
+        every random draw, so inflight = 0 leaves the weights, pages and every other step as they are.
+
+        kv_pool_pages = P >= 1 (needs inflight) makes the in-flight rows share one pool of P pages per layer, K and V, instead of owning
+        batch * table_blocks of them (DESIGN.md 3.12): the schedule grants pages inside the captured step (a decoding row takes a page when its
+        context reaches one, a prefilling row the pages of its whole target when it starts) and, when the pool runs dry, preempts the youngest
+        page-holding row, which recomputes its prompt and generated tokens as a prefill.  P >= ceil((ctx + T + 1) / 64), so the oldest request
+        always fits.  The per-row random pages are not made; the pools are zero-filled after every random draw, so the weights are those of
+        kv_pool_pages = 0.  The tables cover max(ctx + T + 1, ctx + T - 1 + C) tokens (a recomputed row's prefix reaches ctx + T - 1).  Pool mode
+        is fixed at construction: prefill, fork, reset_generation and load_shard_of refuse it."""
         self.cfg = cfg = MODELS[model]
         self.max_pos = min(8192, cfg.max_pos)  # the positions the attention kernels support
         beam_width, inflight, ops = int(beam_width), int(inflight), ops or DEFAULT_OPS
@@ -244,10 +261,14 @@ class DecodeRunner:
                 (inflight and (not generate or verify_len or beam_width or shared_prefix),
                  "in-flight batching needs generate=True and is not combined with verify_len, beam_width or shared_prefix"),
                 (inflight and (prompt_tokens < 1 or inflight < 1), "in-flight batching needs prompt_tokens >= 1 and a queue of at least one request"),
-                (inflight and not 1 <= batch <= _ext.MAX_INFLIGHT_ROWS, f"in-flight batching runs 1 .. {_ext.MAX_INFLIGHT_ROWS} rows")):
+                (inflight and not 1 <= batch <= _ext.MAX_INFLIGHT_ROWS, f"in-flight batching runs 1 .. {_ext.MAX_INFLIGHT_ROWS} rows"),
+                (kv_pool_pages and not inflight, "kv_pool_pages needs in-flight batching (inflight >= 1)"),
+                (kv_pool_pages and not kv_pool_pages >= (ctx + T + 1 + 63) // 64,
+                 f"kv_pool_pages={kv_pool_pages}: at least ceil((ctx + max_new_tokens + 1) / 64) = {(ctx + T + 1 + 63) // 64} pages")):
             if bad:
                 raise RuntimeError(why)
         self.beam_width, self.inflight, self.shared_prefix, self.prompt_tokens = beam_width, inflight, shared_prefix, prompt_tokens
+        self.kv_pool_pages = kv_pool_pages = int(kv_pool_pages)
         self.generate, self.verify_len, self.ops, self.tp_exact = generate, verify_len, ops, tp_exact
         self.no_comm = no_comm  # debugging: run one rank's shard of a tensor-parallel model without the collectives (sanitizer / profiler runs)
         # tensor parallel, fused path: the all-reduce of the row-parallel GEMM outputs is folded into the following add+norm+quant kernel
@@ -296,7 +317,7 @@ class DecodeRunner:
         n_pages = batch * self.blocks_per_seq
         self.kpools, self.vpools, tables = [], [], []
         blk = torch.arange(n_pages, device=dev, dtype=torch.int64).view(batch, self.blocks_per_seq)
-        for _ in range(self.L):
+        for _ in range(0 if kv_pool_pages else self.L):  # pool mode: no per-row pages (and no draws after the weights)
             pools = []
             for _kv in range(2):
                 pool = torch.randint(0, 256, (n_pages, self.page_bytes), dtype=torch.uint8, device=dev, generator=gen)
@@ -310,7 +331,15 @@ class DecodeRunner:
             tables.append(torch.stack([pools[0].data_ptr() + blk * self.page_bytes, pools[1].data_ptr() + blk * self.page_bytes], dim=1))
         self.table_blocks = self.blocks_per_seq
         self.kpools_gen, self.vpools_gen = [], []
-        if generate or beam_width:  # pages for the generated tokens: zero-filled (no generator draws), after the pages above in every row's table
+        if kv_pool_pages:  # one zero-filled pool per layer, K and V; every table entry starts at the layer's page 0 (the schedule writes the rest)
+            self.table_blocks = (max(ctx + max_new_tokens + 1, ctx + max_new_tokens - 1 + prompt_tokens) + 63) // 64
+            for _ in range(self.L):
+                kp = torch.zeros((kv_pool_pages, self.page_bytes), dtype=torch.uint8, device=dev)
+                vp = torch.zeros_like(kp)
+                self.kpools.append(kp); self.vpools.append(vp)
+                tables.append(torch.tensor([kp.data_ptr(), vp.data_ptr()], dtype=torch.int64, device=dev).view(1, 2, 1)
+                              .expand(batch, 2, self.table_blocks))
+        elif generate or beam_width:  # pages for the generated tokens: zero-filled (no generator draws), after the pages above in every row's table
             # (in-flight batching: also the host bound ctx - 1 + C of the chunk segment's prompt attention)
             self.table_blocks = (max(ctx + max_new_tokens + max(1, verify_len), ctx - 1 + prompt_tokens if inflight else 0) + 63) // 64
             extra = self.table_blocks - self.blocks_per_seq
@@ -328,6 +357,8 @@ class DecodeRunner:
         # host bounds of the attention launches: in generation the contexts grow up to ctx + 1 + max_new_tokens
         self.max_seq_len = ctx + 1 + (max_new_tokens if generate or beam_width else 0)
         self.max_prefix_len = ctx + (max_new_tokens if generate or beam_width else 0)
+        # the prompt chunks' prefix bound: a row recomputed after a preemption caches up to ctx + T - 1 tokens
+        self.chunk_prefix_len = ctx + max_new_tokens - 1 if kv_pool_pages else ctx - 1
 
         # ---- persistent ActivationBuffer (input_metadata.py:71-109; aliasing kept) for the rows of the widest step --------------------
         # (H is in the max for tensor parallelism: at TP = 8 a 72B model's sharded qkv / gate_up rows are narrower than the full hidden row of out_buf)
@@ -766,6 +797,7 @@ class DecodeRunner:
         cached).  Sets the history and its lengths, the positions of both step kinds and tokens_in, and clears g_finished; g_budget, g_eos
         and g_stop stay as the caller set them."""
         assert self.generate, "construct the runner with generate=True"
+        self._refuse_pool("reset_generation")
         B, C = self.batch, self.ctx + 1
         assert tuple(prompt.shape) == (B, C) and prompt.dtype == torch.int64, f"prompt must be int64 [{B}, {C}]"
         self.s_history.fill_(-1)
@@ -877,6 +909,7 @@ class DecodeRunner:
         g_logprob / g_top_view(n); generate_forward continues from there."""
         assert self.prompt_tokens, "construct the runner with prompt_tokens > 0"
         assert self.max_new_tokens or not (penalties or logprobs), "construct the runner with max_new_tokens > 0 for penalties / logprobs"
+        self._refuse_pool("prefill")
         B, cfg, dev = self.batch, self.cfg, self.dev
         if not (lens.dtype == torch.int32 and tuple(lens.shape) == (B,)):
             raise RuntimeError(f"lens must be int32 [{B}], got {lens.dtype} {tuple(lens.shape)}")
@@ -999,6 +1032,7 @@ class DecodeRunner:
         gets the parent's history, s_prompt_lens, s_seq_lens, context_lens, g_start / v_start, tokens_in, g_budget, g_eos, g_stop, g_finished,
         penalty parameters and history-aligned log-probabilities.  s_offsets and the sampling parameters stay the child's own, so sampled children diverge.  Eager; the table
         entries are written with torch ops (the attention kernels read the tables before their dependency wait)."""
+        self._refuse_pool("fork")
         children = list(child_rows) if not isinstance(child_rows, int) else [child_rows]
         parents = [parent_rows] * len(children) if isinstance(parent_rows, int) else list(parent_rows)
         parents, children = _ext.fork_pairs(parents, children, self.batch)
@@ -1136,6 +1170,10 @@ class DecodeRunner:
         B, C, T = self.batch, self.prompt_tokens, self.max_new_tokens
         self._alloc_generate_logprobs(0)  # g_logprob: the schedule hands the chosen tokens' log-probabilities to the outputs
         self.i_queue, self.i_rows, self.i_plan, self.i_out = _ext.inflight_buffers(B, self.inflight, C, self.ctx, T, self.dev)
+        self.i_pool = None
+        if self.kv_pool_pages:
+            base = torch.tensor([[k.data_ptr(), v.data_ptr()] for k, v in zip(self.kpools, self.vpools)], dtype=torch.int64, device=self.dev)
+            self.i_pool = _ext.kv_pool_buffers(self.block_tables, base, self.kv_pool_pages, self.page_bytes)
         self._i_submitted = 0       # requests submitted (the host's tail)
         self._i_lens: dict = {}     # prompt length of every request not yet polled
         self._i_unpolled: set = set()
@@ -1206,14 +1244,15 @@ class DecodeRunner:
     def _inflight_schedule(self, chunk_budget: int) -> None:
         _ext.inflight_schedule(self.i_queue, self.i_rows, self.s_history, self.s_prompt_lens, self.s_seq_lens, self.s_temperature, self.s_top_k,
                                self.s_top_p, self.s_repetition, self.s_presence, self.s_frequency, self.g_eos, self.g_stop, self.g_budget,
-                               self.s_offsets, self.g_finished, self.g_start, self.tokens_in, self.g_logprob, self.i_plan, self.i_out, chunk_budget)
+                               self.s_offsets, self.g_finished, self.g_start, self.tokens_in, self.g_logprob, self.i_plan, self.i_out, chunk_budget,
+                               pool=self.i_pool)
 
     def inflight_forward(self, mixed: bool = True, sampled: bool = False, penalties: bool = False, logprobs: int = 0) -> None:
         """One in-flight step; no host synchronisation.  inflight_schedule (chunk budget C, or 0 when mixed=False: nothing is admitted and no
         prompt token is carried), then the layers over M = B + C rows (B without mixed): the B decode rows, idle ones at context length 0,
         and the chunk segment, whose padding slots are neither appended nor attended.  Per layer: single_query_attention_quant over the decode
         rows; apply_bias_rope_update_kv_cache_at + prefix_prefill_attention + invoke_quant[_fuse_sum] over the chunk segment (host bounds
-        max_seqlen = C, max_prefix_len = ctx - 1).  The B logit rows (the decode rows, and for a row whose prompt completes the logit of its
+        max_seqlen = C, max_prefix_len = ctx - 1, or ctx + T - 1 with kv_pool_pages).  The B logit rows (the decode rows, and for a row whose prompt completes the logit of its
         last prompt token) go through lm_head at M = B, then the sampler of generate_forward(1): apply_penalties if penalties, argmax_rows or
         sample_rows if sampled, logprobs_accepted if logprobs, spec_commit with the stop ids.  A completing row's first token is committed in
         the same step.
@@ -1229,7 +1268,7 @@ class DecodeRunner:
         M = B + C if mixed else B
         self._inflight_schedule(C if mixed else 0)
         plan = self.i_plan
-        seg = _Segment(plan.chunk_lens, plan.padding_offset, plan.prefix_lens, plan.cu_seqlens, C, self.ctx - 1)
+        seg = _Segment(plan.chunk_lens, plan.padding_offset, plan.prefix_lens, plan.cu_seqlens, C, self.chunk_prefix_len)
 
         def attention(li, r):
             self._attention_quant(li, r, plan.context_lens, B)
@@ -1262,7 +1301,9 @@ class DecodeRunner:
         if flush:
             self._inflight_schedule(0)
         q, rows, out = self.i_queue, self.i_rows, self.i_out
-        snap = [t.to("cpu", non_blocking=True) for t in (q.counters, rows.phase, rows.done, self.s_prompt_lens, out.ids, out.length, out.reason,
+        # a PREFILL row caches its prompt, or with a pool its target (a preempted row recomputes its generated tokens too)
+        target = self.s_prompt_lens if self.i_pool is None else self.i_pool.target
+        snap = [t.to("cpu", non_blocking=True) for t in (q.counters, rows.phase, rows.done, target, out.ids, out.length, out.reason,
                                                          out.tokens, out.logprob)]
         torch.cuda.current_stream(self.dev).synchronize()
         ctr, phase, done, plen, ids, length, reason, toks, lps = snap
@@ -1281,6 +1322,17 @@ class DecodeRunner:
         prefilling = int(((plen - done) * (phase == _ext.INFLIGHT_PREFILL)).sum())
         return InflightPoll(finished, queued + prefilling)
 
+    def pool_stats(self) -> KvPoolStats:
+        """The shared KV page pool's counters (kv_pool_pages > 0).  One host synchronisation."""
+        if self.i_pool is None:
+            raise RuntimeError("pool_stats needs kv_pool_pages > 0")
+        top, peak, pre, starts = self.i_pool.counters.tolist()
+        return KvPoolStats(top, peak, pre, starts)
+
+    def _refuse_pool(self, what: str) -> None:
+        if self.kv_pool_pages:
+            raise RuntimeError(f"{what} is not available with kv_pool_pages: the in-flight schedule owns the page tables")
+
     # ---------------------------------------------------------------------------------------------------------
     def load_shard_of(self, full: "DecodeRunner") -> None:
         """Make this tensor-parallel runner (rank tp_rank of tp_size) the shard of `full` (a tp_size = 1 runner of the same model /
@@ -1288,6 +1340,7 @@ class DecodeRunner:
         gate | up parts are sliced separately; row parallel: K slices of every band), KV pages by kv head, everything else replicated."""
         from qserve_b200 import tp
 
+        self._refuse_pool("load_shard_of")
         r, n, dev = self.tp_rank, self.tp_size, self.dev
         assert full.tp_size == 1 and full.cfg == self.cfg and full.precision == self.precision and full.batch == self.batch and full.ctx == self.ctx
         assert self.cfg.kv_heads % n == 0, "KV-head replication (tp_size > kv_heads) is not needed by the benchmark models"
