@@ -1,5 +1,7 @@
 """GPU parity: wgmma W4A8 / W8A8 GEMMs vs the CPU oracle.  INT32 accumulators bit-exact, FP16 outputs bit-exact
-(the epilogue is IEEE fp32 in the reference's source order; tolerance 0 ulp) -- through the drop-in Python API."""
+(the epilogue is IEEE fp32 in the reference's source order; tolerance 0 ulp) -- through the drop-in Python API.  The parity tests run
+each problem on both instantiations of the kernel (_run_both): with the INT32 accumulator dump, and without it, as the decode runner
+launches it."""
 import json
 import os
 
@@ -18,6 +20,22 @@ def _acts(rng, M, K):
     x = rng.standard_normal((M, K)).astype(np.float16)
     aq, sa, asum = ops.quant_per_token(x)
     return aq, sa, asum
+
+
+def _run_both(dev, call, M, N):
+    """call(out, acc) with acc an INT32 [M, N] tensor and again with acc=None -> (acc, fp16 out with the dump, fp16 out without), numpy.
+    Both outputs are views [:M] of NaN-filled buffers whose rows past M must stay NaN."""
+    outs = []
+    for dump in (True, False):
+        out = torch.full((M + 8, N), float("nan"), dtype=torch.half, device=dev)
+        acc = torch.zeros((M, N), dtype=torch.int32, device=dev) if dump else None
+        call(out[:M], acc)
+        torch.cuda.synchronize()
+        assert bool(torch.isnan(out[M:]).all()), dump
+        outs.append(np_of(out[:M]))
+        if dump:
+            acc_g = np_of(acc)
+    return acc_g, outs[0], outs[1]
 
 
 def _report(name, acc_g, acc_o, out_g, out_o):
@@ -50,13 +68,12 @@ def test_w4a8_per_channel(dev, M, N, K):
     q, qw, s1, s1z = w4a8.synth_per_channel(rng, N, K)
     aq, sa, asum = _acts(rng, M, K)
     out_o, acc_o = w4a8.gemm_w4a8_per_chn(aq, qw, s1, sa, s1z, asum, return_acc=True)
-    out = torch.full((M, N), float("nan"), dtype=torch.half, device=dev)
-    acc = torch.zeros((M, N), dtype=torch.int32, device=dev)
-    op.gemm_forward_cuda(to_dev(aq, dev), to_dev(qw, dev), to_dev(s1, dev), to_dev(sa, dev), to_dev(s1z, dev), to_dev(asum, dev), out, _acc_out=acc)
-    torch.cuda.synchronize()
-    info = _report(f"chn_{M}x{N}x{K}", np_of(acc), acc_o, np_of(out), out_o)
+    args = [to_dev(a, dev) for a in (aq, qw, s1, sa, s1z, asum)]
+    acc, out, out_n = _run_both(dev, lambda out, acc: op.gemm_forward_cuda(*args, out, _acc_out=acc), M, N)
+    info = _report(f"chn_{M}x{N}x{K}", acc, acc_o, out, out_o)
     assert info["acc_mismatch"] == 0, info
-    assert np.array_equal(bits16(np_of(out)), bits16(out_o)), info
+    assert np.array_equal(bits16(out), bits16(out_o)), info
+    assert np.array_equal(bits16(out_n), bits16(out_o)), info
 
 
 @pytest.mark.parametrize("M,N,K", SHAPES)
@@ -66,13 +83,12 @@ def test_w4a8_per_group(dev, M, N, K):
     q, qw, s1, s2s, s2z = w4a8.synth_per_group(rng, N, K)
     aq, sa, _ = _acts(rng, M, K)
     out_o, acc_o = w4a8.gemm_w4a8_per_group(aq, qw, s2z, s2s, s1, sa, return_acc=True)
-    out = torch.full((M, N), float("nan"), dtype=torch.half, device=dev)
-    acc = torch.zeros((M, N), dtype=torch.int32, device=dev)
-    op.gemm_forward_cuda(to_dev(aq, dev), to_dev(qw, dev), to_dev(s2z, dev), to_dev(s2s, dev), to_dev(s1, dev), to_dev(sa, dev), out, _acc_out=acc)
-    torch.cuda.synchronize()
-    info = _report(f"grp_{M}x{N}x{K}", np_of(acc), acc_o, np_of(out), out_o)
+    args = [to_dev(a, dev) for a in (aq, qw, s2z, s2s, s1, sa)]
+    acc, out, out_n = _run_both(dev, lambda out, acc: op.gemm_forward_cuda(*args, out, _acc_out=acc), M, N)
+    info = _report(f"grp_{M}x{N}x{K}", acc, acc_o, out, out_o)
     assert info["acc_mismatch"] == 0, info
-    assert np.array_equal(bits16(np_of(out)), bits16(out_o)), info
+    assert np.array_equal(bits16(out), bits16(out_o)), info
+    assert np.array_equal(bits16(out_n), bits16(out_o)), info
 
 
 @pytest.mark.parametrize("M,N,K", SHAPES)
@@ -83,13 +99,12 @@ def test_w8a8(dev, M, N, K):
     sw = rng.uniform(0.001, 0.01, size=N).astype(np.float16)
     aq, sa, _ = _acts(rng, M, K)
     out_o, acc_o = w4a8.gemm_w8a8(aq, w, sw, sa, return_acc=True)
-    out = torch.full((M, N), float("nan"), dtype=torch.half, device=dev)
-    acc = torch.zeros((M, N), dtype=torch.int32, device=dev)
-    op.w8a8_gemm_forward_cuda(to_dev(aq, dev), to_dev(w, dev), to_dev(sw, dev), to_dev(sa, dev), out, _acc_out=acc)
-    torch.cuda.synchronize()
-    info = _report(f"w8_{M}x{N}x{K}", np_of(acc), acc_o, np_of(out), out_o)
+    args = [to_dev(a, dev) for a in (aq, w, sw, sa)]
+    acc, out, out_n = _run_both(dev, lambda out, acc: op.w8a8_gemm_forward_cuda(*args, out, _acc_out=acc), M, N)
+    info = _report(f"w8_{M}x{N}x{K}", acc, acc_o, out, out_o)
     assert info["acc_mismatch"] == 0, info
-    assert np.array_equal(bits16(np_of(out)), bits16(out_o)), info
+    assert np.array_equal(bits16(out), bits16(out_o)), info
+    assert np.array_equal(bits16(out_n), bits16(out_o)), info
 
 
 @pytest.mark.parametrize("split", [1, 2, 4, 8])
@@ -137,12 +152,11 @@ def test_llama3_8b_layer_shapes_decode_b64(dev):
         q, qw, s1, s1z = w4a8.synth_per_channel(rng, N, K)
         aq, sa, asum = _acts(rng, 64, K)
         out_o, acc_o = w4a8.gemm_w4a8_per_chn(aq, qw, s1, sa, s1z, asum, return_acc=True)
-        out = torch.empty((64, N), dtype=torch.half, device=dev)
-        acc = torch.zeros((64, N), dtype=torch.int32, device=dev)
-        op.gemm_forward_cuda(*[to_dev(a, dev) for a in (aq, qw, s1, sa, s1z, asum)], out, _acc_out=acc)
-        torch.cuda.synchronize()
-        assert np.array_equal(np_of(acc), acc_o), (K, N)
-        assert np.array_equal(bits16(np_of(out)), bits16(out_o)), (K, N)
+        args = [to_dev(a, dev) for a in (aq, qw, s1, sa, s1z, asum)]
+        acc, out, out_n = _run_both(dev, lambda out, acc: op.gemm_forward_cuda(*args, out, _acc_out=acc), 64, N)
+        assert np.array_equal(acc, acc_o), (K, N)
+        assert np.array_equal(bits16(out), bits16(out_o)), (K, N)
+        assert np.array_equal(bits16(out_n), bits16(out_o)), (K, N)
 
 
 CONFIG_SHAPES = [  # BASELINE.json configs 3-5 (SURVEY.md 8d): (mode, M, N, K)
@@ -157,27 +171,29 @@ def test_baseline_config_shapes_bit_exact(dev, mode, M, N, K):
     """The GEMM shapes of BASELINE configs 3, 4 and 5 (per-rank shards at TP=4): INT32 and FP16 bit-exact at full size."""
     rng = np.random.default_rng(N + K + M)
     aq, sa, asum = _acts(rng, M, K)
-    out = torch.empty((M, N), dtype=torch.half, device=dev)
-    acc = torch.zeros((M, N), dtype=torch.int32, device=dev)
     if mode == "chn":
         import qserve_backend.qgemm_w4a8_per_chn as op
         q, qw, s1, s1z = w4a8.synth_per_channel(rng, N, K)
         out_o, acc_o = w4a8.gemm_w4a8_per_chn(aq, qw, s1, sa, s1z, asum, return_acc=True)
-        op.gemm_forward_cuda(*[to_dev(a, dev) for a in (aq, qw, s1, sa, s1z, asum)], out, _acc_out=acc)
+        args = [to_dev(a, dev) for a in (aq, qw, s1, sa, s1z, asum)]
+        call = lambda out, acc: op.gemm_forward_cuda(*args, out, _acc_out=acc)  # noqa: E731
     elif mode == "grp":
         import qserve_backend.qgemm_w4a8_per_group as op
         q, qw, s1, s2s, s2z = w4a8.synth_per_group(rng, N, K)
         out_o, acc_o = w4a8.gemm_w4a8_per_group(aq, qw, s2z, s2s, s1, sa, return_acc=True)
-        op.gemm_forward_cuda(*[to_dev(a, dev) for a in (aq, qw, s2z, s2s, s1, sa)], out, _acc_out=acc)
+        args = [to_dev(a, dev) for a in (aq, qw, s2z, s2s, s1, sa)]
+        call = lambda out, acc: op.gemm_forward_cuda(*args, out, _acc_out=acc)  # noqa: E731
     else:
         import qserve_backend.qgemm_w8a8 as op
         w = rng.integers(-128, 128, size=(N, K), dtype=np.int8)
         sw = rng.uniform(0.001, 0.01, size=N).astype(np.float16)
         out_o, acc_o = w4a8.gemm_w8a8(aq, w, sw, sa, return_acc=True)
-        op.w8a8_gemm_forward_cuda(*[to_dev(a, dev) for a in (aq, w, sw, sa)], out, _acc_out=acc)
-    torch.cuda.synchronize()
-    assert np.array_equal(np_of(acc), acc_o)
-    assert np.array_equal(bits16(np_of(out)), bits16(out_o))
+        args = [to_dev(a, dev) for a in (aq, w, sw, sa)]
+        call = lambda out, acc: op.w8a8_gemm_forward_cuda(*args, out, _acc_out=acc)  # noqa: E731
+    acc, out, out_n = _run_both(dev, call, M, N)
+    assert np.array_equal(acc, acc_o)
+    assert np.array_equal(bits16(out), bits16(out_o))
+    assert np.array_equal(bits16(out_n), bits16(out_o))
 
 
 @pytest.mark.parametrize("M,N,K", [(64, 28672, 4096), (16, 19072, 384), (33, 37888, 256), (1, 20480, 128), (64, 24576, 1152)])
@@ -189,12 +205,10 @@ def test_wide_layers_bit_exact(dev, M, N, K):
     aq, sa, asum = _acts(rng, M, K)
     out_o, acc_o = w4a8.gemm_w4a8_per_chn(aq, qw, s1, sa, s1z, asum, return_acc=True)
     args = [to_dev(a, dev) for a in (aq, qw, s1, sa, s1z, asum)]
-    out = torch.full((M, N), float("nan"), dtype=torch.half, device=dev)
-    acc = torch.zeros((M, N), dtype=torch.int32, device=dev)
-    op.gemm_forward_cuda(*args, out, _acc_out=acc)
-    torch.cuda.synchronize()
-    assert np.array_equal(np_of(acc), acc_o)
-    assert np.array_equal(bits16(np_of(out)), bits16(out_o))
+    acc, out, out_n = _run_both(dev, lambda out, acc: op.gemm_forward_cuda(*args, out, _acc_out=acc), M, N)
+    assert np.array_equal(acc, acc_o)
+    assert np.array_equal(bits16(out), bits16(out_o))
+    assert np.array_equal(bits16(out_n), bits16(out_o))
 
 
 def test_linearity_property_full_size(dev):

@@ -1,6 +1,7 @@
 """GPU parity of every split-K plan of the decode GEMM: the automatic plan (one wave, sized by the occupancy API) and each forced cluster
 split S in {1, 2, 4, 8}, at the tile size the planner picks for M.  Split-K partials are INT32 and reduced in integer adds, so every plan
-must give the oracle's INT32 accumulators and fp16 outputs bit for bit."""
+must give the oracle's INT32 accumulators and fp16 outputs bit for bit, on the instantiation that dumps the accumulators and on the one
+the decode runner launches (no dump)."""
 import numpy as np
 import pytest
 import torch
@@ -52,11 +53,13 @@ def test_every_split_plan_bit_exact(dev, mode, M, N, K):
     try:
         for split in (0, 1, 2, 4, 8):  # 0: the automatic plan
             lib.qs_gemm_force_split(split)
-            out = torch.full((M, N), float("nan"), dtype=torch.half, device=dev)
-            acc = torch.zeros((M, N), dtype=torch.int32, device=dev)
-            call(out, acc)
-            torch.cuda.synchronize()
-            assert np.array_equal(np_of(acc), acc_o), split
-            assert np.array_equal(bits16(np_of(out)), bits16(out_o)), split
+            for dump in (True, False):
+                out = torch.full((M, N), float("nan"), dtype=torch.half, device=dev)
+                acc = torch.zeros((M, N), dtype=torch.int32, device=dev) if dump else None
+                call(out, acc)
+                torch.cuda.synchronize()
+                if dump:
+                    assert np.array_equal(np_of(acc), acc_o), split
+                assert np.array_equal(bits16(np_of(out)), bits16(out_o)), (split, dump)
     finally:
         lib.qs_gemm_force_split(0)

@@ -2,7 +2,8 @@
 split S in {1, 2, 4, 8}, at token counts on both sides of every tile boundary.  Split-K partials are INT32 and reduced in integer adds, so
 every plan must give the oracle's INT32 accumulators and fp16 outputs bit for bit, and a partial token tile must write nothing past row M.
 K = 384 is included: K % 256 == 128, so the last pipeline stage is half zero-filled.  One test replays a CUDA graph of split launches with
-programmatic dependent launch on: the split-K receive buffer aliases the pipeline rings, so a partial that arrived late or early would show."""
+programmatic dependent launch on: the split-K receive buffer aliases the pipeline rings, so a partial that arrived late or early would show.
+Every plan runs on both instantiations of the kernel: with the INT32 accumulator dump, and without it, as the decode runner launches it."""
 import numpy as np
 import pytest
 import torch
@@ -59,14 +60,20 @@ def test_every_tile_and_split_bit_exact(dev, mode, N, K):
                 for split in (1, 2, 4, 8):
                     lib.qs_gemm_force_tile_tokens(nt)
                     lib.qs_gemm_force_split(split)
-                    out = torch.full((M + PAD_ROWS, N), float("nan"), dtype=torch.half, device=dev)
-                    acc = torch.full((M + PAD_ROWS, N), sentinel, dtype=torch.int32, device=dev)
-                    call(M, out[:M], acc[:M])
-                    torch.cuda.synchronize()
-                    what = (M, nt, split)
-                    assert torch.equal(acc[:M], acc_o[:M]), what
-                    assert torch.equal(out[:M].view(torch.int16), out_o[:M]), what
-                    assert bool(torch.isnan(out[M:]).all()) and bool((acc[M:] == sentinel).all()), what
+                    outs = []
+                    for dump in (True, False):
+                        out = torch.full((M + PAD_ROWS, N), float("nan"), dtype=torch.half, device=dev)
+                        acc = torch.full((M + PAD_ROWS, N), sentinel, dtype=torch.int32, device=dev)
+                        call(M, out[:M], acc[:M] if dump else None)
+                        torch.cuda.synchronize()
+                        what = (M, nt, split, dump)
+                        assert torch.equal(out[:M].view(torch.int16), out_o[:M]), what
+                        assert bool(torch.isnan(out[M:]).all()), what
+                        if dump:
+                            assert torch.equal(acc[:M], acc_o[:M]), what
+                            assert bool((acc[M:] == sentinel).all()), what
+                        outs.append(out)
+                    assert torch.equal(outs[0].view(torch.int16), outs[1].view(torch.int16)), (M, nt, split)
     finally:
         lib.qs_gemm_force_split(0)
         lib.qs_gemm_force_tile_tokens(0)
@@ -75,17 +82,17 @@ def test_every_tile_and_split_bit_exact(dev, mode, N, K):
 @pytest.mark.parametrize("mode", ["chn", "grp", "w8"])
 def test_split_plans_under_graph_replay_with_pdl(dev, mode):
     """Back-to-back split launches of every tile size in one CUDA graph, programmatic dependent launch on: 20 replays, every output
-    equal to the oracle's every time."""
+    equal to the oracle's every time.  Each plan is captured on both instantiations, with and without the accumulator dump."""
     from qserve_b200 import backend
     from qserve_b200._lib import lib
     N, K, M = 4096, 4096, 64
     call, out_o, acc_o = _problem(mode, N, K, dev)
-    plans = [(nt, split) for nt in (32, 64, 128) for split in (2, 4, 8)] + [(0, 0)]
+    plans = [(nt, split, dump) for nt in (32, 64, 128) for split in (2, 4, 8) for dump in (True, False)] + [(0, 0, True), (0, 0, False)]
     outs = [torch.empty((M, N), dtype=torch.half, device=dev) for _ in plans]
-    accs = [torch.empty((M, N), dtype=torch.int32, device=dev) for _ in plans]
+    accs = [torch.empty((M, N), dtype=torch.int32, device=dev) if dump else None for _, _, dump in plans]
 
     def chain():
-        for (nt, split), out, acc in zip(plans, outs, accs):
+        for (nt, split, _), out, acc in zip(plans, outs, accs):
             lib.qs_gemm_force_tile_tokens(nt)
             lib.qs_gemm_force_split(split)
             call(M, out, acc)
@@ -104,11 +111,12 @@ def test_split_plans_under_graph_replay_with_pdl(dev, mode):
         for rep in range(20):
             for out, acc in zip(outs, accs):
                 out.fill_(float("nan"))
-                acc.zero_()
+                if acc is not None:
+                    acc.zero_()
             g.replay()
             torch.cuda.synchronize()
             for plan, out, acc in zip(plans, outs, accs):
-                assert torch.equal(acc, acc_o[:M]), (rep, plan)
+                assert acc is None or torch.equal(acc, acc_o[:M]), (rep, plan)
                 assert torch.equal(out.view(torch.int16), out_o[:M]), (rep, plan)
     finally:
         backend.set_pdl(was)
