@@ -591,6 +591,48 @@ typedef struct qs_kv_pool_args {
 } qs_kv_pool_args;
 QS_API int qs_inflight_schedule_pool(const qs_inflight_args* args, const qs_kv_pool_args* pool, void* stream);
 
+/* Automatic prefix caching over the shared KV page pool (DESIGN.md 3.12, "Prefix cache"): rows reuse the cached full 64-token pages of a
+ * common prefix.  The key of page j of a row is (parent, parent epoch, history[64 j .. 64 j + 64)), where the parent is the row's page
+ * j - 1 (epoch[parent] when the key is made) or -1 with parent epoch 0 for j = 0.  A page's epoch increases when it is registered and when
+ * it is evicted, so a key names exact content and exact ancestry.  Lookups compare parent, parent epoch and all 64 ids; the hash only picks
+ * the index slot.  Every page is in exactly one state: FREE (on the free stack; state 0, ref 0), HELD (ref >= 1 = the number of row page
+ * lists holding it; state 1 private, which has ref 1, or state 2 registered) or EVICTABLE (state 2, ref 0, in the LRU list).  Per row, its
+ * first reg[b] pages are registered and form a key chain, and stop[b] = 1 ends registration for the rest of the row's tenure.
+ *
+ * qs_inflight_schedule_pool_cache follows qs_inflight_schedule_pool with these changes (tests/prefix_cache_oracle.py restates them):
+ *   0. Register, first, over every row that holds pages in row order (DECODE rows about to retire too): with cached = done (PREFILL) or
+ *      seq_len - 1 (DECODE), pages j = reg[b] .. cached / 64 - 1 in order, unless stop[b]: if the key is in the index, stop[b] = 1 and the
+ *      row registers no more (a duplicate); otherwise the page becomes registered, its epoch increases, it enters the index, reg[b] = j + 1.
+ *   1. Release (retire and every preemption victim): private pages go onto the free stack in page order; then from the last registered
+ *      page to the first, ref decreases and a page that reaches 0 goes to the LRU tail (a chain's tail is queued before its head).
+ *      reg[b] = stop[b] = 0.
+ *   3. A page is taken from the free stack if top > 0, else the LRU head is evicted (out of the index, epoch + 1) and taken; a taken page is
+ *      private with ref 1.  If neither exists the youngest page holder is preempted, as in the pool, and again until a page can be taken or
+ *      the requester is itself the victim (a victim whose pages are all shared frees none).
+ *   4. Starts, strictly first-come-first-served: m = the longest chain of registered pages matching history[0 .. 64 m), m <=
+ *      (target - 1) / 64; e = how many of them are EVICTABLE.  The row starts when top + evictable - e >= ceil(target / 64) - m: the m pages
+ *      leave the LRU, gain a ref and head the page list, the rest are taken as in 3, done = 64 m and reg[b] = m.
+ *   5., 6. as the pool; prefix_lens = done starts at 64 m and the tables of a started row are written from entry 0.
+ * counters int32 [8]: LRU head, LRU tail (-1: empty), evictable pages, registered pages, hit pages, registrations, evictions, duplicates.
+ * The pool's peak counts the pages held by rows.  Limits: index_size a power of two >= 2 pages.                                         */
+typedef struct qs_prefix_cache_args {
+  int32_t* ref;        /* [pages] */
+  int32_t* state;      /* [pages] 0 free, 1 private, 2 registered */
+  int32_t* epoch;      /* [pages] */
+  int32_t* key_parent; /* [pages] */
+  int32_t* key_epoch;  /* [pages] */
+  int32_t* hash;       /* [pages] key hash of a registered page */
+  int32_t* key_tokens; /* [pages, 64] */
+  int32_t* lru_prev;   /* [pages] -1 ends */
+  int32_t* lru_next;   /* [pages] */
+  int32_t* index;      /* [index_size] page ids, -1 empty (open addressing, linear probing, backward-shift deletion) */
+  int32_t* reg;        /* [batch] */
+  int32_t* stop;       /* [batch] */
+  int32_t* counters;   /* [8] */
+  int index_size;
+} qs_prefix_cache_args;
+QS_API int qs_inflight_schedule_pool_cache(const qs_inflight_args* args, const qs_kv_pool_args* pool, const qs_prefix_cache_args* cache, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

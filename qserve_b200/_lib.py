@@ -47,6 +47,7 @@ SIGNATURES = {
     "qs_beam_select": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "qs_inflight_schedule": (c_int, [_P, _P]),
     "qs_inflight_schedule_pool": (c_int, [_P, _P, _P]),
+    "qs_inflight_schedule_pool_cache": (c_int, [_P, _P, _P, _P]),
     "qs_beam_reorder": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "qs_sample_rows": (c_int, [_P, _P, _P, _P, _P, ctypes.c_uint64, _P, _I, _I, _P]),
     "qs_tree_accept_sampling": (c_int, [_P, _P, _P, _P, _P, _P, _P, ctypes.c_uint64, _P, _P, _P, _P, _I, _I, _I, _P]),

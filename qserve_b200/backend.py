@@ -951,9 +951,45 @@ class _KvPoolArgs(ctypes.Structure):
         [("page_bytes", ctypes.c_longlong)] + [(n, ctypes.c_int) for n in ("pages", "blocks", "layers")]
 
 
+class PrefixCache(NamedTuple):
+    """The prefix cache over a KvPool (qs_inflight_schedule_pool_cache): per page its ref, state (0 free, 1 private, 2 registered), epoch and
+    key, the LRU list of the evictable pages, the index of the registered ones and per row its registered pages and stop flag."""
+    ref: torch.Tensor         # int32 [P]
+    state: torch.Tensor       # int32 [P]
+    epoch: torch.Tensor       # int32 [P]
+    key_parent: torch.Tensor  # int32 [P]
+    key_epoch: torch.Tensor   # int32 [P]
+    hash: torch.Tensor        # int32 [P]
+    key_tokens: torch.Tensor  # int32 [P, 64]
+    lru_prev: torch.Tensor    # int32 [P]
+    lru_next: torch.Tensor    # int32 [P]
+    index: torch.Tensor       # int32 [S]: page ids, -1 empty; S the smallest power of two >= 2 P
+    reg: torch.Tensor         # int32 [B]
+    stop: torch.Tensor        # int32 [B]
+    counters: torch.Tensor    # int32 [8]: LRU head, LRU tail, evictable, registered, hit pages, registrations, evictions, duplicates
+
+
+def prefix_cache_buffers(pool: KvPool) -> PrefixCache:
+    """A fresh, empty PrefixCache for `pool` (torch.full / torch.zeros: no random draws)."""
+    P = _tensor(pool.free, "pool.free", torch.int32, (None,)).size(0)
+    B = _tensor(pool.count, "pool.count", torch.int32, (None,), pool.free.device).size(0)
+    dev = pool.free.device
+    z = lambda *shape: torch.zeros(shape, dtype=torch.int32, device=dev)
+    m1 = lambda *shape: torch.full(shape, -1, dtype=torch.int32, device=dev)
+    counters = z(8)
+    counters[:2] = -1
+    S = 1 << (2 * P - 1).bit_length()
+    return PrefixCache(z(P), z(P), z(P), m1(P), z(P), z(P), z(P, 64), m1(P), m1(P), m1(S), z(B), z(B), counters)
+
+
+class _PrefixCacheArgs(ctypes.Structure):
+    """qs_prefix_cache_args of include/qserve_b200.h, field for field."""
+    _fields_ = [(n, ctypes.c_void_p) for n in PrefixCache._fields] + [("index_size", ctypes.c_int)]
+
+
 def inflight_schedule(queue: InflightQueue, rows: InflightRows, history, prompt_lens, seq_lens, temperature, top_k, top_p, repetition, presence,
                       frequency, eos, stop, budget, offsets, finished, start_pos, tokens_in, logprob: Optional[torch.Tensor], plan: InflightPlan,
-                      out: InflightOutputs, chunk_budget: int, pool: Optional[KvPool] = None) -> None:
+                      out: InflightOutputs, chunk_budget: int, pool: Optional[KvPool] = None, cache: Optional[PrefixCache] = None) -> None:
     """One in-flight schedule, in place and without host synchronisation (include/qserve_b200.h qs_inflight_schedule; restated in
     tests/inflight_oracle.py): retire the DECODE rows with finished = 1 into `out`, admit queued requests into FREE rows first-come-first-served
     (chunk_budget > 0 only), plan the chunk segment (chunk_budget = C or 0) and the decode segment into `plan`, and set the tail masks.  The
@@ -961,7 +997,11 @@ def inflight_schedule(queue: InflightQueue, rows: InflightRows, history, prompt_
 
     pool (kv_pool_buffers): qs_inflight_schedule_pool instead (restated in tests/kv_pool_oracle.py): the rows draw their pages from the pool,
     with decode growth, preemption by recompute and first-come-first-served starts, and the schedule writes the new entries of pool.tables.
-    The pool needs at least ceil((prompt_cols + max_tokens + 1) / 64) pages, and the tables as many blocks."""
+    The pool needs at least ceil((prompt_cols + max_tokens + 1) / 64) pages, and the tables as many blocks.
+
+    cache (prefix_cache_buffers(pool)): qs_inflight_schedule_pool_cache instead (restated in tests/prefix_cache_oracle.py): the full pages
+    rows cache are registered under their content and ancestry, and a starting row takes the longest chain of them that matches its history
+    and computes only the rest; released registered pages stay cached until a page is needed and they are evicted, oldest release first."""
     B = _tensor(rows.phase, "phase", torch.int32, (None,)).size(0)
     dev = rows.phase.device
     _require(1 <= B <= MAX_INFLIGHT_ROWS, f"batch={B}: 1 .. {MAX_INFLIGHT_ROWS} rows")
@@ -1006,6 +1046,7 @@ def inflight_schedule(queue: InflightQueue, rows: InflightRows, history, prompt_
                 out_tokens=out.tokens, out_len=out.length, out_reason=out.reason, out_logprob=out.logprob, out_ids=out.ids)
     a = _InflightArgs(**{k: _ptr(v) for k, v in ptrs.items()}, batch=B, queue=Q, prompt_cols=P, history_len=H, max_tokens=T, chunk=C,
                       chunk_budget=int(chunk_budget))
+    _require(cache is None or pool is not None, "the prefix cache needs a pool")
     if pool is None:
         _call(rows.phase, lib.qs_inflight_schedule, ctypes.addressof(a))
         return
@@ -1023,7 +1064,19 @@ def inflight_schedule(queue: InflightQueue, rows: InflightRows, history, prompt_
     pa = _KvPoolArgs(free_pages=pool.free.data_ptr(), counters=pool.counters.data_ptr(), row_pages=pool.pages.data_ptr(), row_count=pool.count.data_ptr(),
                      target=pool.target.data_ptr(), tables=pool.tables.data_ptr(), layer_base=pool.layer_base.data_ptr(), page_bytes=int(pool.page_bytes),
                      pages=n_pages, blocks=nb, layers=L)
-    _call(rows.phase, lib.qs_inflight_schedule_pool, ctypes.addressof(a), ctypes.addressof(pa))
+    if cache is None:
+        _call(rows.phase, lib.qs_inflight_schedule_pool, ctypes.addressof(a), ctypes.addressof(pa))
+        return
+    for name in ("ref", "state", "epoch", "key_parent", "key_epoch", "hash", "lru_prev", "lru_next"):
+        _tensor(getattr(cache, name), f"cache.{name}", torch.int32, (n_pages,), dev)
+    _tensor(cache.key_tokens, "cache.key_tokens", torch.int32, (n_pages, 64), dev)
+    S = _tensor(cache.index, "cache.index", torch.int32, (None,), dev).size(0)
+    _require(S >= 2 * n_pages and S & (S - 1) == 0, f"cache.index of {S} slots: a power of two >= 2 x {n_pages} pages")
+    _tensor(cache.reg, "cache.reg", torch.int32, (B,), dev)
+    _tensor(cache.stop, "cache.stop", torch.int32, (B,), dev)
+    _tensor(cache.counters, "cache.counters", torch.int32, (8,), dev)
+    ca = _PrefixCacheArgs(**{n: getattr(cache, n).data_ptr() for n in PrefixCache._fields}, index_size=S)
+    _call(rows.phase, lib.qs_inflight_schedule_pool_cache, ctypes.addressof(a), ctypes.addressof(pa), ctypes.addressof(ca))
 
 
 def _row_vec(v, n: int, dev, dt, name: str, ok, what: str) -> torch.Tensor:

@@ -579,4 +579,9 @@ int qs_inflight_schedule_pool(const qs_inflight_args* args, const qs_kv_pool_arg
   return inflight_schedule_pool(*args, *pool, stream);
 }
 
+int qs_inflight_schedule_pool_cache(const qs_inflight_args* args, const qs_kv_pool_args* pool, const qs_prefix_cache_args* cache, void* stream) {
+  QS_REQUIRE(args != nullptr && pool != nullptr && cache != nullptr, "inflight_schedule_pool_cache: null arguments");
+  return inflight_schedule_pool_cache(*args, *pool, *cache, stream);
+}
+
 }  // extern "C"

@@ -14,6 +14,13 @@
 // inflight_schedule_kernel<true> adds the shared KV page pool of qs_inflight_schedule_pool: thread 0 also keeps the free stack (retire and
 // preemption push, decode growth and starts pop, in the header's order), and the block then writes the new table entries of every layer.
 // <false> is the own-pages schedule above, unchanged.
+//
+// inflight_schedule_kernel<true, true> adds the prefix cache of qs_inflight_schedule_pool_cache: per-page refs, states, epochs and keys, an LRU
+// list of the evictable pages and an open-addressing index of the registered ones, all in device memory.  The two scans that touch the 64
+// token ids of a page run block-parallel, a warp per page or row, so thread 0 only makes the serial decisions: the token hashes of the pages
+// rule 0 may register (written with the ids into the pages' key slots; a private page's key slot is scratch), and the longest match of every
+// waiting row, searched after the decode growth.  Registrations happen only in rule 0, so during the starts a match can only shrink, when a
+// start evicts one of its pages: thread 0 cuts it at the first page that is no longer registered, which gives the sequential rule exactly.
 #include <math_constants.h>
 
 #include <climits>
@@ -28,8 +35,13 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kMaxRows = 512;
 constexpr int kStops = 8;  // stop ids per request (MAX_STOP_TOKENS)
+constexpr int kWarps = kThreads / 32;
 constexpr int kPageTokens = 64;
 enum : int { kFree = 0, kPrefill = 1, kDecode = 2 };
+enum : int { kPageFree = 0, kPagePrivate = 1, kPageRegistered = 2 };
+// qs_prefix_cache_args.counters
+enum : int { kLruHead = 0, kLruTail = 1, kEvictable = 2, kRegistered = 3, kHitPages = 4, kRegistrations = 5, kEvictions = 6, kDuplicates = 7,
+             kCacheCounters = 8 };
 enum : int { kHead = 0, kTail = 1, kRetired = 2, kAdmitted = 3 };
 enum : int { kReasonEos = 1, kReasonStop = 2, kReasonBudget = 3 };
 
@@ -39,11 +51,151 @@ __device__ __forceinline__ void push_pages(const qs_kv_pool_args& p, int b, int 
   for (int j = 0; j < count; ++j) p.free_pages[top++] = pg[j];
 }
 
+// ---- prefix cache (qs_inflight_schedule_pool_cache); tests/prefix_cache_oracle.py computes the same hashes ----
+__device__ __forceinline__ uint32_t fmix32(uint32_t x) {
+  x ^= x >> 16;
+  x *= 0x85EBCA6Bu;
+  x ^= x >> 13;
+  x *= 0xC2B2AE35u;
+  x ^= x >> 16;
+  return x;
+}
+
+// The token hash of a page: the sum of every id's mix with its slot, summed over a warp (lane i holds ids i and i + 32).
+__device__ __forceinline__ uint32_t token_hash(int t0, int t1, int lane) {
+  uint32_t s = fmix32(static_cast<uint32_t>(t0) + static_cast<uint32_t>(lane) * 0x9E3779B9u) +
+               fmix32(static_cast<uint32_t>(t1) + static_cast<uint32_t>(lane + 32) * 0x9E3779B9u);
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  return s;
+}
+
+__device__ __forceinline__ int key_hash(uint32_t tokens, int parent, int parent_epoch) {
+  return static_cast<int>(fmix32(tokens ^ fmix32(static_cast<uint32_t>(parent) * 0x27D4EB2Fu + static_cast<uint32_t>(parent_epoch))));
+}
+
+// Index lookup by thread 0: the registered page whose key is (parent, parent_epoch, tok[0 .. 64)) and whose hash is h, else -1.
+__device__ int cache_find(const qs_prefix_cache_args& c, int h, int parent, int parent_epoch, const int32_t* tok) {
+  const int mask = c.index_size - 1;
+  for (int i = h & mask;; i = (i + 1) & mask) {
+    const int q = c.index[i];
+    if (q < 0) return -1;
+    if (c.hash[q] != h || c.key_parent[q] != parent || c.key_epoch[q] != parent_epoch) continue;
+    const int4* x = reinterpret_cast<const int4*>(c.key_tokens + static_cast<size_t>(q) * kPageTokens);
+    const int4* y = reinterpret_cast<const int4*>(tok);
+    bool same = true;
+    for (int k = 0; k < kPageTokens / 4 && same; ++k) {
+      const int4 u = x[k], v = y[k];
+      same = u.x == v.x && u.y == v.y && u.z == v.z && u.w == v.w;
+    }
+    if (same) return q;
+  }
+}
+
+__device__ void cache_insert(const qs_prefix_cache_args& c, int q) {
+  const int mask = c.index_size - 1;
+  int i = c.hash[q] & mask;
+  while (c.index[i] >= 0) i = (i + 1) & mask;
+  c.index[i] = q;
+}
+
+// Backward-shift deletion: every later entry of the probe run that may fill the hole moves into it, so the index never holds tombstones.
+__device__ void cache_erase(const qs_prefix_cache_args& c, int q) {
+  const int mask = c.index_size - 1;
+  int i = c.hash[q] & mask;
+  while (c.index[i] != q) i = (i + 1) & mask;
+  for (int j = (i + 1) & mask;; j = (j + 1) & mask) {
+    const int r = c.index[j];
+    if (r < 0) break;
+    const int k = c.hash[r] & mask;  // r's home slot: r may move to i unless k lies cyclically in (i, j]
+    if (i <= j ? (i < k && k <= j) : (i < k || k <= j)) continue;
+    c.index[i] = r;
+    i = j;
+  }
+  c.index[i] = -1;
+}
+
+__device__ void lru_push(const qs_prefix_cache_args& c, int* cc, int q) {
+  const int t = cc[kLruTail];
+  c.lru_prev[q] = t;
+  c.lru_next[q] = -1;
+  if (t >= 0) c.lru_next[t] = q;
+  else cc[kLruHead] = q;
+  cc[kLruTail] = q;
+  ++cc[kEvictable];
+}
+
+__device__ void lru_remove(const qs_prefix_cache_args& c, int* cc, int q) {
+  const int pr = c.lru_prev[q], nx = c.lru_next[q];
+  if (pr >= 0) c.lru_next[pr] = nx;
+  else cc[kLruHead] = nx;
+  if (nx >= 0) c.lru_prev[nx] = pr;
+  else cc[kLruTail] = pr;
+  --cc[kEvictable];
+}
+
+// Rule 1 (thread 0): row b's private pages [reg, count) onto the free stack in page order, then its registered pages from the last to the
+// first lose a ref, and those at ref 0 join the LRU tail.
+__device__ void cache_release(const qs_kv_pool_args& p, const qs_prefix_cache_args& c, int* cc, int b, int count, int* s_reg, int* s_stop,
+                              int& top) {
+  const int32_t* pg = p.row_pages + static_cast<size_t>(b) * p.blocks;
+  for (int j = s_reg[b]; j < count; ++j) {
+    const int q = pg[j];
+    p.free_pages[top++] = q;
+    c.ref[q] = 0;
+    c.state[q] = kPageFree;
+  }
+  for (int j = s_reg[b] - 1; j >= 0; --j)
+    if (--c.ref[pg[j]] == 0) lru_push(c, cc, pg[j]);
+  s_reg[b] = s_stop[b] = 0;
+}
+
+// Rule 3's page (thread 0): the top of the free stack, else the evicted LRU head; the caller has checked that one exists.
+__device__ int cache_take(const qs_kv_pool_args& p, const qs_prefix_cache_args& c, int* cc, int& top) {
+  int q;
+  if (top > 0) {
+    q = p.free_pages[--top];
+  } else {
+    q = cc[kLruHead];
+    lru_remove(c, cc, q);
+    cache_erase(c, q);
+    ++c.epoch[q];
+    --cc[kRegistered];
+    ++cc[kEvictions];
+  }
+  c.ref[q] = 1;
+  c.state[q] = kPagePrivate;
+  return q;
+}
+
+// The youngest row that holds pages and is younger than the requester b of admission rank r, else b (thread 0).
+__device__ __forceinline__ int youngest_holder(int r, int b, int n_live, const int* s_order, const int* s_cnt) {
+  for (int q = n_live - 1; q > r; --q)
+    if (s_cnt[s_order[q]] > 0) return s_order[q];
+  return b;
+}
+
+// Pool rule 5 (thread 0): the chunk budget over the started rows in admission order, then the row-order offsets.
+__device__ __forceinline__ void pool_budget(const qs_inflight_args& a, int B, int n_live, const int* s_phase, const int* s_order, const int* s_rank,
+                                            const int* s_cnt, const int* s_tgt, const int* s_done, int* s_rem, int* s_cu) {
+  int used = 0;
+  for (int r = 0; r < n_live; ++r) {
+    const int b = s_order[r];
+    const int take = s_phase[b] == kPrefill && s_cnt[b] > 0 ? min(s_tgt[b] - s_done[b], a.chunk_budget - used) : 0;
+    s_rem[r] = take;
+    used += take;
+  }
+  s_cu[0] = 0;
+  for (int b = 0; b < B; ++b) s_cu[b + 1] = s_cu[b] + (s_phase[b] == kPrefill ? s_rem[s_rank[b]] : 0);
+}
+
 // Pool rules 3-5 (qs_inflight_schedule_pool), called by the whole block after the admissions: admission ranks of every live row and the
 // shared copies of seq_lens / done (parallel), then thread 0 runs the decode growth (with preemption), the starts and the chunk budget scan
-// over the started rows in admission order, and the row-order offsets.  Ends with a barrier.
-__device__ void pool_plan(const qs_inflight_args& a, const qs_kv_pool_args& p, int* s_phase, int* s_adm, int* s_rem, int* s_rank, int* s_done,
-                          int* s_cu, int* s_cnt, int* s_keep, int* s_tgt, int* s_len, int* s_order) {
+// over the started rows in admission order, and the row-order offsets.  Ends with a barrier.  With the prefix cache the starts follow a
+// block-parallel search of every waiting row's longest match (s_m) after the decode growth.
+template <bool kCache>
+__device__ void pool_plan(const qs_inflight_args& a, const qs_kv_pool_args& p, const qs_prefix_cache_args& c, int* s_phase, int* s_adm,
+                          int* s_rem, int* s_rank, int* s_done, int* s_cu, int* s_cnt, int* s_keep, int* s_tgt, int* s_len, int* s_order, int* s_reg,
+                          int* s_stop, int* s_m, int* s_cc) {
   const int B = a.batch, tid = threadIdx.x;
   for (int b = tid; b < B; b += kThreads) {
     s_adm[b] = s_phase[b] != kFree ? a.adm[b] : INT_MAX;
@@ -64,14 +216,36 @@ __device__ void pool_plan(const qs_inflight_args& a, const qs_kv_pool_args& p, i
     for (int b = 0; b < B; ++b) n_live += s_phase[b] != kFree;
     int top = p.counters[0], peak = p.counters[1], preempted = p.counters[2], started = p.counters[3];
     auto pop = [&](int b) {
-      p.row_pages[static_cast<size_t>(b) * p.blocks + s_cnt[b]++] = p.free_pages[--top];
-      peak = max(peak, p.pages - top);
+      if constexpr (kCache) {
+        p.row_pages[static_cast<size_t>(b) * p.blocks + s_cnt[b]++] = cache_take(p, c, s_cc, top);
+        peak = max(peak, p.pages - top - s_cc[kEvictable]);
+      } else {
+        p.row_pages[static_cast<size_t>(b) * p.blocks + s_cnt[b]++] = p.free_pages[--top];
+        peak = max(peak, p.pages - top);
+      }
     };
-    // 3: decode growth; the victim is the youngest page holder, never older than the requester (which holds pages)
+    auto preempt = [&](int v) {  // the cache's victim, after its release
+      s_cnt[v] = s_keep[v] = s_done[v] = 0;
+      s_tgt[v] = s_len[v];
+      s_phase[v] = kPrefill;
+      a.phase[v] = kPrefill;
+      ++preempted;
+    };
+    // 3: decode growth; the victim is the youngest page holder, never older than the requester (which holds pages).  With the cache a
+    // victim whose pages are all shared frees none, so the preemptions go on until a page can be taken or the requester was the victim.
     for (int r = 0; r < n_live; ++r) {
       const int b = s_order[r];
       if (s_phase[b] != kDecode || s_cnt[b] > (s_len[b] - 1) / kPageTokens) continue;
-      if (top == 0) {
+      if constexpr (kCache) {
+        bool self = false;
+        while (top == 0 && s_cc[kEvictable] == 0 && !self) {
+          const int v = youngest_holder(r, b, n_live, s_order, s_cnt);
+          cache_release(p, c, s_cc, v, s_cnt[v], s_reg, s_stop, top);
+          preempt(v);
+          self = v == b;
+        }
+        if (self) continue;
+      } else if (top == 0) {
         int v = b;
         for (int q = n_live - 1; q > r; --q)
           if (s_cnt[s_order[q]] > 0) {
@@ -88,35 +262,95 @@ __device__ void pool_plan(const qs_inflight_args& a, const qs_kv_pool_args& p, i
       }
       pop(b);
     }
-    // 4: starts, strict first-come-first-served
-    for (int r = 0; r < n_live; ++r) {
-      const int b = s_order[r];
-      if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;
-      const int need = (s_tgt[b] + kPageTokens - 1) / kPageTokens;
-      if (need > top) break;
-      while (s_cnt[b] < need) pop(b);
-      ++started;
+    if constexpr (kCache) {
+      p.counters[0] = top;
+      p.counters[1] = peak;
+      p.counters[2] = preempted;
+    } else {
+      // 4: starts, strict first-come-first-served
+      for (int r = 0; r < n_live; ++r) {
+        const int b = s_order[r];
+        if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;
+        const int need = (s_tgt[b] + kPageTokens - 1) / kPageTokens;
+        if (need > top) break;
+        while (s_cnt[b] < need) pop(b);
+        ++started;
+      }
+      // 5
+      pool_budget(a, B, n_live, s_phase, s_order, s_rank, s_cnt, s_tgt, s_done, s_rem, s_cu);
+      p.counters[0] = top;
+      p.counters[1] = peak;
+      p.counters[2] = preempted;
+      p.counters[3] = started;
     }
-    // 5: the chunk budget over the started rows in admission order, then the row-order offsets
-    int used = 0;
-    for (int r = 0; r < n_live; ++r) {
-      const int b = s_order[r];
-      const int take = s_phase[b] == kPrefill && s_cnt[b] > 0 ? min(s_tgt[b] - s_done[b], a.chunk_budget - used) : 0;
-      s_rem[r] = take;
-      used += take;
+  }
+  if constexpr (kCache) {
+    __syncthreads();
+    // 4, in parallel: every waiting row's longest chain of registered pages matching its history, a warp per row, with full key checks;
+    // the pages go to the row's (empty) page list, their number to s_m
+    const int warp = tid >> 5, lane = tid & 31, mask = c.index_size - 1;
+    for (int b = warp; b < B; b += kWarps) {
+      if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;  // warp-uniform
+      const int64_t* h = a.history + static_cast<size_t>(b) * a.history_len;
+      int32_t* pg = p.row_pages + static_cast<size_t>(b) * p.blocks;
+      const int most = (s_tgt[b] - 1) / kPageTokens;  // at least one token is computed, so the completing step has a logit
+      int parent = -1, pe = 0, m = 0;
+      for (; m < most; ++m) {
+        const int t0 = static_cast<int>(h[m * kPageTokens + lane]), t1 = static_cast<int>(h[m * kPageTokens + 32 + lane]);
+        const int key = key_hash(token_hash(t0, t1, lane), parent, pe);
+        int q = -1;
+        for (int i = key & mask;; i = (i + 1) & mask) {
+          const int r = c.index[i];
+          if (r < 0) break;
+          const int32_t* kt = c.key_tokens + static_cast<size_t>(r) * kPageTokens;
+          if (c.hash[r] == key && c.key_parent[r] == parent && c.key_epoch[r] == pe && __all_sync(0xffffffffu, kt[lane] == t0 && kt[lane + 32] == t1)) {
+            q = r;
+            break;
+          }
+        }
+        if (q < 0) break;
+        if (lane == 0) pg[m] = q;
+        parent = q;
+        pe = c.epoch[q];
+      }
+      if (lane == 0) s_m[b] = m;
     }
-    s_cu[0] = 0;
-    for (int b = 0; b < B; ++b) s_cu[b + 1] = s_cu[b] + (s_phase[b] == kPrefill ? s_rem[s_rank[b]] : 0);
-    p.counters[0] = top;
-    p.counters[1] = peak;
-    p.counters[2] = preempted;
-    p.counters[3] = started;
+    __syncthreads();
+    if (tid == 0) {
+      int n_live = 0;
+      for (int b = 0; b < B; ++b) n_live += s_phase[b] != kFree;
+      int top = p.counters[0], peak = p.counters[1], started = p.counters[3];
+      // 4: starts, strict first-come-first-served; a match is cut at the first page an earlier start evicted
+      for (int r = 0; r < n_live; ++r) {
+        const int b = s_order[r];
+        if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;
+        const int need = (s_tgt[b] + kPageTokens - 1) / kPageTokens;
+        int32_t* pg = p.row_pages + static_cast<size_t>(b) * p.blocks;
+        int m = 0, e = 0;
+        for (; m < s_m[b] && c.state[pg[m]] == kPageRegistered; ++m) e += c.ref[pg[m]] == 0;
+        if (top + s_cc[kEvictable] - e < need - m) break;
+        for (int j = 0; j < m; ++j)
+          if (c.ref[pg[j]]++ == 0) lru_remove(c, s_cc, pg[j]);
+        s_cnt[b] = s_reg[b] = m;
+        s_done[b] = m * kPageTokens;
+        s_cc[kHitPages] += m;
+        while (s_cnt[b] < need) {  // need > m: the takes also count the matched pages in the peak
+          pg[s_cnt[b]++] = cache_take(p, c, s_cc, top);
+          peak = max(peak, p.pages - top - s_cc[kEvictable]);
+        }
+        ++started;
+      }
+      pool_budget(a, B, n_live, s_phase, s_order, s_rank, s_cnt, s_tgt, s_done, s_rem, s_cu);
+      p.counters[0] = top;
+      p.counters[1] = peak;
+      p.counters[3] = started;
+    }
   }
   __syncthreads();
 }
 
-template <bool kPool>
-__global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_inflight_args a, const qs_kv_pool_args p) {
+template <bool kPool, bool kCache>
+__global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_inflight_args a, const qs_kv_pool_args p, const qs_prefix_cache_args c) {
   __shared__ int s_phase[kMaxRows];  // phase before this call (after the retire: FREE)
   __shared__ int s_ring[kMaxRows];   // retire: index in the retired ring + 1, else 0
   __shared__ int s_gone[kMaxRows];   // retire: the request the row hands back (row_req is cleared while the block still copies its outputs)
@@ -132,6 +366,11 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
   __shared__ int s_tgt[kPoolRows];    // pool: prefill target
   __shared__ int s_len[kPoolRows];    // pool: seq_lens after the admissions
   __shared__ int s_order[kPoolRows];  // pool: the live rows by admission rank
+  constexpr int kCacheRows = kCache ? kMaxRows : 1;
+  __shared__ int s_reg[kCacheRows];   // cache: registered leading pages
+  __shared__ int s_stop[kCacheRows];  // cache: registration stopped by a duplicate
+  __shared__ int s_m[kCacheRows];     // cache: rule 0's end page, then a waiting row's longest match
+  __shared__ int s_cc[kCacheCounters];
   if (threadIdx.x == 0) pdl_launch_dependents();
   pdl_wait();
   const int B = a.batch, Q = a.queue, H = a.history_len, T = a.max_tokens, C = a.chunk;
@@ -140,6 +379,32 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
     for (int b = tid; b < B; b += kThreads) {
       s_cnt[b] = s_keep[b] = p.row_count[b];
       s_tgt[b] = p.target[b];
+      if constexpr (kCache) {
+        s_reg[b] = c.reg[b];
+        s_stop[b] = c.stop[b];
+        const int ph = a.phase[b], cached = ph == kPrefill ? a.done[b] : ph == kDecode ? a.seq_lens[b] - 1 : 0;
+        s_m[b] = s_cnt[b] > 0 && !s_stop[b] ? cached / kPageTokens : 0;
+      }
+    }
+    if constexpr (kCache) {
+      if (tid < kCacheCounters) s_cc[tid] = c.counters[tid];
+    }
+    __syncthreads();
+  }
+  if constexpr (kCache) {
+    // ---- cache 0, in parallel: the token hashes and key ids of the pages the registration may take, a warp per page ----
+    const int warp = tid >> 5, lane = tid & 31;
+    for (int b = 0; b < B; ++b) {
+      for (int j = s_reg[b] + warp; j < s_m[b]; j += kWarps) {
+        const int q = p.row_pages[static_cast<size_t>(b) * p.blocks + j];
+        const int64_t* h = a.history + static_cast<size_t>(b) * H + j * kPageTokens;
+        const int t0 = static_cast<int>(h[lane]), t1 = static_cast<int>(h[lane + 32]);
+        int32_t* kt = c.key_tokens + static_cast<size_t>(q) * kPageTokens;
+        kt[lane] = t0;
+        kt[lane + 32] = t1;
+        const uint32_t th = token_hash(t0, t1, lane);
+        if (lane == 0) c.hash[q] = static_cast<int>(th);
+      }
     }
     __syncthreads();
   }
@@ -151,6 +416,30 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
     const int tail = a.counters[kTail];
     int admitted = a.counters[kAdmitted];
     int top = kPool ? p.counters[0] : 0;
+    if constexpr (kCache) {
+      // 0: register, in row order, the full cached pages past each row's registered ones, until a key is already cached
+      for (int b = 0; b < B; ++b) {
+        const int32_t* pg = p.row_pages + static_cast<size_t>(b) * p.blocks;
+        for (int j = s_reg[b]; j < s_m[b]; ++j) {
+          const int q = pg[j], parent = j > 0 ? pg[j - 1] : -1, pe = j > 0 ? c.epoch[parent] : 0;
+          const int key = key_hash(static_cast<uint32_t>(c.hash[q]), parent, pe);
+          if (cache_find(c, key, parent, pe, c.key_tokens + static_cast<size_t>(q) * kPageTokens) >= 0) {
+            s_stop[b] = 1;
+            ++s_cc[kDuplicates];
+            break;
+          }
+          c.state[q] = kPageRegistered;
+          ++c.epoch[q];
+          c.key_parent[q] = parent;
+          c.key_epoch[q] = pe;
+          c.hash[q] = key;
+          cache_insert(c, q);
+          s_reg[b] = j + 1;
+          ++s_cc[kRegistrations];
+          ++s_cc[kRegistered];
+        }
+      }
+    }
     for (int b = 0; b < B; ++b) {
       int ph = a.phase[b];
       s_ring[b] = 0;
@@ -158,10 +447,9 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
         s_ring[b] = ++retired;
         s_gone[b] = a.row_req[b];
         ph = kFree;
-        if constexpr (kPool) {
-          push_pages(p, b, s_cnt[b], top);
-          s_cnt[b] = s_keep[b] = 0;
-        }
+        if constexpr (kCache) cache_release(p, c, s_cc, b, s_cnt[b], s_reg, s_stop, top);
+        else if constexpr (kPool) push_pages(p, b, s_cnt[b], top);
+        if constexpr (kPool) s_cnt[b] = s_keep[b] = 0;
       }
       s_phase[b] = ph;
       s_req[b] = -1;
@@ -241,7 +529,7 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
   __syncthreads();
 
   if constexpr (kPool) {
-    pool_plan(a, p, s_phase, s_adm, s_rem, s_rank, s_done, s_cu, s_cnt, s_keep, s_tgt, s_len, s_order);
+    pool_plan<kCache>(a, p, c, s_phase, s_adm, s_rem, s_rank, s_done, s_cu, s_cnt, s_keep, s_tgt, s_len, s_order, s_reg, s_stop, s_m, s_cc);
   } else {
     // ---- 3: admission ranks of the PREFILL rows (parallel), the budget scan in admission order and the row-order offsets (thread 0) ----
     for (int b = tid; b < B; b += kThreads) s_adm[b] = s_phase[b] == kPrefill ? a.adm[b] : INT_MAX;
@@ -327,7 +615,14 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
     for (int b = tid; b < B; b += kThreads) {
       p.row_count[b] = s_cnt[b];
       p.target[b] = s_tgt[b];
+      if constexpr (kCache) {
+        c.reg[b] = s_reg[b];
+        c.stop[b] = s_stop[b];
+      }
     }
+  }
+  if constexpr (kCache) {
+    if (tid < kCacheCounters) c.counters[tid] = s_cc[tid];
   }
 }
 
@@ -350,23 +645,40 @@ int check_inflight_args(const qs_inflight_args& a) {
   return 0;
 }
 
-}  // namespace
-
-int inflight_schedule(const qs_inflight_args& a, void* stream) {
-  const int rc = check_inflight_args(a);
-  if (rc) return rc;
-  return launch(inflight_schedule_kernel<false>, dim3(1), dim3(kThreads), 0, 0, stream, "inflight_schedule", a, qs_kv_pool_args{});
-}
-
-int inflight_schedule_pool(const qs_inflight_args& a, const qs_kv_pool_args& p, void* stream) {
+// The argument checks of both pool schedules.
+int check_pool_args(const qs_inflight_args& a, const qs_kv_pool_args& p) {
   const long long need = (static_cast<long long>(a.prompt_cols) + a.max_tokens + 1 + kPageTokens - 1) / kPageTokens;
   QS_REQUIRE(p.pages >= need && p.blocks >= need, "inflight_schedule_pool: pages=%d blocks=%d (each at least ceil((prompt_cols %d + max_tokens %d + 1) / 64) = %lld)",
              p.pages, p.blocks, a.prompt_cols, a.max_tokens, need);
   QS_REQUIRE(p.layers >= 1 && p.page_bytes >= 1, "inflight_schedule_pool: layers=%d page_bytes=%lld", p.layers, p.page_bytes);
   QS_REQUIRE(p.free_pages && p.counters && p.row_pages && p.row_count && p.target && p.tables && p.layer_base, "inflight_schedule_pool: null pointer");
+  return check_inflight_args(a);
+}
+
+}  // namespace
+
+int inflight_schedule(const qs_inflight_args& a, void* stream) {
   const int rc = check_inflight_args(a);
   if (rc) return rc;
-  return launch(inflight_schedule_kernel<true>, dim3(1), dim3(kThreads), 0, 0, stream, "inflight_schedule_pool", a, p);
+  return launch(inflight_schedule_kernel<false, false>, dim3(1), dim3(kThreads), 0, 0, stream, "inflight_schedule", a, qs_kv_pool_args{},
+                qs_prefix_cache_args{});
+}
+
+int inflight_schedule_pool(const qs_inflight_args& a, const qs_kv_pool_args& p, void* stream) {
+  const int rc = check_pool_args(a, p);
+  if (rc) return rc;
+  return launch(inflight_schedule_kernel<true, false>, dim3(1), dim3(kThreads), 0, 0, stream, "inflight_schedule_pool", a, p, qs_prefix_cache_args{});
+}
+
+int inflight_schedule_pool_cache(const qs_inflight_args& a, const qs_kv_pool_args& p, const qs_prefix_cache_args& c, void* stream) {
+  QS_REQUIRE(c.index_size >= 2 * p.pages && (c.index_size & (c.index_size - 1)) == 0,
+             "inflight_schedule_pool_cache: index_size=%d must be a power of two >= 2 pages (%d)", c.index_size, p.pages);
+  QS_REQUIRE(c.ref && c.state && c.epoch && c.key_parent && c.key_epoch && c.hash && c.key_tokens && c.lru_prev && c.lru_next && c.index && c.reg &&
+                 c.stop && c.counters,
+             "inflight_schedule_pool_cache: null pointer");
+  const int rc = check_pool_args(a, p);
+  if (rc) return rc;
+  return launch(inflight_schedule_kernel<true, true>, dim3(1), dim3(kThreads), 0, 0, stream, "inflight_schedule_pool_cache", a, p, c);
 }
 
 }  // namespace qs

@@ -5,6 +5,7 @@
 
 struct qs_inflight_args;  // include/qserve_b200.h
 struct qs_kv_pool_args;
+struct qs_prefix_cache_args;
 
 namespace qs {
 
@@ -367,5 +368,7 @@ int spec_commit_stops(const SpecCommitArgs& a, const long long* stop_ids, int nu
 int inflight_schedule(const qs_inflight_args& a, void* stream);
 // ... and of qs_inflight_schedule_pool
 int inflight_schedule_pool(const qs_inflight_args& a, const qs_kv_pool_args& p, void* stream);
+// ... and of qs_inflight_schedule_pool_cache
+int inflight_schedule_pool_cache(const qs_inflight_args& a, const qs_kv_pool_args& p, const qs_prefix_cache_args& c, void* stream);
 
 }  // namespace qs

@@ -177,6 +177,19 @@ class KvPoolStats(NamedTuple):
     starts: int
 
 
+class PrefixCacheStats(NamedTuple):
+    """DecodeRunner.prefix_cache_stats: the registered pages now and how many of them are evictable (held by no row), and since
+    construction the pages and prompt tokens starting rows took from the cache instead of computing them, the registrations, the evictions
+    and the duplicates (full pages not registered because a page of the same key was already cached)."""
+    cached_pages: int
+    evictable_pages: int
+    hit_pages: int
+    hit_tokens: int
+    registrations: int
+    evictions: int
+    duplicates: int
+
+
 _PROMPT_LOGITS_BYTES = 64 << 20  # prompt_logprobs: fp16 logits of at most this many bytes exist at once
 
 
@@ -185,7 +198,7 @@ class DecodeRunner:
                  device: Optional[torch.device] = None, tp_rank: int = 0, tp_size: int = 1, seed: int = 0, layers: Optional[int] = None,
                  process_group=None, fused: bool = True, ops: Optional[OpSet] = None, tp_exact: bool = False, tp_peer: bool = False, no_comm: bool = False,
                  verify_len: int = 0, max_new_tokens: int = 0, generate: bool = False, prompt_tokens: int = 0, shared_prefix: bool = False,
-                 beam_width: int = 0, inflight: int = 0, kv_pool_pages: int = 0):
+                 beam_width: int = 0, inflight: int = 0, kv_pool_pages: int = 0, prefix_cache: bool = False):
         """verify_len > 0 (single GPU, fused path) adds the speculative-decoding verify step (`verify_forward`): the page tables cover
         ctx + verify_len tokens and the activation buffers hold batch * verify_len rows.  verify_len = 0 leaves the decode step, its buffers
         and its random draws exactly as they are without it.
@@ -235,7 +248,13 @@ class DecodeRunner:
         page-holding row, which recomputes its prompt and generated tokens as a prefill.  P >= ceil((ctx + T + 1) / 64), so the oldest request
         always fits.  The per-row random pages are not made; the pools are zero-filled after every random draw, so the weights are those of
         kv_pool_pages = 0.  The tables cover max(ctx + T + 1, ctx + T - 1 + C) tokens (a recomputed row's prefix reaches ctx + T - 1).  Pool mode
-        is fixed at construction: prefill, fork, reset_generation and load_shard_of refuse it."""
+        is fixed at construction: prefill, fork, reset_generation and load_shard_of refuse it.
+
+        prefix_cache=True (needs kv_pool_pages) adds automatic prefix caching over the pool (DESIGN.md 3.12, "Prefix cache"): the schedule
+        registers every full 64-token page a row has cached under its tokens and its parent page, and a starting row takes the longest chain
+        of registered pages that matches its prompt (or, after a preemption, its history) and prefills only the rest.  Pages no row holds
+        stay cached until the pool needs them (least recently released first).  Automatic, with no per-request option; fixed at construction.
+        prefix_cache_stats reports it."""
         self.cfg = cfg = MODELS[model]
         self.max_pos = min(8192, cfg.max_pos)  # the positions the attention kernels support
         beam_width, inflight, ops = int(beam_width), int(inflight), ops or DEFAULT_OPS
@@ -264,11 +283,13 @@ class DecodeRunner:
                 (inflight and not 1 <= batch <= _ext.MAX_INFLIGHT_ROWS, f"in-flight batching runs 1 .. {_ext.MAX_INFLIGHT_ROWS} rows"),
                 (kv_pool_pages and not inflight, "kv_pool_pages needs in-flight batching (inflight >= 1)"),
                 (kv_pool_pages and not kv_pool_pages >= (ctx + T + 1 + 63) // 64,
-                 f"kv_pool_pages={kv_pool_pages}: at least ceil((ctx + max_new_tokens + 1) / 64) = {(ctx + T + 1 + 63) // 64} pages")):
+                 f"kv_pool_pages={kv_pool_pages}: at least ceil((ctx + max_new_tokens + 1) / 64) = {(ctx + T + 1 + 63) // 64} pages"),
+                (prefix_cache and not kv_pool_pages, "prefix_cache needs the shared KV page pool (kv_pool_pages >= 1)")):
             if bad:
                 raise RuntimeError(why)
         self.beam_width, self.inflight, self.shared_prefix, self.prompt_tokens = beam_width, inflight, shared_prefix, prompt_tokens
         self.kv_pool_pages = kv_pool_pages = int(kv_pool_pages)
+        self.prefix_cache = bool(prefix_cache)
         self.generate, self.verify_len, self.ops, self.tp_exact = generate, verify_len, ops, tp_exact
         self.no_comm = no_comm  # debugging: run one rank's shard of a tensor-parallel model without the collectives (sanitizer / profiler runs)
         # tensor parallel, fused path: the all-reduce of the row-parallel GEMM outputs is folded into the following add+norm+quant kernel
@@ -1174,6 +1195,7 @@ class DecodeRunner:
         if self.kv_pool_pages:
             base = torch.tensor([[k.data_ptr(), v.data_ptr()] for k, v in zip(self.kpools, self.vpools)], dtype=torch.int64, device=self.dev)
             self.i_pool = _ext.kv_pool_buffers(self.block_tables, base, self.kv_pool_pages, self.page_bytes)
+        self.i_cache = _ext.prefix_cache_buffers(self.i_pool) if self.prefix_cache else None
         self._i_submitted = 0       # requests submitted (the host's tail)
         self._i_lens: dict = {}     # prompt length of every request not yet polled
         self._i_unpolled: set = set()
@@ -1245,7 +1267,7 @@ class DecodeRunner:
         _ext.inflight_schedule(self.i_queue, self.i_rows, self.s_history, self.s_prompt_lens, self.s_seq_lens, self.s_temperature, self.s_top_k,
                                self.s_top_p, self.s_repetition, self.s_presence, self.s_frequency, self.g_eos, self.g_stop, self.g_budget,
                                self.s_offsets, self.g_finished, self.g_start, self.tokens_in, self.g_logprob, self.i_plan, self.i_out, chunk_budget,
-                               pool=self.i_pool)
+                               pool=self.i_pool, cache=self.i_cache)
 
     def inflight_forward(self, mixed: bool = True, sampled: bool = False, penalties: bool = False, logprobs: int = 0) -> None:
         """One in-flight step; no host synchronisation.  inflight_schedule (chunk budget C, or 0 when mixed=False: nothing is admitted and no
@@ -1323,11 +1345,19 @@ class DecodeRunner:
         return InflightPoll(finished, queued + prefilling)
 
     def pool_stats(self) -> KvPoolStats:
-        """The shared KV page pool's counters (kv_pool_pages > 0).  One host synchronisation."""
+        """The shared KV page pool's counters (kv_pool_pages > 0).  One host synchronisation.  With prefix_cache, free_pages is the free
+        stack only (the evictable pages are in prefix_cache_stats) and peak_pages counts the pages held by rows."""
         if self.i_pool is None:
             raise RuntimeError("pool_stats needs kv_pool_pages > 0")
         top, peak, pre, starts = self.i_pool.counters.tolist()
         return KvPoolStats(top, peak, pre, starts)
+
+    def prefix_cache_stats(self) -> PrefixCacheStats:
+        """The prefix cache's counters (prefix_cache=True).  One host synchronisation."""
+        if self.i_cache is None:
+            raise RuntimeError("prefix_cache_stats needs prefix_cache=True")
+        _, _, evictable, cached, hits, regs, evictions, dups = self.i_cache.counters.tolist()
+        return PrefixCacheStats(cached, evictable, hits, 64 * hits, regs, evictions, dups)
 
     def _refuse_pool(self, what: str) -> None:
         if self.kv_pool_pages:
