@@ -11,9 +11,9 @@
 // the PDL dependency wait: the previous step's commit writes the lengths, the histories and `finished`, and the host writes the queue and
 // the tail counter between steps.
 //
-// inflight_schedule_kernel<true> adds the shared KV page pool of qs_inflight_schedule_pool: thread 0 also keeps the free stack (retire and
-// preemption push, decode growth and starts pop, in the header's order), and the block then writes the new table entries of every layer.
-// <false> is the own-pages schedule above, unchanged.
+// inflight_schedule_kernel<true, false> adds the shared KV page pool of qs_inflight_schedule_pool: thread 0 also keeps the free stack (retire
+// and preemption push, decode growth and starts pop, in the header's order), and the block then writes the new table entries of every layer.
+// <false, false> is the same body with no page step: every PREFILL row counts as started and its target is its prompt length.
 //
 // inflight_schedule_kernel<true, true> adds the prefix cache of qs_inflight_schedule_pool_cache: per-page refs, states, epochs and keys, an LRU
 // list of the evictable pages and an open-addressing index of the registered ones, all in device memory.  The two scans that touch the 64
@@ -174,198 +174,25 @@ __device__ __forceinline__ int youngest_holder(int r, int b, int n_live, const i
   return b;
 }
 
-// Pool rule 5 (thread 0): the chunk budget over the started rows in admission order, then the row-order offsets.
-__device__ __forceinline__ void pool_budget(const qs_inflight_args& a, int B, int n_live, const int* s_phase, const int* s_order, const int* s_rank,
-                                            const int* s_cnt, const int* s_tgt, const int* s_done, int* s_rem, int* s_cu) {
-  int used = 0;
-  for (int r = 0; r < n_live; ++r) {
-    const int b = s_order[r];
-    const int take = s_phase[b] == kPrefill && s_cnt[b] > 0 ? min(s_tgt[b] - s_done[b], a.chunk_budget - used) : 0;
-    s_rem[r] = take;
-    used += take;
-  }
-  s_cu[0] = 0;
-  for (int b = 0; b < B; ++b) s_cu[b + 1] = s_cu[b] + (s_phase[b] == kPrefill ? s_rem[s_rank[b]] : 0);
-}
-
-// Pool rules 3-5 (qs_inflight_schedule_pool), called by the whole block after the admissions: admission ranks of every live row and the
-// shared copies of seq_lens / done (parallel), then thread 0 runs the decode growth (with preemption), the starts and the chunk budget scan
-// over the started rows in admission order, and the row-order offsets.  Ends with a barrier.  With the prefix cache the starts follow a
-// block-parallel search of every waiting row's longest match (s_m) after the decode growth.
-template <bool kCache>
-__device__ void pool_plan(const qs_inflight_args& a, const qs_kv_pool_args& p, const qs_prefix_cache_args& c, int* s_phase, int* s_adm,
-                          int* s_rem, int* s_rank, int* s_done, int* s_cu, int* s_cnt, int* s_keep, int* s_tgt, int* s_len, int* s_order, int* s_reg,
-                          int* s_stop, int* s_m, int* s_cc) {
-  const int B = a.batch, tid = threadIdx.x;
-  for (int b = tid; b < B; b += kThreads) {
-    s_adm[b] = s_phase[b] != kFree ? a.adm[b] : INT_MAX;
-    s_len[b] = a.seq_lens[b];
-  }
-  __syncthreads();
-  for (int b = tid; b < B; b += kThreads) {
-    if (s_phase[b] == kFree) continue;
-    int r = 0;
-    for (int o = 0; o < B; ++o) r += s_adm[o] < s_adm[b];  // admission numbers are distinct
-    s_rank[b] = r;
-    s_order[r] = b;
-    s_done[b] = a.done[b];
-  }
-  __syncthreads();
-  if (tid == 0) {
-    int n_live = 0;
-    for (int b = 0; b < B; ++b) n_live += s_phase[b] != kFree;
-    int top = p.counters[0], peak = p.counters[1], preempted = p.counters[2], started = p.counters[3];
-    auto pop = [&](int b) {
-      if constexpr (kCache) {
-        p.row_pages[static_cast<size_t>(b) * p.blocks + s_cnt[b]++] = cache_take(p, c, s_cc, top);
-        peak = max(peak, p.pages - top - s_cc[kEvictable]);
-      } else {
-        p.row_pages[static_cast<size_t>(b) * p.blocks + s_cnt[b]++] = p.free_pages[--top];
-        peak = max(peak, p.pages - top);
-      }
-    };
-    auto preempt = [&](int v) {  // the cache's victim, after its release
-      s_cnt[v] = s_keep[v] = s_done[v] = 0;
-      s_tgt[v] = s_len[v];
-      s_phase[v] = kPrefill;
-      a.phase[v] = kPrefill;
-      ++preempted;
-    };
-    // 3: decode growth; the victim is the youngest page holder, never older than the requester (which holds pages).  With the cache a
-    // victim whose pages are all shared frees none, so the preemptions go on until a page can be taken or the requester was the victim.
-    for (int r = 0; r < n_live; ++r) {
-      const int b = s_order[r];
-      if (s_phase[b] != kDecode || s_cnt[b] > (s_len[b] - 1) / kPageTokens) continue;
-      if constexpr (kCache) {
-        bool self = false;
-        while (top == 0 && s_cc[kEvictable] == 0 && !self) {
-          const int v = youngest_holder(r, b, n_live, s_order, s_cnt);
-          cache_release(p, c, s_cc, v, s_cnt[v], s_reg, s_stop, top);
-          preempt(v);
-          self = v == b;
-        }
-        if (self) continue;
-      } else if (top == 0) {
-        int v = b;
-        for (int q = n_live - 1; q > r; --q)
-          if (s_cnt[s_order[q]] > 0) {
-            v = s_order[q];
-            break;
-          }
-        push_pages(p, v, s_cnt[v], top);
-        s_cnt[v] = s_keep[v] = s_done[v] = 0;
-        s_tgt[v] = s_len[v];
-        s_phase[v] = kPrefill;
-        a.phase[v] = kPrefill;
-        ++preempted;
-        if (v == b) continue;
-      }
-      pop(b);
-    }
-    if constexpr (kCache) {
-      p.counters[0] = top;
-      p.counters[1] = peak;
-      p.counters[2] = preempted;
-    } else {
-      // 4: starts, strict first-come-first-served
-      for (int r = 0; r < n_live; ++r) {
-        const int b = s_order[r];
-        if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;
-        const int need = (s_tgt[b] + kPageTokens - 1) / kPageTokens;
-        if (need > top) break;
-        while (s_cnt[b] < need) pop(b);
-        ++started;
-      }
-      // 5
-      pool_budget(a, B, n_live, s_phase, s_order, s_rank, s_cnt, s_tgt, s_done, s_rem, s_cu);
-      p.counters[0] = top;
-      p.counters[1] = peak;
-      p.counters[2] = preempted;
-      p.counters[3] = started;
-    }
-  }
-  if constexpr (kCache) {
-    __syncthreads();
-    // 4, in parallel: every waiting row's longest chain of registered pages matching its history, a warp per row, with full key checks;
-    // the pages go to the row's (empty) page list, their number to s_m
-    const int warp = tid >> 5, lane = tid & 31, mask = c.index_size - 1;
-    for (int b = warp; b < B; b += kWarps) {
-      if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;  // warp-uniform
-      const int64_t* h = a.history + static_cast<size_t>(b) * a.history_len;
-      int32_t* pg = p.row_pages + static_cast<size_t>(b) * p.blocks;
-      const int most = (s_tgt[b] - 1) / kPageTokens;  // at least one token is computed, so the completing step has a logit
-      int parent = -1, pe = 0, m = 0;
-      for (; m < most; ++m) {
-        const int t0 = static_cast<int>(h[m * kPageTokens + lane]), t1 = static_cast<int>(h[m * kPageTokens + 32 + lane]);
-        const int key = key_hash(token_hash(t0, t1, lane), parent, pe);
-        int q = -1;
-        for (int i = key & mask;; i = (i + 1) & mask) {
-          const int r = c.index[i];
-          if (r < 0) break;
-          const int32_t* kt = c.key_tokens + static_cast<size_t>(r) * kPageTokens;
-          if (c.hash[r] == key && c.key_parent[r] == parent && c.key_epoch[r] == pe && __all_sync(0xffffffffu, kt[lane] == t0 && kt[lane + 32] == t1)) {
-            q = r;
-            break;
-          }
-        }
-        if (q < 0) break;
-        if (lane == 0) pg[m] = q;
-        parent = q;
-        pe = c.epoch[q];
-      }
-      if (lane == 0) s_m[b] = m;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      int n_live = 0;
-      for (int b = 0; b < B; ++b) n_live += s_phase[b] != kFree;
-      int top = p.counters[0], peak = p.counters[1], started = p.counters[3];
-      // 4: starts, strict first-come-first-served; a match is cut at the first page an earlier start evicted
-      for (int r = 0; r < n_live; ++r) {
-        const int b = s_order[r];
-        if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;
-        const int need = (s_tgt[b] + kPageTokens - 1) / kPageTokens;
-        int32_t* pg = p.row_pages + static_cast<size_t>(b) * p.blocks;
-        int m = 0, e = 0;
-        for (; m < s_m[b] && c.state[pg[m]] == kPageRegistered; ++m) e += c.ref[pg[m]] == 0;
-        if (top + s_cc[kEvictable] - e < need - m) break;
-        for (int j = 0; j < m; ++j)
-          if (c.ref[pg[j]]++ == 0) lru_remove(c, s_cc, pg[j]);
-        s_cnt[b] = s_reg[b] = m;
-        s_done[b] = m * kPageTokens;
-        s_cc[kHitPages] += m;
-        while (s_cnt[b] < need) {  // need > m: the takes also count the matched pages in the peak
-          pg[s_cnt[b]++] = cache_take(p, c, s_cc, top);
-          peak = max(peak, p.pages - top - s_cc[kEvictable]);
-        }
-        ++started;
-      }
-      pool_budget(a, B, n_live, s_phase, s_order, s_rank, s_cnt, s_tgt, s_done, s_rem, s_cu);
-      p.counters[0] = top;
-      p.counters[1] = peak;
-      p.counters[3] = started;
-    }
-  }
-  __syncthreads();
-}
-
+// One body for the three schedules: `if constexpr` guards only the state a mode adds, pages and tables (kPool), registration, LRU and match
+// (kCache), never a second copy of a rule.
 template <bool kPool, bool kCache>
 __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_inflight_args a, const qs_kv_pool_args p, const qs_prefix_cache_args c) {
   __shared__ int s_phase[kMaxRows];  // phase before this call (after the retire: FREE)
   __shared__ int s_ring[kMaxRows];   // retire: index in the retired ring + 1, else 0
   __shared__ int s_gone[kMaxRows];   // retire: the request the row hands back (row_req is cleared while the block still copies its outputs)
   __shared__ int s_req[kMaxRows];    // admit: the request taken in this call, else -1
-  __shared__ int s_adm[kMaxRows];    // admission numbers of the PREFILL rows (pool: of every live row)
-  __shared__ int s_rem[kMaxRows];    // prompt tokens still to cache, by admission rank, then the tokens taken, by rank
+  __shared__ int s_adm[kMaxRows];    // admission numbers of the live rows
+  __shared__ int s_rem[kMaxRows];    // prompt tokens taken, by admission rank
   __shared__ int s_rank[kMaxRows];
+  __shared__ int s_order[kMaxRows];  // the live rows by admission rank
   __shared__ int s_done[kMaxRows];   // prompt tokens cached before this call
+  __shared__ int s_tgt[kMaxRows];    // prefill target
   __shared__ int s_cu[kMaxRows + 1];
   constexpr int kPoolRows = kPool ? kMaxRows : 1;
-  __shared__ int s_cnt[kPoolRows];    // pool: pages held
-  __shared__ int s_keep[kPoolRows];   // pool: leading page-list entries this call leaves as they were
-  __shared__ int s_tgt[kPoolRows];    // pool: prefill target
-  __shared__ int s_len[kPoolRows];    // pool: seq_lens after the admissions
-  __shared__ int s_order[kPoolRows];  // pool: the live rows by admission rank
+  __shared__ int s_cnt[kPoolRows];   // pool: pages held
+  __shared__ int s_keep[kPoolRows];  // pool: leading page-list entries this call leaves as they were
+  __shared__ int s_len[kPoolRows];   // pool: seq_lens after the admissions
   constexpr int kCacheRows = kCache ? kMaxRows : 1;
   __shared__ int s_reg[kCacheRows];   // cache: registered leading pages
   __shared__ int s_stop[kCacheRows];  // cache: registration stopped by a duplicate
@@ -375,22 +202,39 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
   pdl_wait();
   const int B = a.batch, Q = a.queue, H = a.history_len, T = a.max_tokens, C = a.chunk;
   const int tid = threadIdx.x;
-  if constexpr (kPool) {
-    for (int b = tid; b < B; b += kThreads) {
-      s_cnt[b] = s_keep[b] = p.row_count[b];
-      s_tgt[b] = p.target[b];
-      if constexpr (kCache) {
-        s_reg[b] = c.reg[b];
-        s_stop[b] = c.stop[b];
-        const int ph = a.phase[b], cached = ph == kPrefill ? a.done[b] : ph == kDecode ? a.seq_lens[b] - 1 : 0;
-        s_m[b] = s_cnt[b] > 0 && !s_stop[b] ? cached / kPageTokens : 0;
-      }
-    }
+  for (int b = tid; b < B; b += kThreads) {
+    s_tgt[b] = kPool ? p.target[b] : a.prompt_lens[b];
+    if constexpr (kPool) s_cnt[b] = s_keep[b] = p.row_count[b];
     if constexpr (kCache) {
-      if (tid < kCacheCounters) s_cc[tid] = c.counters[tid];
+      s_reg[b] = c.reg[b];
+      s_stop[b] = c.stop[b];
+      const int ph = a.phase[b], cached = ph == kPrefill ? a.done[b] : ph == kDecode ? a.seq_lens[b] - 1 : 0;
+      s_m[b] = s_cnt[b] > 0 && !s_stop[b] ? cached / kPageTokens : 0;
     }
-    __syncthreads();
   }
+  if constexpr (kCache) {
+    if (tid < kCacheCounters) s_cc[tid] = c.counters[tid];
+  }
+  __syncthreads();
+
+  // Thread 0's page steps, in the header's order.  The free-stack top and the pool counters stay in its registers from the retire to the
+  // starts.  A page is taken from the free stack, else (cache) from the evicted LRU head; a released row's pages go back to the free stack,
+  // or (cache, registered pages) lose a ref and join the LRU at ref 0.
+  int top = 0, peak = 0, preempted = 0, started = 0, n_live = 0;
+  auto takeable = [&] { return top + (kCache ? s_cc[kEvictable] : 0); };
+  auto take = [&](int b) {
+    int q;
+    if constexpr (kCache) q = cache_take(p, c, s_cc, top);
+    else q = p.free_pages[--top];
+    p.row_pages[static_cast<size_t>(b) * p.blocks + s_cnt[b]++] = q;
+    peak = max(peak, p.pages - takeable());
+  };
+  auto release = [&](int b) {
+    if constexpr (kCache) cache_release(p, c, s_cc, b, s_cnt[b], s_reg, s_stop, top);
+    else push_pages(p, b, s_cnt[b], top);
+    s_cnt[b] = s_keep[b] = 0;
+  };
+
   if constexpr (kCache) {
     // ---- cache 0, in parallel: the token hashes and key ids of the pages the registration may take, a warp per page ----
     const int warp = tid >> 5, lane = tid & 31;
@@ -415,7 +259,12 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
     int head = a.counters[kHead];
     const int tail = a.counters[kTail];
     int admitted = a.counters[kAdmitted];
-    int top = kPool ? p.counters[0] : 0;
+    if constexpr (kPool) {
+      top = p.counters[0];
+      peak = p.counters[1];
+      preempted = p.counters[2];
+      started = p.counters[3];
+    }
     if constexpr (kCache) {
       // 0: register, in row order, the full cached pages past each row's registered ones, until a key is already cached
       for (int b = 0; b < B; ++b) {
@@ -447,9 +296,7 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
         s_ring[b] = ++retired;
         s_gone[b] = a.row_req[b];
         ph = kFree;
-        if constexpr (kCache) cache_release(p, c, s_cc, b, s_cnt[b], s_reg, s_stop, top);
-        else if constexpr (kPool) push_pages(p, b, s_cnt[b], top);
-        if constexpr (kPool) s_cnt[b] = s_keep[b] = 0;
+        if constexpr (kPool) release(b);
       }
       s_phase[b] = ph;
       s_req[b] = -1;
@@ -461,7 +308,6 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
     a.counters[kRetired] = retired;
     a.counters[kHead] = head;
     a.counters[kAdmitted] = admitted;
-    if constexpr (kPool) p.counters[0] = top;
   }
   __syncthreads();
 
@@ -523,40 +369,123 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
       a.row_req[b] = req;
       a.phase[b] = kPrefill;
       s_phase[b] = kPrefill;
-      if constexpr (kPool) s_tgt[b] = len;
+      s_tgt[b] = len;
     }
   }
   __syncthreads();
 
-  if constexpr (kPool) {
-    pool_plan<kCache>(a, p, c, s_phase, s_adm, s_rem, s_rank, s_done, s_cu, s_cnt, s_keep, s_tgt, s_len, s_order, s_reg, s_stop, s_m, s_cc);
-  } else {
-    // ---- 3: admission ranks of the PREFILL rows (parallel), the budget scan in admission order and the row-order offsets (thread 0) ----
-    for (int b = tid; b < B; b += kThreads) s_adm[b] = s_phase[b] == kPrefill ? a.adm[b] : INT_MAX;
-    __syncthreads();
-    for (int b = tid; b < B; b += kThreads) {
-      if (s_phase[b] != kPrefill) continue;
-      int r = 0;
-      for (int o = 0; o < B; ++o) r += s_adm[o] < s_adm[b];  // admission numbers are distinct
-      s_rank[b] = r;
-      s_done[b] = a.done[b];
-      s_rem[r] = a.prompt_lens[b] - s_done[b];
-    }
-    __syncthreads();
-    if (tid == 0) {
-      int n_pre = 0;
-      for (int b = 0; b < B; ++b) n_pre += s_phase[b] == kPrefill;
-      int used = 0;
-      for (int r = 0; r < n_pre; ++r) {
-        const int take = min(s_rem[r], a.chunk_budget - used);
-        s_rem[r] = take;
-        used += take;
+  // ---- admission ranks of the live rows and shared copies of done / seq_lens (parallel) ----
+  for (int b = tid; b < B; b += kThreads) {
+    s_adm[b] = s_phase[b] != kFree ? a.adm[b] : INT_MAX;
+    if constexpr (kPool) s_len[b] = a.seq_lens[b];
+  }
+  __syncthreads();
+  for (int b = tid; b < B; b += kThreads) {
+    if (s_phase[b] == kFree) continue;
+    int r = 0;
+    for (int o = 0; o < B; ++o) r += s_adm[o] < s_adm[b];  // admission numbers are distinct
+    s_rank[b] = r;
+    s_order[r] = b;
+    s_done[b] = a.done[b];
+  }
+  __syncthreads();
+  // ---- pool 3: decode growth (thread 0); the victim is the youngest page holder, never older than the requester (which holds pages).  With
+  // the cache a victim whose pages are all shared frees none, so the preemptions go on until a page can be taken or the requester was the victim ----
+  if (tid == 0) {
+    for (int b = 0; b < B; ++b) n_live += s_phase[b] != kFree;
+    if constexpr (kPool) {
+      for (int r = 0; r < n_live; ++r) {
+        const int b = s_order[r];
+        if (s_phase[b] != kDecode || s_cnt[b] > (s_len[b] - 1) / kPageTokens) continue;
+        bool self = false;
+        while (!self && takeable() == 0) {
+          const int v = youngest_holder(r, b, n_live, s_order, s_cnt);
+          release(v);
+          s_done[v] = 0;
+          s_tgt[v] = s_len[v];
+          s_phase[v] = kPrefill;
+          a.phase[v] = kPrefill;
+          ++preempted;
+          self = v == b;
+        }
+        if (!self) take(b);
       }
-      s_cu[0] = 0;
-      for (int b = 0; b < B; ++b) s_cu[b + 1] = s_cu[b] + (s_phase[b] == kPrefill ? s_rem[s_rank[b]] : 0);
+    }
+  }
+  if constexpr (kCache) {
+    __syncthreads();
+    // 4, in parallel: every waiting row's longest chain of registered pages matching its history, a warp per row, with full key checks;
+    // the pages go to the row's (empty) page list, their number to s_m
+    const int warp = tid >> 5, lane = tid & 31, mask = c.index_size - 1;
+    for (int b = warp; b < B; b += kWarps) {
+      if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;  // warp-uniform
+      const int64_t* h = a.history + static_cast<size_t>(b) * a.history_len;
+      int32_t* pg = p.row_pages + static_cast<size_t>(b) * p.blocks;
+      const int most = (s_tgt[b] - 1) / kPageTokens;  // at least one token is computed, so the completing step has a logit
+      int parent = -1, pe = 0, m = 0;
+      for (; m < most; ++m) {
+        const int t0 = static_cast<int>(h[m * kPageTokens + lane]), t1 = static_cast<int>(h[m * kPageTokens + 32 + lane]);
+        const int key = key_hash(token_hash(t0, t1, lane), parent, pe);
+        int q = -1;
+        for (int i = key & mask;; i = (i + 1) & mask) {
+          const int r = c.index[i];
+          if (r < 0) break;
+          const int32_t* kt = c.key_tokens + static_cast<size_t>(r) * kPageTokens;
+          if (c.hash[r] == key && c.key_parent[r] == parent && c.key_epoch[r] == pe && __all_sync(0xffffffffu, kt[lane] == t0 && kt[lane + 32] == t1)) {
+            q = r;
+            break;
+          }
+        }
+        if (q < 0) break;
+        if (lane == 0) pg[m] = q;
+        parent = q;
+        pe = c.epoch[q];
+      }
+      if (lane == 0) s_m[b] = m;
     }
     __syncthreads();
   }
+  if (tid == 0) {
+    if constexpr (kPool) {
+      // 4: starts, strict first-come-first-served.  With the cache a row reuses its match, cut at the first page an earlier start evicted,
+      // and needs e pages fewer to reach: the evictable pages of its match are its own
+      for (int r = 0; r < n_live; ++r) {
+        const int b = s_order[r];
+        if (s_phase[b] != kPrefill || s_cnt[b] > 0) continue;
+        const int need = (s_tgt[b] + kPageTokens - 1) / kPageTokens;
+        const int32_t* pg = p.row_pages + static_cast<size_t>(b) * p.blocks;
+        int m = 0, e = 0;
+        if constexpr (kCache)
+          for (; m < s_m[b] && c.state[pg[m]] == kPageRegistered; ++m) e += c.ref[pg[m]] == 0;
+        if (takeable() - e < need - m) break;
+        if constexpr (kCache) {
+          for (int j = 0; j < m; ++j)
+            if (c.ref[pg[j]]++ == 0) lru_remove(c, s_cc, pg[j]);
+          s_reg[b] = m;
+          s_cc[kHitPages] += m;
+        }
+        s_cnt[b] = m;
+        s_done[b] = m * kPageTokens;
+        while (s_cnt[b] < need) take(b);  // need > m: the takes also count the matched pages in the peak
+        ++started;
+      }
+      p.counters[0] = top;
+      p.counters[1] = peak;
+      p.counters[2] = preempted;
+      p.counters[3] = started;
+    }
+    // 5: the chunk budget over the started PREFILL rows in admission order, then the row-order offsets
+    int used = 0;
+    for (int r = 0; r < n_live; ++r) {
+      const int b = s_order[r];
+      const int n = s_phase[b] == kPrefill && (!kPool || s_cnt[b] > 0) ? min(s_tgt[b] - s_done[b], a.chunk_budget - used) : 0;
+      s_rem[r] = n;
+      used += n;
+    }
+    s_cu[0] = 0;
+    for (int b = 0; b < B; ++b) s_cu[b + 1] = s_cu[b] + (s_phase[b] == kPrefill ? s_rem[s_rank[b]] : 0);
+  }
+  __syncthreads();
 
   // ---- 3 + 4: the plan and the tail masks, one thread per row ----
   if (tid == 0) a.cu_seqlens[0] = 0;
@@ -570,7 +499,7 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
     long long logit = b;
     int fin = ph == kDecode ? 0 : 1;
     if (ph == kPrefill) {
-      const int d = s_done[b], len = kPool ? s_tgt[b] : a.prompt_lens[b];
+      const int d = s_done[b], len = s_tgt[b];
       a.prefix_lens[b] = d;
       a.done[b] = d + c;
       if (d + c == len) {
@@ -601,7 +530,7 @@ __global__ void __launch_bounds__(kThreads) inflight_schedule_kernel(const qs_in
     a.padding_offset[t] = C - 1 - t;
   }
   if constexpr (kPool) {
-    // ---- pool 6: the new table entries [keep, count) of every row, all layers, K and V (pool_plan's page lists are visible after its barrier) ----
+    // ---- pool 6: the new table entries [keep, count) of every row, all layers, K and V (the page lists are visible after the barrier) ----
     const int L = p.layers, nb = p.blocks;
     for (int b = 0; b < B; ++b) {
       const int k0 = s_keep[b], n = (s_cnt[b] - k0) * L * 2;

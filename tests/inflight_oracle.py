@@ -15,6 +15,8 @@ Rules of one schedule(chunk_budget) call, in this order:
      exists, so the append skips it).  Decode segment: context_lens = seq_len and token = tokens_in for DECODE rows, 0 and token 0 otherwise.
   4. Tail masks: a row whose prompt completes becomes DECODE with logit row B + cu_seqlens[b + 1] - 1 and start_pos = len; DECODE rows use
      logit row b; every other row gets logit row b and finished = 1 (the commit skips it); completing and decoding rows get finished = 0.
+Here len is the row's target, which admission sets to the prompt length.  schedule states these rules once for all three schedules: the
+page steps of tests/kv_pool_oracle.py and tests/prefix_cache_oracle.py are hooks that do nothing for rows that own their pages.
 """
 from __future__ import annotations
 
@@ -72,6 +74,7 @@ class InflightOracle:
         self.stop = [(-1,) * MAX_STOPS for _ in range(B)]
         self.budget = [self.max_tokens] * B
         self.start_pos = [0] * B
+        self.target = [0] * B  # the prompt tokens a PREFILL row caches: its prompt, or its history when a pool preempted it
         self.tokens_in = [0] * B
         self.ring: List[int] = []  # retired request ids, in retire order
         self.outputs: dict = {}    # request id -> (tokens, reason)
@@ -86,6 +89,7 @@ class InflightOracle:
 
     def schedule(self, chunk_budget: int) -> Plan:
         B, C = self.batch, self.chunk
+        self._register()
         # 1. retire
         for b in range(B):
             if self.phase[b] == DECODE and self.finished[b]:
@@ -102,6 +106,7 @@ class InflightOracle:
                 self.ring.append(r)
                 self.retired += 1
                 self.phase[b], self.row_req[b] = FREE, -1
+                self._release(b)
         # 2. admit
         if chunk_budget > 0:
             for b in range(B):
@@ -111,7 +116,7 @@ class InflightOracle:
                     q = self.requests[r]
                     n = len(q.prompt)
                     self.history[b] = list(q.prompt)
-                    self.prompt_lens[b] = self.seq_lens[b] = n
+                    self.prompt_lens[b] = self.seq_lens[b] = self.target[b] = n
                     self.eos[b] = q.eos
                     self.stop[b] = tuple(q.stop) + (-1,) * (MAX_STOPS - len(q.stop))
                     self.budget[b] = q.max_tokens
@@ -120,12 +125,15 @@ class InflightOracle:
                     self.admitted += 1
                     self.row_req[b] = r
                     self.phase[b] = PREFILL
+        order = sorted((b for b in range(B) if self.phase[b] != FREE), key=lambda b: self.adm[b])
+        self._grow(order)
+        self._start(order)
         # 3. plan
-        order = sorted((b for b in range(B) if self.phase[b] == PREFILL), key=lambda b: self.adm[b])
         take, used = [0] * B, 0
         for b in order:
-            take[b] = min(self.prompt_lens[b] - self.done[b], chunk_budget - used)
-            used += take[b]
+            if self.phase[b] == PREFILL and self._started(b):
+                take[b] = min(self.target[b] - self.done[b], chunk_budget - used)
+                used += take[b]
         cu = [0]
         for b in range(B):
             cu.append(cu[-1] + take[b])
@@ -141,9 +149,9 @@ class InflightOracle:
         for b in range(B):
             if self.phase[b] == PREFILL:
                 self.done[b] += take[b]
-                if self.done[b] == self.prompt_lens[b]:
+                if self.done[b] == self.target[b]:
                     self.phase[b] = DECODE
-                    self.start_pos[b] = self.prompt_lens[b]
+                    self.start_pos[b] = self.target[b]
                     plan.logit_rows[b] = B + cu[b + 1] - 1
                     self.finished[b] = 0
                 else:
@@ -152,7 +160,28 @@ class InflightOracle:
                 self.finished[b] = 0
             else:
                 self.finished[b] = 1
+        self._write_tables()
         return plan
+
+    # ---- the page steps, which rows that own their pages do not take (KvPoolOracle, PrefixCacheOracle) ----
+    def _register(self) -> None:
+        """Rule 0 of the prefix cache."""
+
+    def _release(self, b: int) -> None:
+        """A retired or preempted row's pages go back."""
+
+    def _grow(self, order: List[int]) -> None:
+        """Decode growth, over the live rows in admission order."""
+
+    def _start(self, order: List[int]) -> None:
+        """Starts, over the live rows in admission order."""
+
+    def _started(self, b: int) -> bool:
+        """Whether PREFILL row b takes prompt tokens in this call: every one does without a pool."""
+        return True
+
+    def _write_tables(self) -> None:
+        """The page-table entries of the pages taken in this call."""
 
     def commit(self, tokens) -> None:
         """spec_commit_stops of a plain step (one token per row): every unfinished row appends its token, and finishes on eos, a stop id or
@@ -175,7 +204,7 @@ class InflightOracle:
     def pending_prompt_tokens(self) -> int:
         """Prompt tokens still to prefill: the queued requests' and the prefilling rows' remaining ones."""
         queued = sum(len(self.requests[r].prompt) for r in range(self.head, self.tail))
-        return queued + sum(self.prompt_lens[b] - self.done[b] for b in range(self.batch) if self.phase[b] == PREFILL)
+        return queued + sum(self.target[b] - self.done[b] for b in range(self.batch) if self.phase[b] == PREFILL)
 
 
 def appended_positions(plan: Plan, row_req: List[int], batch: int, chunk: int) -> list:

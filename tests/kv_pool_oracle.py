@@ -15,12 +15,15 @@ Rules of one schedule(chunk_budget) call, in this order:
   5. Plan and tail masks as InflightOracle over the started PREFILL rows, with target in place of the prompt length.
   6. Table writes: entries [keep, count) of every row, where keep is the count before the call, or 0 if the row lost its pages in the call.
 It also counts events: decode victims, prefill victims, self-preemptions and calls whose starts were blocked.
+Rules 1, 2 and 5 are InflightOracle.schedule's; this class adds the page steps through its hooks, and PrefixCacheOracle changes how a page
+is taken and released and what a start reuses.
 """
 from __future__ import annotations
 
+from collections import Counter
 from typing import Dict, List, Tuple
 
-from tests.inflight_oracle import BUDGET, DECODE, EOS, FREE, MAX_STOPS, PREFILL, STOP, InflightOracle, Plan
+from tests.inflight_oracle import DECODE, FREE, PREFILL, InflightOracle
 
 PAGE = 64
 
@@ -39,121 +42,81 @@ class KvPoolOracle(InflightOracle):
         self.pages, self.blocks, self.layers = pages, blocks, layers
         self.free: List[int] = list(range(pages - 1, -1, -1))
         self.row_pages: List[List[int]] = [[] for _ in range(batch)]
-        self.target = [0] * batch
+        self.keep = [0] * batch  # leading page-list entries whose table entries are written
         self.peak = self.preemptions = self.starts = 0
         self.tables: Dict[Tuple[int, int, int, int], int] = {}  # (layer, row, kv, block) -> page
         self.events = {"decode_victim": 0, "prefill_victim": 0, "self_preemption": 0, "blocked_start": 0}
 
+    # ---- the pages a row can take ----
+    def _take(self) -> int:
+        return self.free.pop()
+
+    def _takeable(self, match=()) -> int:
+        """How many pages a take can reach, besides the pages of a start's match: the free stack."""
+        return len(self.free)
+
     def _pop(self, b: int) -> None:
-        self.row_pages[b].append(self.free.pop())
-        self.peak = max(self.peak, self.pages - len(self.free))
+        self.row_pages[b].append(self._take())
+        self.peak = max(self.peak, self.pages - self._takeable())
 
     def _release(self, b: int) -> None:
         self.free.extend(self.row_pages[b])
         self.row_pages[b] = []
+        self.keep[b] = 0
 
-    def schedule(self, chunk_budget: int) -> Plan:
-        B, C = self.batch, self.chunk
-        keep = [len(p) for p in self.row_pages]
-        # 1. retire
-        for b in range(B):
-            if self.phase[b] == DECODE and self.finished[b]:
-                r, p, L = self.row_req[b], self.prompt_lens[b], self.seq_lens[b]
-                last = self.history[b][L - 1] if L > 0 else -1
-                reason = BUDGET
-                if last >= 0 and last == self.eos[b]:
-                    reason = EOS
-                elif last >= 0 and last in self.stop[b]:
-                    reason = STOP
-                assert r not in self.outputs, f"request {r} retired twice"
-                self.outputs[r] = (list(self.history[b][p:L]), reason)
-                self.ring.append(r)
-                self.retired += 1
-                self.phase[b], self.row_req[b] = FREE, -1
-                self._release(b)
-                keep[b] = 0
-        # 2. admit
-        if chunk_budget > 0:
-            for b in range(B):
-                if self.phase[b] == FREE and self.head < self.tail:
-                    r = self.head
-                    self.head += 1
-                    q = self.requests[r]
-                    n = len(q.prompt)
-                    self.history[b] = list(q.prompt)
-                    self.prompt_lens[b] = self.seq_lens[b] = self.target[b] = n
-                    self.eos[b] = q.eos
-                    self.stop[b] = tuple(q.stop) + (-1,) * (MAX_STOPS - len(q.stop))
-                    self.budget[b] = q.max_tokens
-                    self.done[b] = 0
-                    self.adm[b] = self.admitted
-                    self.admitted += 1
-                    self.row_req[b] = r
-                    self.phase[b] = PREFILL
-        order = sorted((b for b in range(B) if self.phase[b] != FREE), key=lambda b: self.adm[b])
-        # 3. decode growth
+    def match(self, b: int) -> List[int]:
+        """The cached pages a start of row b reuses: none without the prefix cache."""
+        return []
+
+    def _share(self, b: int, match: List[int]) -> None:
+        """A start takes the pages of its match (the prefix cache's refs and LRU)."""
+
+    # ---- the page steps of InflightOracle.schedule ----
+    def _started(self, b: int) -> bool:
+        return bool(self.row_pages[b])
+
+    def _grow(self, order: List[int]) -> None:
         for i, b in enumerate(order):
             if self.phase[b] != DECODE or len(self.row_pages[b]) > (self.seq_lens[b] - 1) // PAGE:
                 continue
-            if not self.free:
+            victims = 0
+            while not self._takeable():
                 v = next((o for o in reversed(order[i + 1:]) if self.row_pages[o]), b)
                 self.events["self_preemption" if v == b else "decode_victim" if self.phase[v] == DECODE else "prefill_victim"] += 1
                 self._release(v)
-                keep[v] = 0
                 self.phase[v], self.done[v], self.target[v] = PREFILL, 0, self.seq_lens[v]
                 self.preemptions += 1
+                victims += 1
                 if v == b:
-                    continue
-            self._pop(b)
-        # 4. starts
+                    break
+            if victims > 1:  # only the prefix cache's victim can free no page: all of its pages may be shared
+                self.events["multi_victim"] += 1
+            if self.phase[b] == DECODE:
+                self._pop(b)
+
+    def _start(self, order: List[int]) -> None:
         for b in order:
             if self.phase[b] != PREFILL or self.row_pages[b]:
                 continue
+            m = self.match(b)
             need = -(-self.target[b] // PAGE)
-            if need > len(self.free):
+            if self._takeable(m) < need - len(m):
                 self.events["blocked_start"] += 1
                 break
-            for _ in range(need):
+            self._share(b, m)
+            self.row_pages[b] = list(m)
+            while len(self.row_pages[b]) < need:
                 self._pop(b)
+            self.done[b] = PAGE * len(m)
             self.starts += 1
-        # 5. plan
-        take, used = [0] * B, 0
-        for b in order:
-            if self.phase[b] == PREFILL and self.row_pages[b]:
-                take[b] = min(self.target[b] - self.done[b], chunk_budget - used)
-                used += take[b]
-        cu = [0]
-        for b in range(B):
-            cu.append(cu[-1] + take[b])
-        tokens = [self.tokens_in[b] if self.phase[b] == DECODE else 0 for b in range(B)] + [0] * C
-        pad = [C - 1 - t for t in range(C)]
-        for b in range(B):
-            for j in range(take[b]):
-                tokens[B + cu[b] + j] = self.history[b][self.done[b] + j]
-                pad[cu[b] + j] = b * C - cu[b]
-        plan = Plan(cu, take, [self.done[b] if self.phase[b] == PREFILL else 0 for b in range(B)],
-                    [self.seq_lens[b] if self.phase[b] == DECODE else 0 for b in range(B)], tokens, pad, list(range(B)), used)
-        for b in range(B):
-            if self.phase[b] == PREFILL:
-                self.done[b] += take[b]
-                if self.done[b] == self.target[b]:
-                    self.phase[b] = DECODE
-                    self.start_pos[b] = self.target[b]
-                    plan.logit_rows[b] = B + cu[b + 1] - 1
-                    self.finished[b] = 0
-                else:
-                    self.finished[b] = 1
-            elif self.phase[b] == DECODE:
-                self.finished[b] = 0
-            else:
-                self.finished[b] = 1
-        # 6. table writes
-        for b in range(B):
-            for j in range(keep[b], len(self.row_pages[b])):
+
+    def _write_tables(self) -> None:
+        for b in range(self.batch):
+            for j in range(self.keep[b], len(self.row_pages[b])):
                 for li in range(self.layers):
                     for kv in range(2):
                         self.tables[(li, b, kv, j)] = self.row_pages[b][j]
-        return plan
+            self.keep[b] = len(self.row_pages[b])
 
     @property
     def top(self) -> int:
@@ -162,11 +125,21 @@ class KvPoolOracle(InflightOracle):
     def counters(self) -> List[int]:
         return [self.top, self.peak, self.preemptions, self.starts]
 
+    def _evictable(self) -> List[int]:
+        """The pages no row holds that are not free: the prefix cache's LRU list."""
+        return []
+
+    def _shared(self, q: int) -> bool:
+        """Whether page q may be held by several rows: only a registered page of the prefix cache."""
+        return False
+
     def check_conservation(self) -> None:
-        """Every page is free or held by exactly one row, exactly once; FREE rows hold none; a PREFILL row holds none (waiting) or the
-        ceil(target / 64) pages of its start; a DECODE row holds at least the pages of the tokens it has cached."""
-        held = [p for b in range(self.batch) for p in self.row_pages[b]]
-        assert sorted(held + self.free) == list(range(self.pages)), "a page is lost or held twice"
+        """Every page is free, held or (with the prefix cache) evictable, in one place; only a shared page is held more than once; FREE rows
+        hold none; a PREFILL row holds none (waiting) or the ceil(target / 64) pages of its start; a DECODE row holds at least the pages of
+        the tokens it has cached."""
+        held = Counter(q for b in range(self.batch) for q in self.row_pages[b])
+        assert sorted(list(held) + self.free + self._evictable()) == list(range(self.pages)), "a page is lost or in two places"
+        assert all(n == 1 or self._shared(q) for q, n in held.items()), "a private page is held twice"
         for b in range(self.batch):
             n = len(self.row_pages[b])
             if self.phase[b] == FREE:
@@ -176,7 +149,3 @@ class KvPoolOracle(InflightOracle):
                 assert n or self.done[b] == 0, b
             else:
                 assert n >= -(-(self.seq_lens[b] - 1) // PAGE) and n <= self.blocks, b
-
-    def pending_prompt_tokens(self) -> int:
-        queued = sum(len(self.requests[r].prompt) for r in range(self.head, self.tail))
-        return queued + sum(self.target[b] - self.done[b] for b in range(self.batch) if self.phase[b] == PREFILL)

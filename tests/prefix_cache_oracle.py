@@ -23,7 +23,7 @@ from __future__ import annotations
 
 from typing import Dict, List, Tuple
 
-from tests.inflight_oracle import BUDGET, DECODE, EOS, FREE, MAX_STOPS, PREFILL, STOP, Plan
+from tests.inflight_oracle import PREFILL
 from tests.kv_pool_oracle import PAGE, KvPoolOracle
 
 PAGE_FREE, PAGE_PRIVATE, PAGE_REGISTERED = 0, 1, 2
@@ -64,7 +64,7 @@ class PrefixCacheOracle(KvPoolOracle):
         self.hit_pages = self.registrations = self.evictions = self.duplicates = 0
         self.events.update(multi_victim=0, hit_start=0)
 
-    # ---- page helpers ----
+    # ---- what the cache changes in KvPoolOracle's page steps ----
     def _key(self, b: int, j: int) -> Key:
         parent = self.row_pages[b][j - 1] if j else -1
         return (parent, self.epoch[parent] if j else 0, tuple(self.history[b][PAGE * j:PAGE * (j + 1)]))
@@ -80,21 +80,20 @@ class PrefixCacheOracle(KvPoolOracle):
         self.ref[q], self.state[q] = 1, PAGE_PRIVATE
         return q
 
-    def _pop(self, b: int) -> None:
-        self.row_pages[b].append(self._take())
-        self.peak = max(self.peak, self.held_pages())
+    def _takeable(self, match=()) -> int:
+        return len(self.free) + len(self.lru) - sum(self.ref[q] == 0 for q in match)
 
     def _release(self, b: int) -> None:
         pages, R = self.row_pages[b], self.reg[b]
         for q in pages[R:]:
-            self.free.append(q)
             self.ref[q], self.state[q] = 0, PAGE_FREE
         for q in reversed(pages[:R]):
             self.ref[q] -= 1
             if self.ref[q] == 0:
                 self.lru.append(q)
-        self.row_pages[b] = []
         self.reg[b] = self.halted[b] = 0
+        self.row_pages[b] = pages[R:]  # the private pages go onto the free stack
+        super()._release(b)
 
     def match(self, b: int) -> List[int]:
         """The longest chain of registered pages matching row b's history, at most (target - 1) // 64 pages."""
@@ -107,89 +106,23 @@ class PrefixCacheOracle(KvPoolOracle):
             parent, pe = q, self.epoch[q]
         return out
 
-    def held_pages(self) -> int:
-        return self.pages - len(self.free) - len(self.lru)
+    def _share(self, b: int, match: List[int]) -> None:
+        for q in match:
+            if self.ref[q] == 0:
+                self.lru.remove(q)
+            self.ref[q] += 1
+        self.reg[b] = len(match)
+        self.hit_pages += len(match)
+        self.events["hit_start"] += bool(match)
 
-    # ---- rules 1, 2, 5 and 6 of KvPoolOracle.schedule, unchanged ----
-    def _retire(self, b: int) -> None:
-        r, p, L = self.row_req[b], self.prompt_lens[b], self.seq_lens[b]
-        last = self.history[b][L - 1] if L > 0 else -1
-        reason = BUDGET
-        if last >= 0 and last == self.eos[b]:
-            reason = EOS
-        elif last >= 0 and last in self.stop[b]:
-            reason = STOP
-        assert r not in self.outputs, f"request {r} retired twice"
-        self.outputs[r] = (list(self.history[b][p:L]), reason)
-        self.ring.append(r)
-        self.retired += 1
-        self.phase[b], self.row_req[b] = FREE, -1
+    def _evictable(self) -> List[int]:
+        return self.lru
 
-    def _admit(self, chunk_budget: int) -> None:
-        if chunk_budget <= 0:
-            return
+    def _shared(self, q: int) -> bool:
+        return self.state[q] == PAGE_REGISTERED
+
+    def _register(self) -> None:
         for b in range(self.batch):
-            if self.phase[b] == FREE and self.head < self.tail:
-                r = self.head
-                self.head += 1
-                q = self.requests[r]
-                n = len(q.prompt)
-                self.history[b] = list(q.prompt)
-                self.prompt_lens[b] = self.seq_lens[b] = self.target[b] = n
-                self.eos[b] = q.eos
-                self.stop[b] = tuple(q.stop) + (-1,) * (MAX_STOPS - len(q.stop))
-                self.budget[b] = q.max_tokens
-                self.done[b] = 0
-                self.adm[b] = self.admitted
-                self.admitted += 1
-                self.row_req[b] = r
-                self.phase[b] = PREFILL
-
-    def _plan(self, chunk_budget: int, order: List[int], keep: List[int]) -> Plan:
-        B, C = self.batch, self.chunk
-        take, used = [0] * B, 0
-        for b in order:
-            if self.phase[b] == PREFILL and self.row_pages[b]:
-                take[b] = min(self.target[b] - self.done[b], chunk_budget - used)
-                used += take[b]
-        cu = [0]
-        for b in range(B):
-            cu.append(cu[-1] + take[b])
-        tokens = [self.tokens_in[b] if self.phase[b] == DECODE else 0 for b in range(B)] + [0] * C
-        pad = [C - 1 - t for t in range(C)]
-        for b in range(B):
-            for j in range(take[b]):
-                tokens[B + cu[b] + j] = self.history[b][self.done[b] + j]
-                pad[cu[b] + j] = b * C - cu[b]
-        plan = Plan(cu, take, [self.done[b] if self.phase[b] == PREFILL else 0 for b in range(B)],
-                    [self.seq_lens[b] if self.phase[b] == DECODE else 0 for b in range(B)], tokens, pad, list(range(B)), used)
-        for b in range(B):
-            if self.phase[b] == PREFILL:
-                self.done[b] += take[b]
-                if self.done[b] == self.target[b]:
-                    self.phase[b] = DECODE
-                    self.start_pos[b] = self.target[b]
-                    plan.logit_rows[b] = B + cu[b + 1] - 1
-                    self.finished[b] = 0
-                else:
-                    self.finished[b] = 1
-            elif self.phase[b] == DECODE:
-                self.finished[b] = 0
-            else:
-                self.finished[b] = 1
-        for b in range(B):
-            for j in range(keep[b], len(self.row_pages[b])):
-                for li in range(self.layers):
-                    for kv in range(2):
-                        self.tables[(li, b, kv, j)] = self.row_pages[b][j]
-        return plan
-
-    # ---- one schedule call ----
-    def schedule(self, chunk_budget: int) -> Plan:
-        B = self.batch
-        keep = [len(p) for p in self.row_pages]
-        # 0. register
-        for b in range(B):
             if not self.row_pages[b] or self.halted[b]:
                 continue
             cached = self.done[b] if self.phase[b] == PREFILL else self.seq_lens[b] - 1
@@ -206,57 +139,6 @@ class PrefixCacheOracle(KvPoolOracle):
                 self.index[k] = q
                 self.reg[b] = j + 1
                 self.registrations += 1
-        # 1. retire
-        for b in range(B):
-            if self.phase[b] == DECODE and self.finished[b]:
-                self._retire(b)
-                self._release(b)
-                keep[b] = 0
-        # 2. admit
-        self._admit(chunk_budget)
-        order = sorted((b for b in range(B) if self.phase[b] != FREE), key=lambda b: self.adm[b])
-        # 3. decode growth
-        for i, b in enumerate(order):
-            if self.phase[b] != DECODE or len(self.row_pages[b]) > (self.seq_lens[b] - 1) // PAGE:
-                continue
-            victims = 0
-            while not self.free and not self.lru:
-                v = next((o for o in reversed(order[i + 1:]) if self.row_pages[o]), b)
-                self.events["self_preemption" if v == b else "decode_victim" if self.phase[v] == DECODE else "prefill_victim"] += 1
-                self._release(v)
-                keep[v] = 0
-                self.phase[v], self.done[v], self.target[v] = PREFILL, 0, self.seq_lens[v]
-                self.preemptions += 1
-                victims += 1
-                if v == b:
-                    break
-            self.events["multi_victim"] += victims > 1
-            if self.phase[b] == DECODE:
-                self._pop(b)
-        # 4. starts
-        for b in order:
-            if self.phase[b] != PREFILL or self.row_pages[b]:
-                continue
-            m = self.match(b)
-            need = -(-self.target[b] // PAGE)
-            e = sum(self.ref[q] == 0 for q in m)
-            if len(self.free) + len(self.lru) - e < need - len(m):
-                self.events["blocked_start"] += 1
-                break
-            for q in m:
-                if self.ref[q] == 0:
-                    self.lru.remove(q)
-                self.ref[q] += 1
-            self.row_pages[b] = list(m)
-            while len(self.row_pages[b]) < need:
-                self._pop(b)
-            self.done[b] = PAGE * len(m)
-            self.reg[b] = len(m)
-            self.hit_pages += len(m)
-            self.events["hit_start"] += bool(m)
-            self.starts += 1
-        # 5. plan, 6. table writes
-        return self._plan(chunk_budget, order, keep)
 
     def cache_counters(self) -> List[int]:
         """The device's counters: LRU head, LRU tail, evictable, registered, hit pages, registrations, evictions, duplicates."""
@@ -295,18 +177,3 @@ class PrefixCacheOracle(KvPoolOracle):
                 assert self.state[q] == PAGE_REGISTERED and self.key[q] == self._key(b, j), (b, j)
             for q in pages[self.reg[b]:]:
                 assert self.state[q] == PAGE_PRIVATE, (b, q)
-
-    def check_conservation(self) -> None:
-        """Every page is free, evictable or held; a DECODE row holds at least the pages of its cached tokens; a started PREFILL row holds its
-        target's pages."""
-        held = {q for b in range(self.batch) for q in self.row_pages[b]}
-        assert sorted(list(held) + self.free + self.lru) == list(range(self.pages)), "a page is lost or in two places"
-        for b in range(self.batch):
-            n = len(self.row_pages[b])
-            if self.phase[b] == FREE:
-                assert n == 0, b
-            elif self.phase[b] == PREFILL:
-                assert n in (0, -(-self.target[b] // PAGE)), b
-                assert n or self.done[b] == 0, b
-            else:
-                assert n >= -(-(self.seq_lens[b] - 1) // PAGE) and n <= self.blocks, b

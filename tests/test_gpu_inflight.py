@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from tests.inflight_oracle import InflightOracle, Request
+from tests.kv_pool_oracle import min_pages
 
 pytestmark = pytest.mark.gpu
 
@@ -99,70 +100,141 @@ def _reference(dev, reqs, C, penalties=False, logprobs=0, model="tiny", layers=N
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------------------
-def test_schedule_matches_oracle(dev):
-    """The kernel against the oracle after every call: row state, plan, per-row vectors and outputs, with a plain commit of random tokens
-    (spec_commit_stops) in between; requests end by eos, stop ids and budget; queue slots are reused."""
-    from qserve_b200 import backend as ext
+class _Device:
+    """The schedule kernel on device buffers, driven like the oracle: submit(request), schedule(budget), commit(tokens).  P pages: the pool
+    schedule (qs_inflight_schedule_pool) over L layers; cache=True: with the prefix cache (qs_inflight_schedule_pool_cache)."""
 
-    Bn, Q, C, ctx, Tn, vocab = 6, 5, 20, 16, 6, 12
-    H = ctx + 1 + Tn
-    queue, rows, plan, out = ext.inflight_buffers(Bn, Q, C, ctx, Tn, dev)
-    full = lambda shape, v, dt: torch.full(shape, v, dtype=dt, device=dev)
-    history, plen, slen = full((Bn, H), -1, torch.int64), full((Bn,), 0, torch.int32), full((Bn,), 0, torch.int32)
-    temp, topk, topp = full((Bn,), 1.0, torch.float32), full((Bn,), 1, torch.int32), full((Bn,), 1.0, torch.float32)
-    rep, pres, freq = full((Bn,), 1.0, torch.float32), full((Bn,), 0.0, torch.float32), full((Bn,), 0.0, torch.float32)
-    eos, stop, budget = full((Bn,), -1, torch.int64), full((Bn, 8), -1, torch.int64), full((Bn,), Tn, torch.int32)
-    offs, fin, start, tin = full((Bn,), 7, torch.int64), full((Bn,), 0, torch.int32), full((Bn,), 0, torch.int32), full((Bn,), 0, torch.int64)
-    logprob, ctxl = full((Bn, H), float("nan"), torch.float32), full((Bn,), 0, torch.int32)
-    path, acc = full((Bn, 1), 0, torch.int32), full((Bn,), 1, torch.int32)
-    o = InflightOracle(Bn, Q, C, Tn)
-    rng = random.Random(7)
-    reqs = _script(40, ctx, Tn, vocab, seed=11)
-    nxt, reasons, prev = 0, set(), 0
-    for step in range(400):
-        while nxt < len(reqs) and rng.random() < 0.5 and (nxt - Q < 0 or (nxt - Q) in o.outputs):
-            r = reqs[nxt]
-            s = nxt % Q
-            queue.prompts[s].fill_(-1)
-            queue.prompts[s, : len(r["prompt"])] = torch.tensor(r["prompt"])
-            queue.lens[s], queue.max_tokens[s], queue.eos[s] = len(r["prompt"]), r["max_tokens"], r["eos"]
-            queue.stop[s] = torch.tensor(list(r["stop"]) + [-1] * (8 - len(r["stop"])))
-            o.submit(Request(r["prompt"], r["max_tokens"], r["eos"], tuple(r["stop"])))
-            nxt += 1
-            queue.counters[1] = nxt
-        cb = 0 if rng.random() < 0.15 else C
-        ext.inflight_schedule(queue, rows, history, plen, slen, temp, topk, topp, rep, pres, freq, eos, stop, budget, offs, fin, start, tin,
-                              logprob, plan, out, cb)
-        want = o.schedule(cb)
+    def __init__(self, dev, Bn, Q, Cn, ctx, Tn, P=None, L=1, cache=False):
+        from qserve_b200 import backend as ext
+
+        self.ext, self.B, self.Q, self.L = ext, Bn, Q, L
+        H = ctx + 1 + Tn
+        self.queue, self.rows, self.plan, self.out = ext.inflight_buffers(Bn, Q, Cn, ctx, Tn, dev)
+        full = lambda shape, v, dt: torch.full(shape, v, dtype=dt, device=dev)
+        self.history, self.plen, self.slen = full((Bn, H), -1, torch.int64), full((Bn,), 0, torch.int32), full((Bn,), 0, torch.int32)
+        self.samp = (full((Bn,), 1.0, torch.float32), full((Bn,), 1, torch.int32), full((Bn,), 1.0, torch.float32), full((Bn,), 1.0, torch.float32),
+                     full((Bn,), 0.0, torch.float32), full((Bn,), 0.0, torch.float32))
+        self.eos, self.stop, self.budget = full((Bn,), -1, torch.int64), full((Bn, 8), -1, torch.int64), full((Bn,), Tn, torch.int32)
+        self.offs, self.fin, self.start = full((Bn,), 0, torch.int64), full((Bn,), 0, torch.int32), full((Bn,), 0, torch.int32)
+        self.tin, self.logprob, self.ctxl = full((Bn,), 0, torch.int64), full((Bn, H), float("nan"), torch.float32), full((Bn,), 0, torch.int32)
+        self.path, self.acc = full((Bn, 1), 0, torch.int32), full((Bn,), 1, torch.int32)
+        self.pool = self.cache = None
+        if P is not None:
+            nb = min_pages(ctx, Tn) + 1
+            self.page_bytes = 4160
+            self.base = torch.tensor([[(2 * li + kv + 1) << 36 for kv in range(2)] for li in range(L)], dtype=torch.int64, device=dev)
+            self.pool = ext.kv_pool_buffers(torch.zeros((L, Bn, 2, nb), dtype=torch.int64, device=dev), self.base, P, self.page_bytes)
+            if cache:
+                self.cache = ext.prefix_cache_buffers(self.pool)
+        self.n = self.polled = 0
+
+    def submit(self, r):
+        s = self.n % self.Q
+        q = self.queue
+        q.prompts[s].fill_(-1)
+        q.prompts[s, : len(r.prompt)] = torch.tensor(r.prompt)
+        q.lens[s], q.max_tokens[s], q.eos[s] = len(r.prompt), r.max_tokens, r.eos
+        q.stop[s] = torch.tensor(list(r.stop) + [-1] * (8 - len(r.stop)))
+        self.n += 1
+        q.counters[1] = self.n
+        return self.n - 1
+
+    def schedule(self, budget):
+        self.ext.inflight_schedule(self.queue, self.rows, self.history, self.plen, self.slen, *self.samp, self.eos, self.stop, self.budget, self.offs,
+                                   self.fin, self.start, self.tin, self.logprob, self.plan, self.out, budget, pool=self.pool, cache=self.cache)
+
+    def commit(self, toks):
+        tok = torch.tensor(toks, dtype=torch.int64, device=self.fin.device)
+        self.ext.spec_commit(tok.view(-1, 1), self.path, self.acc, tok, self.history, self.slen, self.plen, self.budget, self.eos, self.fin, self.start,
+                             self.ctxl, self.tin, stop_ids=self.stop)
+
+    def check(self, o, want, step):
+        """After a schedule call: everything the oracle o of this mode keeps equals the device's, and the oracle's invariants hold."""
+        from tests.prefix_cache_oracle import key_hash
+
         got = lambda t: t.tolist()
-        assert got(rows.phase) == o.phase and got(rows.request) == o.row_req, step
-        assert [d for d, ph in zip(got(rows.done), o.phase) if ph] == [d for d, ph in zip(o.done, o.phase) if ph]
+        plan, Bn, Q = self.plan, self.B, self.Q
+        assert got(self.rows.phase) == o.phase and got(self.rows.request) == o.row_req, step
+        assert [x for x, ph in zip(got(self.rows.done), o.phase) if ph] == [x for x, ph in zip(o.done, o.phase) if ph], step
         assert got(plan.cu_seqlens) == want.cu_seqlens and got(plan.chunk_lens) == want.chunk_lens, step
         assert got(plan.prefix_lens) == want.prefix_lens and got(plan.context_lens) == want.context_lens, step
         assert got(plan.tokens) == want.tokens and got(plan.padding_offset) == want.padding_offset, step
-        assert got(plan.logit_rows) == want.logit_rows and got(fin) == o.finished, step
-        assert got(queue.counters)[:3] == [o.head, o.tail, o.retired]
+        assert got(plan.logit_rows) == want.logit_rows and got(self.fin) == o.finished, step
+        assert got(self.queue.counters)[:3] == [o.head, o.tail, o.retired], step
         for b in range(Bn):
             if o.row_req[b] >= 0:
-                assert int(plen[b]) == o.prompt_lens[b] and int(slen[b]) == o.seq_lens[b] and int(budget[b]) == o.budget[b]
-                assert int(eos[b]) == o.eos[b] and tuple(stop[b].tolist()) == o.stop[b]
-                assert history[b, : o.seq_lens[b]].tolist() == o.history[b][: o.seq_lens[b]]
-                if o.phase[b] == 2:
-                    assert int(start[b]) == o.start_pos[b]
-        ring = got(out.ids)
-        for i in range(prev, len(o.ring)):
+                assert int(self.plen[b]) == o.prompt_lens[b] and int(self.slen[b]) == o.seq_lens[b] and int(self.budget[b]) == o.budget[b], (step, b)
+                assert int(self.eos[b]) == o.eos[b] and tuple(self.stop[b].tolist()) == o.stop[b], (step, b)
+                assert self.history[b, : o.seq_lens[b]].tolist() == o.history[b][: o.seq_lens[b]], (step, b)
+                assert o.phase[b] != 2 or int(self.start[b]) == o.start_pos[b], (step, b)
+        ring = got(self.out.ids)
+        for i in range(self.polled, len(o.ring)):
             r = o.ring[i]
-            assert ring[i % Q] == r
+            assert ring[i % Q] == r, (step, i)
             toks, reason = o.outputs[r]
-            assert out.tokens[r % Q, : len(toks)].tolist() == toks and int(out.length[r % Q]) == len(toks) and int(out.reason[r % Q]) == reason
-            reasons.add(reason)
-        prev = len(o.ring)
-        tok = torch.tensor([rng.randrange(vocab) for _ in range(Bn)], dtype=torch.int64, device=dev)
-        ext.spec_commit(tok.view(Bn, 1), path, acc, tok, history, slen, plen, budget, eos, fin, start, ctxl, tin, stop_ids=stop)
-        o.commit(tok.tolist())
+            assert self.out.tokens[r % Q, : len(toks)].tolist() == toks and int(self.out.length[r % Q]) == len(toks), (step, r)
+            assert int(self.out.reason[r % Q]) == reason, (step, r)
+        self.polled = len(o.ring)
+        if self.pool is None:
+            return
+        pool = self.pool
+        assert got(pool.counters) == o.counters(), step
+        assert got(pool.free)[: o.top] == o.free, step
+        assert got(pool.count) == [len(p) for p in o.row_pages] and got(pool.target) == o.target, step
+        pages, tables, base = got(pool.pages), pool.tables.cpu(), got(self.base)
+        for b in range(Bn):
+            assert pages[b][: len(o.row_pages[b])] == o.row_pages[b], (step, b)
+            for li in range(self.L):
+                for kv in range(2):
+                    want_t = [base[li][kv] + p * self.page_bytes for p in o.row_pages[b]]
+                    assert tables[li, b, kv, : len(want_t)].tolist() == want_t, (step, b, li, kv)
+        o.check_conservation()
+        if self.cache is None:
+            return
+        cache = self.cache
+        assert got(cache.ref) == o.ref and got(cache.state) == o.state and got(cache.epoch) == o.epoch, step
+        assert got(cache.reg) == o.reg and got(cache.stop) == o.halted, step
+        lru, head, nxt = [], int(cache.counters[0]), got(cache.lru_next)
+        while head >= 0:
+            lru.append(head)
+            head = nxt[head]
+        assert got(cache.counters) == o.cache_counters() and lru == o.lru, step
+        index, hashes, S = got(cache.index), got(cache.hash), cache.index.numel()
+        assert sorted(x for x in index if x >= 0) == sorted(o.index.values()), step
+        for (parent, pe, toks), q in o.index.items():
+            h = key_hash(toks, parent, pe)
+            assert hashes[q] & 0xFFFFFFFF == h and got(cache.key_tokens[q]) == list(toks), (step, q)
+            i = h & (S - 1)
+            while index[i] != q:
+                assert index[i] >= 0, (step, q)
+                i = (i + 1) & (S - 1)
+        o.check_cache()
+
+
+def test_schedule_matches_oracle(dev):
+    """The kernel against the oracle after every call: row state, plan, per-row vectors and outputs, with a plain commit of random tokens
+    (spec_commit_stops) in between; requests end by eos, stop ids and budget; queue slots are reused."""
+    Bn, Q, C, ctx, Tn, vocab = 6, 5, 20, 16, 6, 12
+    o, d = InflightOracle(Bn, Q, C, Tn), _Device(dev, Bn, Q, C, ctx, Tn)
+    rng = random.Random(7)
+    reqs = _script(40, ctx, Tn, vocab, seed=11)
+    nxt = 0
+    for step in range(400):
+        while nxt < len(reqs) and rng.random() < 0.5 and (nxt - Q < 0 or (nxt - Q) in o.outputs):
+            r = reqs[nxt]
+            req = Request(r["prompt"], r["max_tokens"], r["eos"], tuple(r["stop"]))
+            d.submit(req)
+            o.submit(req)
+            nxt += 1
+        cb = 0 if rng.random() < 0.15 else C
+        d.schedule(cb)
+        d.check(o, o.schedule(cb), step)
+        tok = [rng.randrange(vocab) for _ in range(Bn)]
+        d.commit(tok)
+        o.commit(tok)
         if len(o.outputs) == len(reqs):
             break
-    assert len(o.outputs) == len(reqs) and reasons == {1, 2, 3}
+    assert len(o.outputs) == len(reqs) and {reason for _, reason in o.outputs.values()} == {1, 2, 3}
 
 
 @pytest.mark.parametrize("int4", [True, False])

@@ -11,7 +11,7 @@ import pytest
 import torch
 
 from tests.kv_pool_oracle import KvPoolOracle, min_pages
-from tests.test_gpu_inflight import _reason, _runner, _script, _submit
+from tests.test_gpu_inflight import _Device, _reason, _runner, _script, _submit
 from tests.test_oracle_kv_pool import _drive
 
 pytestmark = pytest.mark.gpu
@@ -21,82 +21,12 @@ C = B * (CTX + T)  # every prefill, recomputations included, is carried in one p
 BLOCKS = (max(CTX + T + 1, CTX + T - 1 + C) + 63) // 64
 
 
-class _Device:
-    """qs_inflight_schedule_pool on device buffers, driven like the oracle: submit(request), schedule(budget), commit(tokens)."""
-
-    def __init__(self, dev, Bn, Q, Cn, ctx, Tn, P, L):
-        from qserve_b200 import backend as ext
-
-        self.ext, self.B, self.Q, self.L = ext, Bn, Q, L
-        H = ctx + 1 + Tn
-        self.queue, self.rows, self.plan, self.out = ext.inflight_buffers(Bn, Q, Cn, ctx, Tn, dev)
-        full = lambda shape, v, dt: torch.full(shape, v, dtype=dt, device=dev)
-        self.history, self.plen, self.slen = full((Bn, H), -1, torch.int64), full((Bn,), 0, torch.int32), full((Bn,), 0, torch.int32)
-        self.samp = (full((Bn,), 1.0, torch.float32), full((Bn,), 1, torch.int32), full((Bn,), 1.0, torch.float32), full((Bn,), 1.0, torch.float32),
-                     full((Bn,), 0.0, torch.float32), full((Bn,), 0.0, torch.float32))
-        self.eos, self.stop, self.budget = full((Bn,), -1, torch.int64), full((Bn, 8), -1, torch.int64), full((Bn,), Tn, torch.int32)
-        self.offs, self.fin, self.start = full((Bn,), 0, torch.int64), full((Bn,), 0, torch.int32), full((Bn,), 0, torch.int32)
-        self.tin, self.logprob, self.ctxl = full((Bn,), 0, torch.int64), full((Bn, H), float("nan"), torch.float32), full((Bn,), 0, torch.int32)
-        self.path, self.acc = full((Bn, 1), 0, torch.int32), full((Bn,), 1, torch.int32)
-        nb = min_pages(ctx, Tn) + 1
-        self.page_bytes = 4160
-        self.base = torch.tensor([[(2 * li + kv + 1) << 36 for kv in range(2)] for li in range(L)], dtype=torch.int64, device=dev)
-        self.pool = ext.kv_pool_buffers(torch.zeros((L, Bn, 2, nb), dtype=torch.int64, device=dev), self.base, P, self.page_bytes)
-        self.n = 0
-
-    def submit(self, r):
-        s = self.n % self.Q
-        q = self.queue
-        q.prompts[s].fill_(-1)
-        q.prompts[s, : len(r.prompt)] = torch.tensor(r.prompt)
-        q.lens[s], q.max_tokens[s], q.eos[s] = len(r.prompt), r.max_tokens, r.eos
-        q.stop[s] = torch.tensor(list(r.stop) + [-1] * (8 - len(r.stop)))
-        self.n += 1
-        q.counters[1] = self.n
-
-    def schedule(self, budget):
-        self.ext.inflight_schedule(self.queue, self.rows, self.history, self.plen, self.slen, *self.samp, self.eos, self.stop, self.budget, self.offs,
-                                   self.fin, self.start, self.tin, self.logprob, self.plan, self.out, budget, pool=self.pool)
-
-    def commit(self, toks):
-        tok = torch.tensor(toks, dtype=torch.int64, device=self.fin.device)
-        self.ext.spec_commit(tok.view(-1, 1), self.path, self.acc, tok, self.history, self.slen, self.plen, self.budget, self.eos, self.fin, self.start,
-                             self.ctxl, self.tin, stop_ids=self.stop)
-
-
 def test_schedule_matches_oracle(dev):
     """The kernel against the oracle after every call, with random commits in between, at a pool small enough for every event kind."""
     Bn, Q, Cn, ctx, Tn, P, L = 6, 7, 40, 150, 60, 7, 3
     o = KvPoolOracle(Bn, Q, Cn, Tn, ctx, P, min_pages(ctx, Tn) + 1, layers=L)
     d = _Device(dev, Bn, Q, Cn, ctx, Tn, P, L)
-
-    def check(step, plans):
-        want, plan, pool = plans[0], d.plan, d.pool
-        got = lambda t: t.tolist()
-        assert got(d.rows.phase) == o.phase and got(d.rows.request) == o.row_req, step
-        assert [x for x, ph in zip(got(d.rows.done), o.phase) if ph] == [x for x, ph in zip(o.done, o.phase) if ph], step
-        assert got(plan.cu_seqlens) == want.cu_seqlens and got(plan.chunk_lens) == want.chunk_lens, step
-        assert got(plan.prefix_lens) == want.prefix_lens and got(plan.context_lens) == want.context_lens, step
-        assert got(plan.tokens) == want.tokens and got(plan.padding_offset) == want.padding_offset, step
-        assert got(plan.logit_rows) == want.logit_rows and got(d.fin) == o.finished, step
-        assert got(d.queue.counters)[:3] == [o.head, o.tail, o.retired], step
-        assert got(pool.counters) == o.counters(), step
-        assert got(pool.free)[: o.top] == o.free, step
-        assert got(pool.count) == [len(p) for p in o.row_pages] and got(pool.target) == o.target, step
-        pages, tables, base = got(pool.pages), pool.tables.cpu(), got(d.base)
-        for b in range(Bn):
-            assert pages[b][: len(o.row_pages[b])] == o.row_pages[b], (step, b)
-            for li in range(L):
-                for kv in range(2):
-                    want_t = [base[li][kv] + p * d.page_bytes for p in o.row_pages[b]]
-                    assert tables[li, b, kv, : len(want_t)].tolist() == want_t, (step, b, li, kv)
-        for b in range(Bn):
-            if o.row_req[b] >= 0:
-                assert d.history[b, : o.seq_lens[b]].tolist() == o.history[b][: o.seq_lens[b]], (step, b)
-                assert int(d.slen[b]) == o.seq_lens[b] and (o.phase[b] != 2 or int(d.start[b]) == o.start_pos[b]), (step, b)
-        o.check_conservation()
-
-    _drive([o, d], 31, Bn, Q, Cn, ctx, Tn, 40, vocab=400, check=check)
+    _drive([o, d], 31, Bn, Q, Cn, ctx, Tn, 40, vocab=400, check=lambda step, plans: d.check(o, plans[0], step))
     assert all(v > 0 for v in o.events.values()), o.events
     for r, (toks, reason) in o.outputs.items():
         s = r % Q

@@ -15,79 +15,20 @@ import pytest
 import torch
 
 from tests.kv_pool_oracle import min_pages
-from tests.prefix_cache_oracle import PAGE_REGISTERED, PrefixCacheOracle, key_hash
-from tests.test_gpu_inflight import _reason, _runner, _submit
-from tests.test_gpu_kv_pool import _Device, _fill_random, _reqs, _serve_watch
+from tests.prefix_cache_oracle import PAGE_REGISTERED, PrefixCacheOracle
+from tests.test_gpu_inflight import _Device, _reason, _runner, _submit
+from tests.test_gpu_kv_pool import _fill_random, _reqs, _serve_watch
 from tests.test_oracle_prefix_cache import drive_shared
 
 pytestmark = pytest.mark.gpu
-
-
-class _CacheDevice(_Device):
-    """qs_inflight_schedule_pool_cache on device buffers, driven like the oracle."""
-
-    def __init__(self, *args):
-        super().__init__(*args)
-        self.cache = self.ext.prefix_cache_buffers(self.pool)
-
-    def submit(self, r):
-        super().submit(r)
-        return self.n - 1
-
-    def schedule(self, budget):
-        self.ext.inflight_schedule(self.queue, self.rows, self.history, self.plen, self.slen, *self.samp, self.eos, self.stop, self.budget, self.offs,
-                                   self.fin, self.start, self.tin, self.logprob, self.plan, self.out, budget, pool=self.pool, cache=self.cache)
-
-
-def _lru(cache):
-    head, nxt, out = int(cache.counters[0]), cache.lru_next.tolist(), []
-    while head >= 0:
-        out.append(head)
-        head = nxt[head]
-    return out
 
 
 def test_schedule_matches_oracle(dev):
     Bn, Q, Cn, ctx, Tn, L = 5, 7, 64, 200, 40, 2
     P = min_pages(ctx, Tn) * 2
     o = PrefixCacheOracle(Bn, Q, Cn, Tn, ctx, P, min_pages(ctx, Tn) + 1, layers=L)
-    d = _CacheDevice(dev, Bn, Q, Cn, ctx, Tn, P, L)
-
-    def check(step, plans):
-        want, plan, pool, cache = plans[0], d.plan, d.pool, d.cache
-        got = lambda t: t.tolist()
-        assert got(d.rows.phase) == o.phase and got(d.rows.request) == o.row_req, step
-        assert [x for x, ph in zip(got(d.rows.done), o.phase) if ph] == [x for x, ph in zip(o.done, o.phase) if ph], step
-        assert got(plan.cu_seqlens) == want.cu_seqlens and got(plan.chunk_lens) == want.chunk_lens, step
-        assert got(plan.prefix_lens) == want.prefix_lens and got(plan.context_lens) == want.context_lens, step
-        assert got(plan.tokens) == want.tokens and got(plan.padding_offset) == want.padding_offset, step
-        assert got(plan.logit_rows) == want.logit_rows and got(d.fin) == o.finished, step
-        assert got(pool.counters) == o.counters(), step
-        assert got(pool.free)[: o.top] == o.free, step
-        assert got(pool.count) == [len(p) for p in o.row_pages] and got(pool.target) == o.target, step
-        pages, tables, base = got(pool.pages), pool.tables.cpu(), got(d.base)
-        for b in range(Bn):
-            assert pages[b][: len(o.row_pages[b])] == o.row_pages[b], (step, b)
-            for li in range(L):
-                for kv in range(2):
-                    want_t = [base[li][kv] + p * d.page_bytes for p in o.row_pages[b]]
-                    assert tables[li, b, kv, : len(want_t)].tolist() == want_t, (step, b, li, kv)
-        assert got(cache.ref) == o.ref and got(cache.state) == o.state and got(cache.epoch) == o.epoch, step
-        assert got(cache.reg) == o.reg and got(cache.stop) == o.halted, step
-        assert got(cache.counters) == o.cache_counters() and _lru(cache) == o.lru, step
-        index, hashes, S = got(cache.index), got(cache.hash), cache.index.numel()
-        assert sorted(x for x in index if x >= 0) == sorted(o.index.values()), step
-        for (parent, pe, toks), q in o.index.items():
-            h = key_hash(toks, parent, pe)
-            assert hashes[q] & 0xFFFFFFFF == h and got(cache.key_tokens[q]) == list(toks), (step, q)
-            i = h & (S - 1)
-            while index[i] != q:
-                assert index[i] >= 0, (step, q)
-                i = (i + 1) & (S - 1)
-        o.check_cache()
-        o.check_conservation()
-
-    drive_shared([o, d], 11, Bn, Q, Cn, ctx, Tn, 30, vocab=50, check=check)
+    d = _Device(dev, Bn, Q, Cn, ctx, Tn, P, L, cache=True)
+    drive_shared([o, d], 11, Bn, Q, Cn, ctx, Tn, 30, vocab=50, check=lambda step, plans: d.check(o, plans[0], step))
     assert o.hit_pages > 0 and o.evictions > 0 and o.duplicates > 0 and o.preemptions > 0, o.cache_counters()
     assert any(o.ref[q] == 0 for q in o.lru)
 

@@ -9,7 +9,8 @@ import pytest
 from tests.inflight_oracle import DECODE, FREE, PREFILL, InflightOracle, Request, appended_positions
 
 
-def _run_script(seed: int, B: int, Q: int, C: int, ctx: int, T: int, n_req: int, vocab: int = 50):
+def _run_script(seed: int, B: int, Q: int, C: int, ctx: int, T: int, n_req: int, vocab: int = 50, check=None):
+    """One seeded script; check(oracle, plan) runs after every schedule call.  Returns the number of steps."""
     rng = random.Random(seed)
     o = InflightOracle(B, Q, C, T)
     arrivals = sorted(rng.randrange(0, 3 * n_req) for _ in range(n_req)) if rng.random() < 0.7 else [0] * n_req
@@ -27,6 +28,8 @@ def _run_script(seed: int, B: int, Q: int, C: int, ctx: int, T: int, n_req: int,
         budget = 0 if rng.random() < 0.1 else C
         head0, phase0, req0 = o.head, list(o.phase), list(o.row_req)
         plan = o.schedule(budget)
+        if check:
+            check(o, plan)
         if budget == 0:
             assert o.head == head0, "a budget-0 call admitted a request"
         # first-come-first-served: admitted in id order, into the lowest free rows
@@ -74,13 +77,18 @@ def _run_script(seed: int, B: int, Q: int, C: int, ctx: int, T: int, n_req: int,
     return step
 
 
-@pytest.mark.parametrize("seed", range(12))
-def test_random_scripts(seed):
+def _config(seed):
+    """(B, Q, C, ctx, T, n_req) of the random script `seed`."""
     rng = random.Random(1000 + seed)
     B, ctx = rng.choice([1, 2, 3, 5, 8]), rng.choice([1, 4, 17, 64])
     C = rng.choice([1, 2, 7, ctx, B * ctx, B * ctx + 5])
     Q = rng.choice([1, B, 2 * B + 1])
-    _run_script(seed, B, Q, C, ctx, rng.choice([1, 3, 9]), rng.randint(1, 30))
+    return B, Q, C, ctx, rng.choice([1, 3, 9]), rng.randint(1, 30)
+
+
+@pytest.mark.parametrize("seed", range(12))
+def test_random_scripts(seed):
+    _run_script(seed, *_config(seed))
 
 
 def test_budget_zero_admits_nothing_and_retires():
